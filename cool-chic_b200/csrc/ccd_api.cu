@@ -12,7 +12,6 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -416,7 +415,6 @@ struct CcdContext {
     uint64_t last_upload_bytes = 0;
     uint32_t prod_mask = 0x3777u;  // warps 3, 7, 11 stay idle: the coder warp (15) owns its scheduler
     int n_sm = 132;
-    int narrow_cta = 1;  // (CCD_NARROW_CTA=0 in the environment: always 16-warp CTAs)
     int fused_synthesis = 1;       // 0: layer-by-layer kernels (ccd_debug_set_fused_synthesis, tests compare both)
     // entropy launches of different ARM architectures (e.g. intra / residue / motion streams of a GOP) run
     // side by side on these streams: each launch only fills as many SMs as it has streams
@@ -916,8 +914,6 @@ int ccd_create(int device_ordinal, CcdContext **out) {
     {
         int nsm = 0;
         if (cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device_ordinal) == cudaSuccess && nsm > 0) c->n_sm = nsm;
-        const char *env = getenv("CCD_NARROW_CTA");
-        if (env && env[0] == '0') c->narrow_cta = 0;
     }
     int rc = CCD_OK;
     do {
@@ -1259,7 +1255,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
             }
             const PreparedJob &J0 = P[(size_t)order[(size_t)t]];
             // more streams than SMs: 8-warp CTAs, two per SM (registers: 2 x 256 x 128; shared memory permitting)
-            const bool narrow = mode == 0 && ctx->narrow_cta != 0 && (u - t) > ctx->n_sm &&
+            const bool narrow = mode == 0 && (u - t) > ctx->n_sm &&
                                 2 * (smem + 1024) <= (size_t)227 * 1024;
             EntLaunchCfg cfg{J0.d->n_ctx, J0.d->flag_ifce ? J0.d->n_ifce_out : 0, J0.fast, smem,
                              narrow ? CCD_ENT_THREADS_NARROW : CCD_ENT_THREADS};

@@ -30,7 +30,7 @@ EXPORTS = [
     "ccd_synthesize", "ccd_encode_latents", "ccd_finish_frame", "ccd_inter_predict", "ccd_reconstruct_frame",
     "ccd_pack_frame",
     "ccd_pack_samples",
-    "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_debug_set_fused_synthesis", "ccd_last_timing",
+    "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
 ]
 
 
@@ -117,8 +117,6 @@ def load_library():
         L.ccd_debug_launch_count.argtypes = []
         L.ccd_debug_set_producer_mask.restype = ci
         L.ccd_debug_set_producer_mask.argtypes = [vp, ctypes.c_uint32]
-        L.ccd_debug_set_fused_synthesis.restype = ci
-        L.ccd_debug_set_fused_synthesis.argtypes = [vp, ci]
         L.ccd_last_timing.restype = ci
         L.ccd_last_timing.argtypes = [vp, vp]
         if L.ccd_sizeof_desc() != ctypes.sizeof(CcdCoolChicDesc):
@@ -439,10 +437,6 @@ class Context:
 
     def launch_count(self) -> int:
         return int(self._lib.ccd_debug_launch_count())
-
-    def set_fused_synthesis(self, on: bool) -> None:
-        """Debug switch: fused synthesis kernel (default) vs one kernel per layer; results are bit-identical."""
-        _check(self._lib.ccd_debug_set_fused_synthesis(self._h, int(bool(on))))
 
     def last_status(self):
         st = (ctypes.c_int32 * 16)()

@@ -387,11 +387,12 @@ struct PreparedJob {
     int64_t lat_off_by_grid[CCD_MAX_GRIDS];
     bool pad_lat = false;   // latents owned by the library: every grid starts on a 16-byte boundary (TMA source)
     int64_t lat_bytes = 0;  // bytes of the latent buffer in that layout
-    // batched float tail (run_tail_batched)
+    int nl = 0, gl[CCD_MAX_GRIDS];  // latent grids (not hyper), finest first
+    // float tail (plan_tail)
     bool tail = false;      // goes through the batched path
-    int tail_nl = 0, tail_gl[CCD_MAX_GRIDS];
     int tail_cinp = 0, tail_C = 0;
-    size_t off_tailP = 0, off_tailQ = 0, off_tailRaw = 0, off_rawtmp = 0;  // inside the synthesis scratch
+    size_t off_tailP = 0, off_tailQ = 0, off_tailRaw = 0;  // inside the batched path's scratch
+    size_t off_rawtmp = 0;  // inside the per-stream path's scratch
     // device offsets inside the upload arena
     size_t off_words = 0, off_blob = 0, off_status = 0, off_syn = 0, off_lat = 0;
     std::vector<float> syn_f;  // dequantised synthesis weights, packed
@@ -415,7 +416,6 @@ struct CcdContext {
     uint64_t last_upload_bytes = 0;
     uint32_t prod_mask = 0x3777u;  // warps 3, 7, 11 stay idle: the coder warp (15) owns its scheduler
     int n_sm = 132;
-    int fused_synthesis = 1;       // 0: layer-by-layer kernels (ccd_debug_set_fused_synthesis, tests compare both)
     // entropy launches of different ARM architectures (e.g. intra / residue / motion streams of a GOP) run
     // side by side on these streams: each launch only fills as many SMs as it has streams
     cudaStream_t aux[3] = {nullptr, nullptr, nullptr};
@@ -487,6 +487,9 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
     }
     P.n_sym = nsym;
     P.lat_bytes = off;
+    P.nl = 0;
+    for (int g = 0; g < d->n_grids; g++)
+        if (!d->grid_is_hyper[g]) P.gl[P.nl++] = g;
     if (off >= ((int64_t)1 << 31)) return fail(CCD_ERR_UNSUPPORTED, "more than 2^31 latent symbols");
     // ---- ARM + IFCE integers
     const int dim = L.dim;
@@ -610,10 +613,10 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
     return CCD_OK;
 }
 
-// Device scratch of the float tail of one job.
+// Device scratch of the float tail of one job on the per-stream path.
 struct SynScratch {
     size_t off_nxt = 0, off_a = 0, off_b = 0, off_stab = 0, off_noise_raw = 0, off_noise_a = 0, off_noise_b = 0, total = 0;
-    std::vector<int> fused;  // layer l is evaluated together with l + 1 (two 1x1 layers)
+    std::vector<int> pw2;  // layer l is evaluated together with l + 1 by k_syn_pw2 (two 1x1 layers)
 };
 SynScratch syn_scratch_plan(const CcdCoolChicDesc *d) {
     SynScratch S;
@@ -623,7 +626,7 @@ SynScratch syn_scratch_plan(const CcdCoolChicDesc *d) {
             if (g0 < 0) g0 = g;
             nl++;
         }
-    S.fused.assign((size_t)std::max(d->n_syn_layers, 1), 0);
+    S.pw2.assign((size_t)std::max(d->n_syn_layers, 1), 0);
     if (g0 < 0 || d->n_syn_layers < 1) return S;
     const size_t plane = (size_t)d->grid_h[g0] * d->grid_w[g0];
     const int C = d->syn_out[d->n_syn_layers - 1];
@@ -633,7 +636,7 @@ SynScratch syn_scratch_plan(const CcdCoolChicDesc *d) {
         const bool can = l + 1 < d->n_syn_layers && d->syn_k[l] == 1 && d->syn_k[l + 1] == 1 && !d->syn_res[l] &&
                          !d->syn_res[l + 1] && in_ft <= 16 && d->syn_out[l + 1] <= 8;
         if (can) {
-            S.fused[(size_t)l] = 1;
+            S.pw2[(size_t)l] = 1;
             maxc = std::max(maxc, d->syn_out[l + 1]);
             in_ft = d->syn_out[l + 1];
             l++;
@@ -665,32 +668,73 @@ void expand_sym(const float *par, int k, float *full) {
     for (int i = 0; i < k - np; i++) full[np + i] = par[np - 1 - (k % 2) - i];
 }
 
-// Upsampling cascade + synthesis + final resize for one job (all kernels on `st`).
-int run_synthesis(CcdContext *ctx, const PreparedJob &P, const int8_t *d_lat, const float *d_synw, float *d_out,
-                  unsigned char *scratch, size_t scratch_bytes, cudaStream_t st) {
+// Full 1-D taps of cascade level idx (level 0 upsamples the coarsest grid): quantised parameters -> dequantised ->
+// expand_sym
+void level_taps(const PreparedJob &P, int idx, float full_t[16], float full_c[16]) {
     const CcdCoolChicDesc *d = P.d;
     const NNLayout &L = P.L;
+    const float qs_uw = ldexpf(1.0f, d->qshift[4]);
+    const int kid = idx % d->n_ups;
+    float par_t[8], par_c[8];
+    for (int i = 0; i < L.kt_par; i++) par_t[i] = (float)P.nn[(size_t)(L.ups_tw + (int64_t)kid * L.kt_par + i)] * qs_uw;
+    for (int i = 0; i < L.kc_par; i++) par_c[i] = (float)P.nn[(size_t)(L.ups_cw + (int64_t)kid * L.kc_par + i)] * qs_uw;
+    expand_sym(par_t, d->ups_k, full_t);
+    expand_sym(par_c, d->ups_pre_k, full_c);
+}
+
+// The synthesis of a job as layer descriptors with their weights at d_synw (null when only the shapes are needed)
+struct SynNet {
+    SynLayerDev layers[CCD_MAX_SYN], stab, ot;
+};
+SynNet syn_net(const PreparedJob &P, const float *d_synw) {
+    const CcdCoolChicDesc *d = P.d;
+    const int C = P.L.syn_c;
+    auto at = [&](size_t off) { return d_synw ? d_synw + off : nullptr; };
+    SynNet N;
+    int in_ft = d->syn_in;
+    for (int l = 0; l < d->n_syn_layers; l++) {
+        N.layers[l] = SynLayerDev{in_ft, d->syn_out[l], d->syn_k[l], d->syn_res[l], d->syn_relu[l], at(P.syn_off_w[l]),
+                                  at(P.syn_off_b[l])};
+        in_ft = d->syn_out[l];
+    }
+    N.stab = SynLayerDev{P.L.syn_stab_in, C, 1, 0, 0, at(P.syn_off_st_w), at(P.syn_off_st_b)};
+    N.ot = SynLayerDev{C, C, 1, 0, 0, at(P.syn_off_ot_w), at(P.syn_off_ot_b)};
+    return N;
+}
+
+// final F.interpolate of an output computed at h0 x w0, smaller than the image (component/coolchic.py:187-192)
+int resize_output(const CcdCoolChicDesc *d, const float *src, int C, int h0, int w0, float *dst, cudaStream_t st) {
+    int rc;
+    if (d->final_ups == 0)
+        rc = ccd_resize_nearest(src, C, h0, w0, dst, d->img_h, d->img_w, st);
+    else
+        rc = ccd_resize_torch(src, C, h0, w0, dst, d->img_h, d->img_w, d->final_ups == 1 ? 1 : 2,
+                              (float)h0 / (float)d->img_h, (float)w0 / (float)d->img_w, st);
+    return rc ? fail(CCD_ERR_CUDA, "resize launch") : CCD_OK;
+}
+
+// Upsampling cascade + synthesis + final resize for one job on the per-stream path (all kernels on `st`).
+int run_synthesis(const PreparedJob &P, const int8_t *d_lat, const float *d_synw, float *d_out, unsigned char *scratch,
+                  size_t scratch_bytes, cudaStream_t st) {
+    const CcdCoolChicDesc *d = P.d;
     const int cr = d->common_randomness != 0;
-    int gl[CCD_MAX_GRIDS], nl = 0;
-    for (int g = 0; g < d->n_grids; g++)
-        if (!d->grid_is_hyper[g]) gl[nl++] = g;
+    const int nl = P.nl;
+    const int *gl = P.gl;
     if (nl * (cr ? 2 : 1) != d->syn_in || nl < 1)
         return fail(CCD_ERR_ARG, "synthesis input width %d does not match %d latent grids", d->syn_in, nl);
     const int h0 = d->grid_h[gl[0]], w0 = d->grid_w[gl[0]];
     if (cr && (h0 != d->img_h || w0 != d->img_w || nl != d->latent_res_hi - d->latent_res_lo + 1))
         return fail(CCD_ERR_ARG, "common randomness needs a full-resolution finest latent grid");
     const size_t plane = (size_t)h0 * w0;
-    const int C = L.syn_c;
+    const int C = P.L.syn_c;
     const SynScratch SS = syn_scratch_plan(d);
     if (SS.total > scratch_bytes) return fail(CCD_ERR_NOMEM, "internal: scratch too small (%zu > %zu)", SS.total, scratch_bytes);
-    const std::vector<int> &fused = SS.fused;
     float *cur = reinterpret_cast<float *>(scratch);
     float *nxt = reinterpret_cast<float *>(scratch + SS.off_nxt);
     float *bufa = reinterpret_cast<float *>(scratch + SS.off_a);
     float *bufb = reinterpret_cast<float *>(scratch + SS.off_b);
     float *stab = reinterpret_cast<float *>(scratch + SS.off_stab);
 
-    const float qs_uw = ldexpf(1.0f, d->qshift[4]);
     int gc = gl[nl - 1];
     int ch = d->grid_h[gc], cw = d->grid_w[gc], cc = 1;
     int rc;
@@ -699,13 +743,9 @@ int run_synthesis(CcdContext *ctx, const PreparedJob &P, const int8_t *d_lat, co
         const int gt = gl[nl - 2 - idx];
         const int th = d->grid_h[gt], tw = d->grid_w[gt];
         if (th > 2 * ch || tw > 2 * cw) return fail(CCD_ERR_ARG, "grid %d more than twice the size of its parent", gt);
-        float par_t[8], par_c[8], full_t[16], full_c[16];
-        const int kid = idx % d->n_ups;
-        for (int i = 0; i < L.kt_par; i++) par_t[i] = (float)P.nn[(size_t)(L.ups_tw + (int64_t)kid * L.kt_par + i)] * qs_uw;
-        for (int i = 0; i < L.kc_par; i++) par_c[i] = (float)P.nn[(size_t)(L.ups_cw + (int64_t)kid * L.kc_par + i)] * qs_uw;
-        expand_sym(par_t, d->ups_k, full_t);
-        expand_sym(par_c, d->ups_pre_k, full_c);
-        if (ctx->fused_synthesis && d->ups_k == 8 && d->ups_pre_k == 7) {
+        float full_t[16], full_c[16];
+        level_taps(P, idx, full_t, full_c);
+        if (d->ups_k == 8 && d->ups_pre_k == 7) {
             if ((rc = ccd_ups_level(d_lat + P.lat_off_by_grid[gt], th, tw, cur, cc, ch, cw, full_t, full_c, nxt, st)))
                 return fail(CCD_ERR_CUDA, "ups_level launch");
         } else {
@@ -760,134 +800,238 @@ int run_synthesis(CcdContext *ctx, const PreparedJob &P, const int8_t *d_lat, co
             return fail(CCD_ERR_CUDA, "noise copy");
         // gh[0] x gw[0] == image size here, so the final bicubic interpolate is the identity
     }
-    // ---- synthesis (core/synthesis.py:272-294)
-    auto layer = [&](int l, int cin) {
-        SynLayerDev Ld;
-        Ld.cin = cin;
-        Ld.cout = d->syn_out[l];
-        Ld.k = d->syn_k[l];
-        Ld.residual = d->syn_res[l];
-        Ld.relu = d->syn_relu[l];
-        Ld.w = d_synw + P.syn_off_w[l];
-        Ld.b = d_synw + P.syn_off_b[l];
-        return Ld;
-    };
+    // ---- synthesis (core/synthesis.py:272-294): one kernel in the fused family, else one kernel per layer (two
+    // 1x1 layers at a time where k_syn_pw2 takes them)
+    const SynNet N = syn_net(P, d_synw);
     const bool same = (h0 == d->img_h && w0 == d->img_w);
-    SynLayerDev Lo{C, C, 1, 0, 0, d_synw + P.syn_off_ot_w, d_synw + P.syn_off_ot_b};
-    bool fused_done = false;
-    if (ctx->fused_synthesis) {
-        // one kernel for the whole synthesis when the architecture is in the fused family
-        SynLayerDev Ls{L.syn_stab_in, C, 1, 0, 0, d_synw + P.syn_off_st_w, d_synw + P.syn_off_st_b};
-        SynLayerDev all[CCD_MAX_SYN];
-        int in_ft0 = d->syn_in;
-        for (int l = 0; l < d->n_syn_layers; l++) {
-            all[l] = layer(l, in_ft0);
-            in_ft0 = d->syn_out[l];
-        }
-        rc = ccd_syn_fused(cur, h0, w0, d->syn_in, all, d->n_syn_layers, d->syn_stab ? &Ls : nullptr, Lo,
-                           same ? d_out : bufa, st);
-        if (rc > 0) return fail(CCD_ERR_CUDA, "fused synthesis launch");
-        fused_done = (rc == 0);
-    }
     float *ot_dst = same ? d_out : bufa;
-    if (!fused_done) {
-    if (d->syn_stab) {
-        SynLayerDev Ls{L.syn_stab_in, C, 1, 0, 0, d_synw + P.syn_off_st_w, d_synw + P.syn_off_st_b};
-        if ((rc = ccd_syn_layer(cur, h0, w0, Ls, stab, st))) return fail(CCD_ERR_CUDA, "stabiliser launch");
-    }
-    const float *src = cur;
-    float *dst = bufa, *other = bufb;
-    int in_ft = d->syn_in;
-    for (int l = 0; l < d->n_syn_layers; l++) {
-        if (fused[(size_t)l]) {
-            SynLayerDev L0 = layer(l, in_ft), L1 = layer(l + 1, d->syn_out[l]);
-            if ((rc = ccd_syn_pointwise2(src, h0, w0, L0, L1, dst, st))) return fail(CCD_ERR_CUDA, "pointwise launch");
-            in_ft = d->syn_out[l + 1];
-            l++;
-        } else {
-            SynLayerDev L0 = layer(l, in_ft);
-            if ((rc = ccd_syn_layer(src, h0, w0, L0, dst, st))) return fail(CCD_ERR_CUDA, "synthesis layer launch");
-            in_ft = d->syn_out[l];
+    rc = ccd_syn_fused(cur, h0, w0, d->syn_in, N.layers, d->n_syn_layers, d->syn_stab ? &N.stab : nullptr, N.ot, ot_dst, st);
+    if (rc > 0) return fail(CCD_ERR_CUDA, "fused synthesis launch");
+    if (rc < 0) {
+        if (d->syn_stab && (rc = ccd_syn_layer(cur, h0, w0, N.stab, stab, st))) return fail(CCD_ERR_CUDA, "stabiliser launch");
+        const float *src = cur;
+        float *dst = bufa, *other = bufb;
+        for (int l = 0; l < d->n_syn_layers; l++) {
+            if (SS.pw2[(size_t)l]) {
+                if ((rc = ccd_syn_pointwise2(src, h0, w0, N.layers[l], N.layers[l + 1], dst, st)))
+                    return fail(CCD_ERR_CUDA, "pointwise launch");
+                l++;
+            } else if ((rc = ccd_syn_layer(src, h0, w0, N.layers[l], dst, st))) {
+                return fail(CCD_ERR_CUDA, "synthesis layer launch");
+            }
+            src = dst;
+            std::swap(dst, other);
         }
-        src = dst;
-        std::swap(dst, other);
+        float *trunk = const_cast<float *>(src);
+        if (trunk == cur) return fail(CCD_ERR_ARG, "synthesis without layers");
+        if (d->syn_stab)
+            if ((rc = ccd_syn_add(trunk, stab, plane * (size_t)C, st))) return fail(CCD_ERR_CUDA, "add launch");
+        ot_dst = same ? d_out : dst;
+        if ((rc = ccd_syn_layer(trunk, h0, w0, N.ot, ot_dst, st))) return fail(CCD_ERR_CUDA, "output transform launch");
     }
-    float *trunk = const_cast<float *>(src);
-    if (trunk == cur) return fail(CCD_ERR_ARG, "synthesis without layers");
-    if (d->syn_stab)
-        if ((rc = ccd_syn_add(trunk, stab, plane * (size_t)C, st))) return fail(CCD_ERR_CUDA, "add launch");
-    ot_dst = same ? d_out : dst;
-    if ((rc = ccd_syn_layer(trunk, h0, w0, Lo, ot_dst, st))) return fail(CCD_ERR_CUDA, "output transform launch");
-    }
-    if (!same) {
-        // final F.interpolate (component/coolchic.py:187-192)
-        if (d->final_ups == 0)
-            rc = ccd_resize_nearest(ot_dst, C, h0, w0, d_out, d->img_h, d->img_w, st);
-        else
-            rc = ccd_resize_torch(ot_dst, C, h0, w0, d_out, d->img_h, d->img_w, d->final_ups == 1 ? 1 : 2,
-                                  (float)h0 / (float)d->img_h, (float)w0 / (float)d->img_w, st);
-        if (rc) return fail(CCD_ERR_CUDA, "resize launch");
-    }
-    (void)ctx;
-    return CCD_OK;
+    return same ? CCD_OK : resize_output(d, ot_dst, C, h0, w0, d_out, st);
 }
 
 size_t synthesis_scratch_bytes(const CcdCoolChicDesc *d) { return syn_scratch_plan(d).total + 4096; }
 
-// ---- batched float tail ------------------------------------------------------------------------------------
+// ---- float tail planning -----------------------------------------------------------------------------------
 // A job takes the batched path when its upsampling uses the default kernel sizes (8 / 7), it has at least two
 // latent grids, no common randomness, and its synthesis is in the fused family.  All such jobs of a call share
 //   * one launch per cascade level (all but the last), and
 //   * one launch (per (cinp, C) pair) of the kernel that evaluates the last level, the synthesis and -- for I
 //     frames that ask for it -- the frame tail.
-bool tail_eligible(const CcdCoolChicDesc *d, const NNLayout &L, PreparedJob &P) {
+// Every other job takes the per-stream path (run_synthesis), one job after the other.
+bool tail_eligible(const PreparedJob &P) {
+    const CcdCoolChicDesc *d = P.d;
+    const int nl = P.nl;
     if (d->ups_k != 8 || d->ups_pre_k != 7 || d->common_randomness) return false;
-    int nl = 0;
-    for (int g = 0; g < d->n_grids; g++)
-        if (!d->grid_is_hyper[g]) P.tail_gl[nl++] = g;
     if (nl < 2 || nl > 16 || nl != d->syn_in) return false;
-    const int nlay = d->n_syn_layers;
-    if (nlay < 2 || nlay > 4) return false;
-    const int C = d->syn_out[1];
-    if (d->syn_k[0] != 1 || d->syn_k[1] != 1 || d->syn_res[0] || d->syn_res[1] || d->syn_out[0] > 256 || C < 2 || C > 5) return false;
-    if (L.syn_c != C) return false;
-    for (int l = 2; l < nlay; l++)
-        if (d->syn_k[l] != 3 || d->syn_out[l] != C) return false;
-    if (d->syn_stab && L.syn_stab_in > nl) return false;
+    const SynNet N = syn_net(P, nullptr);
+    if (!ccd_syn_fused_family(nl, N.layers, d->n_syn_layers, d->syn_stab ? &N.stab : nullptr, N.ot)) return false;
     for (int i = 0; i + 1 < nl; i++) {
-        const int gt = P.tail_gl[i], gc = P.tail_gl[i + 1];
-        if (d->grid_h[gt] > 2 * d->grid_h[gc] || d->grid_w[gt] > 2 * d->grid_w[gc]) return false;  // (reported by the generic path)
+        const int gt = P.gl[i], gc = P.gl[i + 1];
+        if (d->grid_h[gt] > 2 * d->grid_h[gc] || d->grid_w[gt] > 2 * d->grid_w[gc]) return false;  // (reported by the per-stream path)
     }
-    P.tail_nl = nl;
-    P.tail_cinp = nl <= 4 ? 4 : (nl <= 8 ? 8 : 16);
-    P.tail_C = C;
     return true;
 }
 
 struct TailScratch {
     size_t p = 0, q = 0, raw = 0, total = 0;
 };
-TailScratch tail_scratch_plan(const CcdCoolChicDesc *d, const PreparedJob &P) {
+TailScratch tail_scratch_plan(const PreparedJob &P) {
+    const CcdCoolChicDesc *d = P.d;
     TailScratch T;
-    const int nl = P.tail_nl;
+    const int nl = P.nl;
     size_t o = 0;
     if (nl >= 3) {
-        const int g1 = P.tail_gl[1];
+        const int g1 = P.gl[1];
         T.p = o;
         o += al((size_t)(nl - 1) * d->grid_h[g1] * d->grid_w[g1] * 4);
     }
     if (nl >= 4) {
-        const int g2 = P.tail_gl[2];
+        const int g2 = P.gl[2];
         T.q = o;
         o += al((size_t)(nl - 2) * d->grid_h[g2] * d->grid_w[g2] * 4);
     }
-    const int g0 = P.tail_gl[0];
+    const int g0 = P.gl[0];
     if (d->grid_h[g0] != d->img_h || d->grid_w[g0] != d->img_w) {
         T.raw = o;
         o += al((size_t)P.tail_C * d->grid_h[g0] * d->grid_w[g0] * 4);
     }
     T.total = o;
     return T;
+}
+
+// The float tail of one call: which path each job takes, the scratch of both paths, the job arrays in the upload
+// arena and the batched path's launches.
+struct TailPlan {
+    struct LevelLaunch { size_t first; int count, planes, max_tw, max_th; };
+    struct SynGroup { int cinp, C, n3_max, hid_max, max_w, max_h, first, count; };
+    std::vector<int> order;                     // jobs of the batched path sorted by (cinp, C), one TailSynJob each
+    std::vector<SynGroup> groups;               // one k_tail_syn launch each
+    std::vector<std::pair<int, int>> lvl_jobs;  // (job, level) of every UpsLevelJob
+    std::vector<LevelLaunch> levels;            // the batched path's k_ups_level_b launches
+    size_t scratch_syn = 0, scratch_tail = 0;   // per-stream path (reused job after job), batched path
+    size_t off_syn = 0, off_lvl = 0;            // job arrays in the upload arena
+};
+
+void plan_tail(std::vector<PreparedJob> &P, const CcdJob *jobs, TailPlan &T) {
+    for (int i = 0; i < (int)P.size(); i++) {
+        PreparedJob &J = P[(size_t)i];
+        J.tail = tail_eligible(J);
+        if (J.tail) {
+            J.tail_cinp = J.nl <= 4 ? 4 : (J.nl <= 8 ? 8 : 16);
+            J.tail_C = J.d->syn_out[1];
+            const TailScratch S = tail_scratch_plan(J);
+            J.off_tailP = T.scratch_tail + S.p;
+            J.off_tailQ = T.scratch_tail + S.q;
+            J.off_tailRaw = T.scratch_tail + S.raw;
+            T.scratch_tail += al(S.total);
+            T.order.push_back(i);
+        } else {
+            size_t need = synthesis_scratch_bytes(J.d);
+            if (jobs[i].finish_bitdepth != 0) {  // raw output first, then the frame tail kernel
+                J.off_rawtmp = al(need);
+                need = J.off_rawtmp + al((size_t)3 * J.d->img_h * J.d->img_w * 4);
+            }
+            T.scratch_syn = std::max(T.scratch_syn, need);
+        }
+    }
+    std::stable_sort(T.order.begin(), T.order.end(), [&](int a, int b) {
+        const PreparedJob &A = P[(size_t)a], &B = P[(size_t)b];
+        return A.tail_cinp * 8 + A.tail_C < B.tail_cinp * 8 + B.tail_C;
+    });
+    // batched path: cascade level idx of every job that has one in one launch (planes = idx + 2)
+    int max_levels = 0;
+    for (int i : T.order) max_levels = std::max(max_levels, P[(size_t)i].nl - 2);
+    for (int idx = 0; idx < max_levels; idx++) {
+        TailPlan::LevelLaunch LL{T.lvl_jobs.size(), 0, idx + 2, 0, 0};
+        for (int i : T.order) {
+            const PreparedJob &J = P[(size_t)i];
+            if (idx >= J.nl - 2) continue;
+            const int gt = J.gl[J.nl - 2 - idx];
+            T.lvl_jobs.push_back({i, idx});
+            LL.count++;
+            LL.max_tw = std::max(LL.max_tw, J.d->grid_w[gt]);
+            LL.max_th = std::max(LL.max_th, J.d->grid_h[gt]);
+        }
+        if (LL.count) T.levels.push_back(LL);
+    }
+    // batched path: last level + synthesis (+ frame tail), one launch per (cinp, C)
+    for (size_t t = 0; t < T.order.size(); t++) {
+        const PreparedJob &J = P[(size_t)T.order[t]];
+        const CcdCoolChicDesc *d = J.d;
+        if (T.groups.empty() || T.groups.back().cinp != J.tail_cinp || T.groups.back().C != J.tail_C)
+            T.groups.push_back(TailPlan::SynGroup{J.tail_cinp, J.tail_C, 0, 0, 0, 0, (int)t, 0});
+        TailPlan::SynGroup &G = T.groups.back();
+        G.count++;
+        G.n3_max = std::max(G.n3_max, d->n_syn_layers - 2);
+        G.hid_max = std::max(G.hid_max, d->syn_out[0]);
+        G.max_w = std::max(G.max_w, d->grid_w[J.gl[0]]);
+        G.max_h = std::max(G.max_h, d->grid_h[J.gl[0]]);
+    }
+}
+
+// Fills the batched path's job arrays at h (host side of the upload arena dv); d_scr_tail: its scratch.
+void fill_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJob *jobs, const std::vector<int8_t *> &d_lat,
+               unsigned char *h, const unsigned char *dv, unsigned char *d_scr_tail) {
+    const size_t lb = ccd_tail_level_job_bytes(), jb = ccd_tail_job_bytes();
+    for (size_t k = 0; k < T.lvl_jobs.size(); k++) {
+        const int i = T.lvl_jobs[k].first, idx = T.lvl_jobs[k].second;
+        const PreparedJob &J = P[(size_t)i];
+        const CcdCoolChicDesc *d = J.d;
+        const int8_t *lat = d_lat[(size_t)i];
+        const int gt = J.gl[J.nl - 2 - idx], gc = J.gl[J.nl - 1 - idx];
+        // level idx writes P when (nl - 3 - idx) is even (the last one, idx = nl - 3, always writes P); level 0 reads
+        // the coarsest int8 grid itself
+        const bool to_p = ((J.nl - 3 - idx) & 1) == 0;
+        float *out = reinterpret_cast<float *>(d_scr_tail + (to_p ? J.off_tailP : J.off_tailQ));
+        const float *in = reinterpret_cast<const float *>(d_scr_tail + (to_p ? J.off_tailQ : J.off_tailP));
+        float full_t[16], full_c[16];
+        level_taps(J, idx, full_t, full_c);
+        ccd_tail_fill_level(h + T.off_lvl + k * lb, lat + J.lat_off_by_grid[gt], idx == 0 ? nullptr : in,
+                            idx == 0 ? lat + J.lat_off_by_grid[gc] : nullptr, out, idx + 1, d->grid_h[gc], d->grid_w[gc],
+                            d->grid_h[gt], d->grid_w[gt], full_t, full_c);
+    }
+    for (size_t t = 0; t < T.order.size(); t++) {
+        const int i = T.order[t];
+        const PreparedJob &J = P[(size_t)i];
+        const CcdCoolChicDesc *d = J.d;
+        const int nl = J.nl, g0 = J.gl[0], g1 = J.gl[1], C = J.tail_C;
+        const SynNet N = syn_net(J, reinterpret_cast<const float *>(dv + J.off_syn));
+        CcdTailSynDesc S;
+        memset(&S, 0, sizeof(S));
+        S.lat = d_lat[(size_t)i] + J.lat_off_by_grid[g0];
+        if (nl == 2) S.stk8 = d_lat[(size_t)i] + J.lat_off_by_grid[g1];
+        else S.stk = reinterpret_cast<const float *>(d_scr_tail + J.off_tailP);
+        S.h = d->grid_h[g0]; S.w = d->grid_w[g0]; S.ch = d->grid_h[g1]; S.cw = d->grid_w[g1]; S.cin = nl;
+        S.layers = N.layers; S.n_layers = d->n_syn_layers; S.stab = d->syn_stab ? &N.stab : nullptr;
+        S.ot = N.ot;
+        const size_t plane = (size_t)S.h * S.w;
+        const CcdJob &job = jobs[i];
+        if (S.h != d->img_h || S.w != d->img_w) {
+            float *raw = reinterpret_cast<float *>(d_scr_tail + J.off_tailRaw);
+            for (int c = 0; c < C; c++) S.out[c] = raw + (size_t)c * plane;
+        } else if (job.finish_bitdepth != 0 && job.finish_type == 1) {
+            S.out[0] = job.d_out; S.out[1] = job.d_out_u; S.out[2] = job.d_out_v;
+            S.finish = 2;
+        } else {
+            for (int c = 0; c < C; c++) S.out[c] = job.d_out + (size_t)c * plane;
+            S.finish = job.finish_bitdepth != 0 ? 1 : 0;
+        }
+        S.M = job.finish_bitdepth != 0 ? (float)((1 << job.finish_bitdepth) - 1) : 0.0f;
+        float full_t[16], full_c[16];
+        level_taps(J, nl - 2, full_t, full_c);
+        S.wt1d = full_t; S.wc1d = full_c;
+        S.allow_tma = J.pad_lat ? 1 : 0;
+        ccd_tail_fill_syn(h + T.off_syn + t * jb, S);
+    }
+}
+
+// The batched path's launches: every cascade level, then the last level + synthesis (+ frame tail) per group, then
+// the final resize of the outputs computed at a smaller size than the image (motion fields).
+int launch_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJob *jobs, const unsigned char *dv,
+                const unsigned char *d_scr_tail, cudaStream_t st) {
+    const size_t lb = ccd_tail_level_job_bytes(), jb = ccd_tail_job_bytes();
+    for (const TailPlan::LevelLaunch &LL : T.levels)
+        if (ccd_tail_launch_level(dv + T.off_lvl + LL.first * lb, LL.count, LL.planes, LL.max_tw, LL.max_th, st))
+            return fail(CCD_ERR_CUDA, "cascade level launch failed");
+    for (const TailPlan::SynGroup &G : T.groups) {
+        const int e = ccd_tail_launch_syn(dv + T.off_syn + (size_t)G.first * jb, G.count, G.cinp, G.C, G.n3_max, G.hid_max,
+                                          G.max_w, G.max_h, st);
+        if (e != 0) return fail(CCD_ERR_CUDA, "fused tail launch failed (%d)", e);
+    }
+    for (int i : T.order) {
+        const PreparedJob &J = P[(size_t)i];
+        const CcdCoolChicDesc *d = J.d;
+        const int h0 = d->grid_h[J.gl[0]], w0 = d->grid_w[J.gl[0]];
+        if (h0 == d->img_h && w0 == d->img_w) continue;
+        if (jobs[i].finish_bitdepth != 0) return fail(CCD_ERR_UNSUPPORTED, "job %d: frame tail on a resized output", i);
+        const int rc = resize_output(d, reinterpret_cast<const float *>(d_scr_tail + J.off_tailRaw), J.tail_C, h0, w0,
+                                     jobs[i].d_out, st);
+        if (rc) return rc;
+    }
+    return CCD_OK;
 }
 
 }  // namespace
@@ -1023,8 +1167,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     CUDA_TRY(cudaEventRecord(ctx->ev[0], st));
 
     std::vector<PreparedJob> P((size_t)n_jobs);
-    size_t up = 0, scratch_syn = 0, scratch_lat = 0, scratch_tail = 0;
-    size_t n_tail = 0, n_tail_levels = 0;
+    size_t up = 0, scratch_lat = 0;
     for (int i = 0; i < n_jobs; i++) {
         P[(size_t)i].job = &jobs[i];
         P[(size_t)i].d = jobs[i].desc;
@@ -1048,49 +1191,32 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         up += al(64);
         J.off_syn = up;
         up += al(J.syn_f.size() * 4);
-        if (stages & 2) {
-            if (jobs[i].finish_bitdepth != 0) {
-                if (jobs[i].finish_bitdepth < 1 || jobs[i].finish_bitdepth > 16 || jobs[i].finish_type < 0 || jobs[i].finish_type > 3)
-                    return fail(CCD_ERR_ARG, "job %d: bad frame tail request (bitdepth %d, type %d)", i, jobs[i].finish_bitdepth, jobs[i].finish_type);
-                if (J.L.syn_c != 3) return fail(CCD_ERR_ARG, "job %d: the frame tail needs a 3-channel output, found %d", i, J.L.syn_c);
-                if (jobs[i].finish_type == 1 && (!jobs[i].d_out_u || !jobs[i].d_out_v))
-                    return fail(CCD_ERR_ARG, "job %d: yuv420 frame tail needs u and v outputs", i);
-            }
-            J.tail = ctx->fused_synthesis && tail_eligible(J.d, J.L, J);
-            if (J.tail) {
-                const TailScratch T = tail_scratch_plan(J.d, J);
-                J.off_tailP = scratch_tail + T.p;
-                J.off_tailQ = scratch_tail + T.q;
-                J.off_tailRaw = scratch_tail + T.raw;
-                scratch_tail += al(T.total);
-                n_tail++;
-                n_tail_levels += (size_t)(J.tail_nl - 2);
-            } else {
-                size_t need = synthesis_scratch_bytes(J.d);
-                if (jobs[i].finish_bitdepth != 0) {  // raw output first, then the frame tail kernel
-                    J.off_rawtmp = al(need);
-                    need = J.off_rawtmp + al((size_t)3 * J.d->img_h * J.d->img_w * 4);
-                }
-                scratch_syn = std::max(scratch_syn, need);
-            }
+        if ((stages & 2) && jobs[i].finish_bitdepth != 0) {
+            if (jobs[i].finish_bitdepth < 1 || jobs[i].finish_bitdepth > 16 || jobs[i].finish_type < 0 || jobs[i].finish_type > 3)
+                return fail(CCD_ERR_ARG, "job %d: bad frame tail request (bitdepth %d, type %d)", i, jobs[i].finish_bitdepth, jobs[i].finish_type);
+            if (J.L.syn_c != 3) return fail(CCD_ERR_ARG, "job %d: the frame tail needs a 3-channel output, found %d", i, J.L.syn_c);
+            if (jobs[i].finish_type == 1 && (!jobs[i].d_out_u || !jobs[i].d_out_v))
+                return fail(CCD_ERR_ARG, "job %d: yuv420 frame tail needs u and v outputs", i);
         }
         J.off_lat = scratch_lat;
         if (own_lat) scratch_lat += al((size_t)J.lat_bytes);
     }
-    // device-resident job arrays of the batched float tail (filled below, uploaded with everything else)
-    const size_t off_tail_syn = up;
-    up += al(n_tail * ccd_tail_job_bytes());
-    const size_t off_tail_lvl = up;
-    up += al(n_tail_levels * ccd_tail_level_job_bytes());
+    TailPlan T;
+    if (stages & 2) plan_tail(P, jobs, T);
+    // device-resident job arrays of the float tail (filled below, uploaded with everything else)
+    T.off_syn = up;
+    up += al(T.order.size() * ccd_tail_job_bytes());
+    T.off_lvl = up;
+    up += al(T.lvl_jobs.size() * ccd_tail_level_job_bytes());
     const size_t off_streams = up;
     up += al(sizeof(EntStream) * (size_t)n_jobs);
     int rc;
     if ((rc = ensure_pin(ctx, up))) return rc;
     if ((rc = ensure_dev(ctx->upload, up))) return rc;
-    if ((rc = ensure_dev(ctx->scratch, scratch_lat + al(scratch_syn) + scratch_tail + 4096))) return rc;
+    if ((rc = ensure_dev(ctx->scratch, scratch_lat + al(T.scratch_syn) + T.scratch_tail + 4096))) return rc;
     unsigned char *h = ctx->h_pin, *dv = ctx->upload.p;
     unsigned char *d_scr_syn = ctx->scratch.p + scratch_lat;
-    unsigned char *d_scr_tail = d_scr_syn + al(scratch_syn);
+    unsigned char *d_scr_tail = d_scr_syn + al(T.scratch_syn);
 
     // group jobs by kernel configuration so that each group is one launch
     std::vector<int> order((size_t)n_jobs);
@@ -1129,117 +1255,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     for (int t = 0; t < n_jobs; t++)
         memcpy(h + off_streams + sizeof(EntStream) * (size_t)t, &P[(size_t)order[(size_t)t]].es, sizeof(EntStream));
 
-    // ---- batched float tail: job arrays.  Launch groups: cascade level `idx` of every stream that has one
-    // (planes = idx + 2), then one launch per (cinp, C) pair for the last level + synthesis (+ frame tail).
-    struct TailGroup { int cinp, C, n3_max, hid_max, max_w, max_h, first, count; };
-    std::vector<TailGroup> tail_groups;
-    struct TailLevelLaunch { size_t first; int count, planes, max_tw, max_th; };
-    std::vector<TailLevelLaunch> tail_levels;
-    std::vector<int> tail_order;  // jobs of the batched path, sorted by (cinp, C)
-    if (n_tail) {
-        for (int i = 0; i < n_jobs; i++)
-            if (P[(size_t)i].tail) tail_order.push_back(i);
-        std::stable_sort(tail_order.begin(), tail_order.end(), [&](int a, int b) {
-            const PreparedJob &A = P[(size_t)a], &B = P[(size_t)b];
-            return A.tail_cinp * 8 + A.tail_C < B.tail_cinp * 8 + B.tail_C;
-        });
-        const size_t jb = ccd_tail_job_bytes(), lb = ccd_tail_level_job_bytes();
-        // cascade levels
-        int max_levels = 0;
-        for (int i : tail_order) max_levels = std::max(max_levels, P[(size_t)i].tail_nl - 2);
-        size_t lvl_at = 0;
-        for (int idx = 0; idx < max_levels; idx++) {
-            TailLevelLaunch LL{lvl_at, 0, idx + 2, 0, 0};
-            for (int i : tail_order) {
-                const PreparedJob &J = P[(size_t)i];
-                const CcdCoolChicDesc *d = J.d;
-                const int nl = J.tail_nl;
-                if (idx >= nl - 2) continue;
-                const int gt = J.tail_gl[nl - 2 - idx], gc = J.tail_gl[nl - 1 - idx];
-                float par_t[8], par_c[8], full_t[16], full_c[16];
-                const float qs_uw = ldexpf(1.0f, d->qshift[4]);
-                const int kid = idx % d->n_ups;
-                for (int t = 0; t < J.L.kt_par; t++) par_t[t] = (float)J.nn[(size_t)(J.L.ups_tw + (int64_t)kid * J.L.kt_par + t)] * qs_uw;
-                for (int t = 0; t < J.L.kc_par; t++) par_c[t] = (float)J.nn[(size_t)(J.L.ups_cw + (int64_t)kid * J.L.kc_par + t)] * qs_uw;
-                expand_sym(par_t, d->ups_k, full_t);
-                expand_sym(par_c, d->ups_pre_k, full_c);
-                // level idx writes P when (nl - 3 - idx) is even (the last one, idx = nl - 3, always writes P)
-                const bool to_p = ((nl - 3 - idx) & 1) == 0;
-                float *out = reinterpret_cast<float *>(d_scr_tail + (to_p ? J.off_tailP : J.off_tailQ));
-                const float *in = reinterpret_cast<const float *>(d_scr_tail + (to_p ? J.off_tailQ : J.off_tailP));
-                const int8_t *in8 = idx == 0 ? d_lat[(size_t)i] + J.lat_off_by_grid[gc] : nullptr;
-                ccd_tail_fill_level(h + off_tail_lvl + (lvl_at + (size_t)LL.count) * lb, d_lat[(size_t)i] + J.lat_off_by_grid[gt],
-                                    idx == 0 ? nullptr : in, in8, out, idx + 1, d->grid_h[gc], d->grid_w[gc], d->grid_h[gt],
-                                    d->grid_w[gt], full_t, full_c);
-                LL.count++;
-                LL.max_tw = std::max(LL.max_tw, d->grid_w[gt]);
-                LL.max_th = std::max(LL.max_th, d->grid_h[gt]);
-            }
-            lvl_at += (size_t)LL.count;
-            if (LL.count) tail_levels.push_back(LL);
-        }
-        // last level + synthesis
-        const float *d_synw_base = reinterpret_cast<const float *>(dv);
-        for (size_t t = 0; t < tail_order.size(); t++) {
-            const int i = tail_order[t];
-            PreparedJob &J = P[(size_t)i];
-            const CcdCoolChicDesc *d = J.d;
-            const NNLayout &L = J.L;
-            const int nl = J.tail_nl, g0 = J.tail_gl[0], g1 = J.tail_gl[1];
-            const float *d_synw = reinterpret_cast<const float *>(dv + J.off_syn);
-            (void)d_synw_base;
-            SynLayerDev all[CCD_MAX_SYN];
-            int in_ft = d->syn_in;
-            for (int l = 0; l < d->n_syn_layers; l++) {
-                all[l] = SynLayerDev{in_ft, d->syn_out[l], d->syn_k[l], d->syn_res[l], d->syn_relu[l], d_synw + J.syn_off_w[l],
-                                     d_synw + J.syn_off_b[l]};
-                in_ft = d->syn_out[l];
-            }
-            const int C = J.tail_C;
-            SynLayerDev Ls{L.syn_stab_in, C, 1, 0, 0, d_synw + J.syn_off_st_w, d_synw + J.syn_off_st_b};
-            CcdTailSynDesc T;
-            memset(&T, 0, sizeof(T));
-            T.lat = d_lat[(size_t)i] + J.lat_off_by_grid[g0];
-            if (nl == 2) T.stk8 = d_lat[(size_t)i] + J.lat_off_by_grid[g1];
-            else T.stk = reinterpret_cast<const float *>(d_scr_tail + J.off_tailP);
-            T.h = d->grid_h[g0]; T.w = d->grid_w[g0]; T.ch = d->grid_h[g1]; T.cw = d->grid_w[g1]; T.cin = nl;
-            T.layers = all; T.n_layers = d->n_syn_layers; T.stab = d->syn_stab ? &Ls : nullptr;
-            T.ot = SynLayerDev{C, C, 1, 0, 0, d_synw + J.syn_off_ot_w, d_synw + J.syn_off_ot_b};
-            const bool same = (T.h == d->img_h && T.w == d->img_w);
-            const size_t plane = (size_t)T.h * T.w;
-            const CcdJob &job = jobs[i];
-            if (!same) {
-                float *raw = reinterpret_cast<float *>(d_scr_tail + J.off_tailRaw);
-                for (int c = 0; c < C; c++) T.out[c] = raw + (size_t)c * plane;
-            } else if (job.finish_bitdepth != 0 && job.finish_type == 1) {
-                T.out[0] = job.d_out; T.out[1] = job.d_out_u; T.out[2] = job.d_out_v;
-                T.finish = 2;
-            } else {
-                for (int c = 0; c < C; c++) T.out[c] = job.d_out + (size_t)c * plane;
-                T.finish = job.finish_bitdepth != 0 ? 1 : 0;
-            }
-            T.M = job.finish_bitdepth != 0 ? (float)((1 << job.finish_bitdepth) - 1) : 0.0f;
-            float par_t[8], par_c[8], full_t[16], full_c[16];
-            const float qs_uw = ldexpf(1.0f, d->qshift[4]);
-            const int kid = (nl - 2) % d->n_ups;
-            for (int k = 0; k < L.kt_par; k++) par_t[k] = (float)J.nn[(size_t)(L.ups_tw + (int64_t)kid * L.kt_par + k)] * qs_uw;
-            for (int k = 0; k < L.kc_par; k++) par_c[k] = (float)J.nn[(size_t)(L.ups_cw + (int64_t)kid * L.kc_par + k)] * qs_uw;
-            expand_sym(par_t, d->ups_k, full_t);
-            expand_sym(par_c, d->ups_pre_k, full_c);
-            T.wt1d = full_t; T.wc1d = full_c;
-            T.allow_tma = J.pad_lat ? 1 : 0;
-            const int tr = ccd_tail_fill_syn(h + off_tail_syn + t * jb, T);
-            if (tr < 0) return fail(CCD_ERR_ARG, "internal: job %d is not in the fused synthesis family", i);
-            if (tail_groups.empty() || tail_groups.back().cinp != J.tail_cinp || tail_groups.back().C != C)
-                tail_groups.push_back(TailGroup{J.tail_cinp, C, 0, 0, 0, 0, (int)t, 0});
-            TailGroup &G = tail_groups.back();
-            G.count++;
-            G.n3_max = std::max(G.n3_max, d->n_syn_layers - 2);
-            G.hid_max = std::max(G.hid_max, d->syn_out[0]);
-            G.max_w = std::max(G.max_w, T.w);
-            G.max_h = std::max(G.max_h, T.h);
-        }
-    }
+    if (stages & 2) fill_tail(T, P, jobs, d_lat, h, dv, d_scr_tail);
     CUDA_TRY(cudaMemcpyAsync(dv, h, up, cudaMemcpyHostToDevice, st));
     ctx->last_upload_bytes = up;
     CUDA_TRY(cudaEventRecord(ctx->ev[1], st));
@@ -1284,49 +1300,23 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     }
     CUDA_TRY(cudaEventRecord(ctx->ev[2], st));
     if (stages & 2) {
-        // batched path: all cascade levels, then the fused last level + synthesis (+ frame tail)
-        const size_t jb = ccd_tail_job_bytes(), lb = ccd_tail_level_job_bytes();
-        for (const TailLevelLaunch &LL : tail_levels)
-            if (ccd_tail_launch_level(dv + off_tail_lvl + LL.first * lb, LL.count, LL.planes, LL.max_tw, LL.max_th, st))
-                return fail(CCD_ERR_CUDA, "cascade level launch failed");
-        for (const TailGroup &G : tail_groups) {
-            const int e = ccd_tail_launch_syn(dv + off_tail_syn + (size_t)G.first * jb, G.count, G.cinp, G.C, G.n3_max, G.hid_max,
-                                              G.max_w, G.max_h, st);
-            if (e != 0) return fail(CCD_ERR_CUDA, "fused tail launch failed (%d)", e);
-        }
-        for (int i : tail_order) {
-            // grids smaller than the image (motion fields): final F.interpolate (component/coolchic.py:187-192)
-            const PreparedJob &J = P[(size_t)i];
-            const CcdCoolChicDesc *d = J.d;
-            const int g0 = J.tail_gl[0], h0 = d->grid_h[g0], w0 = d->grid_w[g0];
-            if (h0 == d->img_h && w0 == d->img_w) continue;
-            const float *raw = reinterpret_cast<const float *>(d_scr_tail + J.off_tailRaw);
-            float *dst = jobs[i].d_out;
-            unsigned char *tmp = nullptr;
-            if (jobs[i].finish_bitdepth != 0) return fail(CCD_ERR_UNSUPPORTED, "job %d: frame tail on a resized output", i);
-            (void)tmp;
-            if (d->final_ups == 0)
-                rc = ccd_resize_nearest(raw, J.tail_C, h0, w0, dst, d->img_h, d->img_w, st);
-            else
-                rc = ccd_resize_torch(raw, J.tail_C, h0, w0, dst, d->img_h, d->img_w, d->final_ups == 1 ? 1 : 2,
-                                      (float)h0 / (float)d->img_h, (float)w0 / (float)d->img_w, st);
-            if (rc) return fail(CCD_ERR_CUDA, "resize launch");
-        }
-        // everything else: one stream after the other through the general kernels
+        if ((rc = launch_tail(T, P, jobs, dv, d_scr_tail, st))) return rc;
+        // everything else: one job after the other through the per-stream path
         for (int i = 0; i < n_jobs; i++) {
-            if (P[(size_t)i].tail) continue;
+            const PreparedJob &J = P[(size_t)i];
+            if (J.tail) continue;
             const bool fin = jobs[i].finish_bitdepth != 0;
-            float *raw_dst = fin ? reinterpret_cast<float *>(d_scr_syn + P[(size_t)i].off_rawtmp) : jobs[i].d_out;
-            rc = run_synthesis(ctx, P[(size_t)i], d_lat[(size_t)i], reinterpret_cast<const float *>(dv + P[(size_t)i].off_syn),
-                               raw_dst, d_scr_syn, scratch_syn, st);
+            float *raw_dst = fin ? reinterpret_cast<float *>(d_scr_syn + J.off_rawtmp) : jobs[i].d_out;
+            rc = run_synthesis(J, d_lat[(size_t)i], reinterpret_cast<const float *>(dv + J.off_syn), raw_dst, d_scr_syn,
+                               T.scratch_syn, st);
             if (rc) {
                 jobs[i].status = rc;
                 return rc;
             }
             if (fin) {
                 const int ft = jobs[i].finish_type == 3 ? 2 : jobs[i].finish_type;
-                if (ccd_finish(raw_dst, P[(size_t)i].d->img_h, P[(size_t)i].d->img_w, jobs[i].finish_bitdepth, ft, jobs[i].d_out,
-                               jobs[i].d_out_u, jobs[i].d_out_v, st))
+                if (ccd_finish(raw_dst, J.d->img_h, J.d->img_w, jobs[i].finish_bitdepth, ft, jobs[i].d_out, jobs[i].d_out_u,
+                               jobs[i].d_out_v, st))
                     return fail(CCD_ERR_CUDA, "finish_frame launch failed");
             }
         }
@@ -1515,12 +1505,6 @@ int ccd_debug_laplace_domain(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *ou
 }
 
 uint64_t ccd_debug_launch_count(void) { return g_ccd_launches; }
-
-int ccd_debug_set_fused_synthesis(CcdContext *ctx, int on) {
-    if (!ctx) return fail(CCD_ERR_ARG, "null context");
-    ctx->fused_synthesis = on ? 1 : 0;
-    return CCD_OK;
-}
 
 int ccd_debug_set_producer_mask(CcdContext *ctx, uint32_t mask) {
     if (!ctx || (mask & 0x3fffu) == 0) return fail(CCD_ERR_ARG, "bad producer mask");

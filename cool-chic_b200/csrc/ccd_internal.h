@@ -111,13 +111,19 @@ int ccd_ups_level(const int8_t *d_lat, int th, int tw, const float *d_in, int cc
 int ccd_syn_layer(const float *d_in, int h, int w, const SynLayerDev &L, float *d_out, cudaStream_t st);
 int ccd_syn_pointwise2(const float *d_in, int h, int w, const SynLayerDev &L0, const SynLayerDev &L1,
                        float *d_out, cudaStream_t st);
-// whole synthesis in one kernel when the architecture allows it (returns -1 otherwise: use the layer kernels)
+// The synthesis architectures that k_syn_fused and k_tail_syn evaluate in one kernel: 1x1 cin -> hid (cin <= 16,
+// hid <= 256), 1x1 hid -> C (C in 2..5), 0-2 3x3 layers C -> C, the stabiliser (if any) 1x1 <= cin -> C, the output
+// transform 1x1 C -> C.
+bool ccd_syn_fused_family(int cin, const SynLayerDev *layers, int n_layers, const SynLayerDev *stab,
+                          const SynLayerDev &ot);
+// whole synthesis in one kernel when the architecture is in the fused family (returns -1 otherwise: use the layer
+// kernels)
 int ccd_syn_fused(const float *d_in, int h, int w, int cin, const SynLayerDev *layers, int n_layers,
                   const SynLayerDev *stab, const SynLayerDev &ot, float *d_out, cudaStream_t st);
 int ccd_syn_add(float *d_a, const float *d_b, size_t n, cudaStream_t st);
 
 // ---- batched float tail (ccd_synth.cu): device-resident job arrays, one launch per cascade level and one for
-// the last level + synthesis + frame tail of ALL streams of a group
+// the last level + synthesis + frame tail of ALL streams of a group (a synthesis in the fused family)
 struct CcdTailSynDesc {
     const int8_t *lat;        // finest latent grid [h][w]
     const float *stk;         // coarser stack [cin - 1][ch][cw] (fp32), or ...
@@ -138,7 +144,7 @@ size_t ccd_tail_level_job_bytes(void);
 void ccd_tail_fill_level(void *dst, const int8_t *lat, const float *in, const int8_t *in8, float *out, int cc, int ch,
                          int cw, int th, int tw, const float *wt1d, const float *wc1d);
 int ccd_tail_launch_level(const void *d_jobs, int n_jobs, int planes, int max_tw, int max_th, cudaStream_t st);
-int ccd_tail_fill_syn(void *dst, const CcdTailSynDesc &T);
+void ccd_tail_fill_syn(void *dst, const CcdTailSynDesc &T);
 int ccd_tail_launch_syn(const void *d_jobs, int n_jobs, int cinp, int C, int n3_max, int hid_max, int max_w, int max_h,
                         cudaStream_t st);
 int ccd_resize_nearest(const float *d_in, int c, int h, int w, float *d_out, int H, int W, cudaStream_t st);

@@ -1161,6 +1161,15 @@ K1d make_k1d(const float *w1d, int k) {
     return r;
 }
 
+// kron(w, w) of a k-tap separable kernel: out[a * k + b] = w[a] * w[b]
+void kron(const float *w, int k, float *out) {
+    for (int a = 0; a < k; a++)
+        for (int b = 0; b < k; b++) {
+            volatile float p = w[a] * w[b];  // one rounded fp32 product, no contraction
+            out[a * k + b] = p;
+        }
+}
+
 }  // namespace
 
 int ccd_ups_first(const int8_t *d_lat, int h, int w, float *d_out, cudaStream_t st) {
@@ -1187,16 +1196,8 @@ int ccd_ups_level(const int8_t *d_lat, int th, int tw, const float *d_in, int cc
                   const float *wc1d, float *d_out, cudaStream_t st) {
     UpsLevelParams P;
     P.lat = d_lat; P.in = d_in; P.out = d_out; P.cc = cc; P.ch = ch; P.cw = cw; P.th = th; P.tw = tw;
-    for (int a = 0; a < 8; a++)
-        for (int b = 0; b < 8; b++) {
-            volatile float k = wt1d[a] * wt1d[b];  // one rounded fp32 product, no contraction
-            P.kt[a][b] = k;
-        }
-    for (int a = 0; a < 7; a++)
-        for (int b = 0; b < 7; b++) {
-            volatile float k = wc1d[a] * wc1d[b];
-            P.kc[a][b] = k;
-        }
+    kron(wt1d, 8, &P.kt[0][0]);
+    kron(wc1d, 7, &P.kc[0][0]);
     k_ups_level<<<grid2(tw, th, cc + 1), kBlock2, 0, st>>>(P);
     g_ccd_launches++;
     return (int)cudaGetLastError();
@@ -1238,17 +1239,24 @@ static int launch_syn_fused(const SynFusedParams &P, cudaStream_t st) {
     return (int)cudaGetLastError();
 }
 
+bool ccd_syn_fused_family(int cin, const SynLayerDev *layers, int n_layers, const SynLayerDev *stab,
+                          const SynLayerDev &ot) {
+    if (n_layers < 2 || n_layers > 4) return false;
+    const SynLayerDev &L0 = layers[0], &L1 = layers[1];
+    const int C = L1.cout;
+    if (L0.k != 1 || L1.k != 1 || L0.residual || L1.residual || cin > 16 || L0.cout > 256 || C < 2 || C > 5) return false;
+    if (ot.cin != C || ot.cout != C) return false;
+    for (int l = 2; l < n_layers; l++)
+        if (layers[l].k != 3 || layers[l].cin != C || layers[l].cout != C) return false;
+    return !stab || (stab->cin <= cin && stab->cout == C);
+}
+
 // returns -1 when the architecture is outside the fused family (caller falls back to the layer kernels)
 int ccd_syn_fused(const float *d_in, int h, int w, int cin, const SynLayerDev *layers, int n_layers,
                   const SynLayerDev *stab, const SynLayerDev &ot, float *d_out, cudaStream_t st) {
-    if (n_layers < 2 || n_layers > 4) return -1;
+    if (!ccd_syn_fused_family(cin, layers, n_layers, stab, ot)) return -1;
     const SynLayerDev &L0 = layers[0], &L1 = layers[1];
     const int C = L1.cout;
-    if (L0.k != 1 || L1.k != 1 || L0.residual || L1.residual || cin > 16 || L0.cout > 256 || C < 2 || C > 5) return -1;
-    if (ot.cin != C || ot.cout != C) return -1;
-    for (int l = 2; l < n_layers; l++)
-        if (layers[l].k != 3 || layers[l].cin != C || layers[l].cout != C) return -1;
-    if (stab && (stab->cin > cin || stab->cout != C)) return -1;
     SynFusedParams P;
     P.in = d_in; P.out = d_out; P.h = h; P.w = w; P.cin = cin; P.hid = L0.cout; P.n3 = n_layers - 2;
     P.relu0 = L0.relu; P.relu1 = L1.relu;
@@ -1281,16 +1289,8 @@ void ccd_tail_fill_level(void *dst, const int8_t *lat, const float *in, const in
     UpsLevelJob J;
     memset(&J, 0, sizeof(J));
     J.lat = lat; J.in = in; J.in8 = in8; J.out = out; J.cc = cc; J.ch = ch; J.cw = cw; J.th = th; J.tw = tw;
-    for (int a = 0; a < 8; a++)
-        for (int b = 0; b < 8; b++) {
-            volatile float k = wt1d[a] * wt1d[b];  // one rounded fp32 product, no contraction
-            J.kt[a][b] = k;
-        }
-    for (int a = 0; a < 7; a++)
-        for (int b = 0; b < 7; b++) {
-            volatile float k = wc1d[a] * wc1d[b];
-            J.kc[a][b] = k;
-        }
+    kron(wt1d, 8, &J.kt[0][0]);
+    kron(wc1d, 7, &J.kc[0][0]);
     memcpy(dst, &J, sizeof(J));
 }
 
@@ -1321,18 +1321,11 @@ PFN_encodeTiled get_encode_tiled() {
 }
 }  // namespace
 
-// Fills one TailSynJob (host memory).  Returns 1 when the tiles are staged with TMA, 0 when with plain loads
-// (pitches / addresses that cuTensorMapEncodeTiled does not take), < 0 when the architecture is outside the family.
-int ccd_tail_fill_syn(void *dst, const CcdTailSynDesc &T) {
+// Fills one TailSynJob (host memory).  The tiles are staged with TMA unless the pitches / addresses are ones that
+// cuTensorMapEncodeTiled does not take (plain loads then).
+void ccd_tail_fill_syn(void *dst, const CcdTailSynDesc &T) {
     const int n_layers = T.n_layers;
-    if (n_layers < 2 || n_layers > 4) return -1;
     const SynLayerDev &L0 = T.layers[0], &L1 = T.layers[1];
-    const int C = L1.cout;
-    if (L0.k != 1 || L1.k != 1 || L0.residual || L1.residual || T.cin > 16 || T.cin < 2 || L0.cout > 256 || C < 2 || C > 5) return -1;
-    if (T.ot.cin != C || T.ot.cout != C) return -1;
-    for (int l = 2; l < n_layers; l++)
-        if (T.layers[l].k != 3 || T.layers[l].cin != C || T.layers[l].cout != C) return -1;
-    if (T.stab && (T.stab->cin > T.cin || T.stab->cout != C)) return -1;
     TailSynJob J;
     memset(&J, 0, sizeof(J));
     J.lat = T.lat; J.stk = T.stk; J.stk8 = T.stk8;
@@ -1352,16 +1345,8 @@ int ccd_tail_fill_syn(void *dst, const CcdTailSynDesc &T) {
     J.wo = T.ot.w; J.bo = T.ot.b;
     J.finish = T.finish;
     J.M = T.M;
-    for (int a = 0; a < 8; a++)
-        for (int b = 0; b < 8; b++) {
-            volatile float k = T.wt1d[a] * T.wt1d[b];
-            J.kt[a][b] = k;
-        }
-    for (int a = 0; a < 7; a++)
-        for (int b = 0; b < 7; b++) {
-            volatile float k = T.wc1d[a] * T.wc1d[b];
-            J.kc[a][b] = k;
-        }
+    kron(T.wt1d, 8, &J.kt[0][0]);
+    kron(T.wc1d, 7, &J.kc[0][0]);
     // TMA descriptors (CU_TENSOR_MAP_DATA_TYPE_UINT8 = 0, FLOAT32 = 7; no interleave, no swizzle, L2 promotion 128 B,
     // out-of-bounds elements read as zero)
     J.use_tma = 0;
@@ -1382,7 +1367,6 @@ int ccd_tail_fill_syn(void *dst, const CcdTailSynDesc &T) {
         J.use_tma = (r0 == 0 && r1 == 0) ? 1 : 0;
     }
     memcpy(dst, &J, sizeof(J));
-    return J.use_tma;
 }
 
 template <int CINP, int C>

@@ -216,9 +216,6 @@ uint64_t ccd_debug_launch_count(void);
  * warp 14 is the coder's helper, warp 15 the range coder).  Default 0x3777: warps 3, 7, 11 stay idle so
  * that the coder owns scheduler partition 3. */
 int ccd_debug_set_producer_mask(CcdContext *ctx, uint32_t mask);
-/* 1 (default): one fused kernel for the synthesis when the architecture allows it; 0: one kernel per
- * layer.  Both give bit-identical results (tests/test_gpu_decode.py). */
-int ccd_debug_set_fused_synthesis(CcdContext *ctx, int on);
 
 /* Entropy-kernel status words of the last job of the last call: [0] error, [1] words consumed,
  * [2] slow-path symbols (outside the 31-symbol window), [3] words emitted (encode modes),

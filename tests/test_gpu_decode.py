@@ -599,43 +599,72 @@ def test_common_randomness_1080p_properties(ctx, seed_stream):
     assert float((a - p).abs().mean()) > 1e-3
 
 
-def test_fused_synthesis_equals_layer_kernels(ctx, seed_stream):
-    """The fused synthesis kernel (tile + halo, shared-memory 3x3 stages) against the one-kernel-per-layer
-    path: bit-identical on every architecture of the fused family that the streams use (3 / 4 / 5 / 2 output
-    channels, 0-2 3x3 layers, with and without stabiliser, common randomness), odd sizes and tiny frames."""
-    import torch
+def _syn(*layers, **fields):
+    """Cool-chic header overrides: these synthesis layers, then any other header fields."""
+    ov = {"n_layer_synthesis": len(layers), **{f"syn_layer_{i}": lay for i, lay in enumerate(layers)}}
+    ov.update(fields)
+    return ov
 
+
+_FIVE_LAYERS = _syn("48-1-linear-relu", "3-1-linear-none", "3-3-residual-relu", "3-3-residual-relu", "3-3-residual-none")
+
+
+# (image size, latent resolution, final upsampling, header overrides, frame tail, library launches of the decode).
+# Every decode launches the entropy kernel once; the rest of each count is broken down in the comment.
+@pytest.mark.parametrize("size,lat,fin_ups,ov,finish,launches", [
+    # batched path: k_ups_level_b per cascade level but the last, k_tail_syn, the final resize if any
+    pytest.param((131, 203), (0, 6), None, None, None, 1 + 5 + 1, id="hop_3ch_two_3x3"),
+    pytest.param((70, 50), (0, 3), None, _syn("16-1-linear-relu", "4-1-linear-none", "4-3-residual-relu",
+                                              "4-3-residual-none"), None, 1 + 2 + 1, id="residue_4ch"),
+    pytest.param((64, 96), (0, 4), None, _syn("16-1-linear-relu", "5-1-linear-none", "5-3-residual-relu"), None,
+                 1 + 3 + 1, id="residue_5ch_one_3x3"),
+    pytest.param((48, 80), (2, 5), "nearest", _syn("16-1-linear-relu", "2-1-linear-none"), None, 1 + 2 + 1 + 1,
+                 id="motion_2ch_no_3x3_resize"),
+    pytest.param((17, 9), (0, 2), None, None, None, 1 + 1 + 1, id="smaller_than_one_tile"),
+    # per-stream path
+    # k_ups_first, k_ups_level per level, k_cr_noise + 3 noise resizes, k_syn_fused (8 inputs, stabiliser on 4)
+    pytest.param((40, 56), (0, 3), None, {"flag_common_randomness": 1}, None, 1 + 1 + 3 + 1 + 3 + 1,
+                 id="common_randomness"),
+    # k_ups_first, k_ups_pre + k_ups_convt per level, k_syn_fused
+    pytest.param((37, 61), (0, 3), None, {"ups_k_size": 6, "ups_preconcat_k_size": 5}, None, 1 + 1 + 2 * 3 + 1,
+                 id="ups_6_5"),
+    # k_ups_first, k_ups_level per level, stabiliser, k_syn_pw2, three k_syn_layer, k_add, output transform
+    pytest.param((40, 56), (0, 3), None, _FIVE_LAYERS, None, 1 + 1 + 3 + 1 + 1 + 3 + 1 + 1, id="five_layers"),
+    # k_ups_first, k_ups_level per level, two k_syn_layer, output transform
+    pytest.param((40, 56), (0, 3), None, _syn("8-3-linear-relu", "3-1-linear-none", linear_stabiliser_synth=0), None,
+                 1 + 1 + 3 + 2 + 1, id="3x3_first_layer"),
+    # k_ups_first, k_syn_fused
+    pytest.param((40, 56), (0, 0), None, None, None, 1 + 1 + 1, id="single_grid"),
+    # as five_layers, then ccd_finish: k_finish_444 on luma, k_finish_420_uv
+    pytest.param((40, 56), (0, 3), None, _FIVE_LAYERS, (8, "yuv420"), 1 + 1 + 3 + 7 + 2,
+                 id="five_layers_finish_yuv420"),
+])
+def test_synthesis_paths_vs_oracle(ctx, oracle, seed_stream, size, lat, fin_ups, ov, finish, launches):
+    """Every path of the float tail against the oracle, bit for bit: the batched path (fused family, default kernel
+    sizes, several grids) and the per-stream path with k_syn_fused or one kernel per layer, default or other
+    upsampling kernel sizes, common randomness, one latent grid, the frame tail.  The number of launches pins
+    which path and which kernels ran."""
     from coolchic_b200 import synth
     from coolchic_b200._desc import desc_from_header
 
-    cases = [
-        ((131, 203), (0, 6), None, None),                                   # hop, 3 channels, 2 x 3x3
-        ((70, 50), (0, 3), None, synth._syn_overrides(16, 4, 4)),           # P residue: 4 channels
-        ((64, 96), (0, 4), None, synth._syn_overrides(16, 5, 3)),           # B residue: 5 channels, one 3x3
-        ((48, 80), (2, 5), "nearest", synth._syn_overrides(16, 2, 2)),      # motion: 2 channels, no 3x3, resize
-        ((40, 56), (0, 3), None, {"flag_common_randomness": 1}),            # 8 inputs, stabiliser on 4
-        ((17, 9), (0, 2), None, None),                                      # smaller than one tile
-    ]
-    try:
-        for size, lat, fin, ov in cases:
-            cc, h, _ = synth.make_coolchic(ctx, seed_stream, size, lat, None, seed=2, final_upsampling_type=fin, overrides=ov)
-            h2 = type(h)()
-            rest = h2.read_header(cc)
-            d = desc_from_header(h2)
-            nnb = rest[:h2.get_value("nn_n_bytes")]
-            lb = rest[h2.get_value("nn_n_bytes"):][:h2.get_value("n_bytes_latent")]
-            ctx.set_fused_synthesis(True)
-            n0 = ctx.launch_count()
-            a = ctx.decode_coolchic(d, nnb, lb)
-            n_fused = ctx.launch_count() - n0
-            ctx.set_fused_synthesis(False)
-            n0 = ctx.launch_count()
-            b = ctx.decode_coolchic(d, nnb, lb)
-            n_layers = ctx.launch_count() - n0
-            assert torch.equal(a, b), (size, lat)
-            assert n_fused < n_layers, (size, n_fused, n_layers)  # the fused kernel did run
-    finally:
-        ctx.set_fused_synthesis(True)
+    cc, h, _ = synth.make_coolchic(ctx, seed_stream, size, lat, None, seed=2, final_upsampling_type=fin_ups, overrides=ov)
+    h2 = type(h)()
+    rest = h2.read_header(cc)
+    d = desc_from_header(h2)
+    nnb = rest[:h2.get_value("nn_n_bytes")]
+    lb = rest[h2.get_value("nn_n_bytes"):][:h2.get_value("n_bytes_latent")]
+    n0 = ctx.launch_count()
+    out, _ = ctx.decode_many([d], [nnb], [lb], finish=[finish])
+    assert ctx.launch_count() - n0 == launches
+    nn = oracle.decode_nn(d, nnb)
+    lat_o, _ = oracle.decode_latents(d, nn, lb)
+    want = oracle.synthesize(d, nn, lat_o)
+    if finish is None:
+        assert np.array_equal(out[0][0].cpu().numpy(), want)
+    else:
+        want = oracle.finish_frame(want, *finish)
+        for k in "yuv":
+            assert np.array_equal(out[0][k][0, 0].cpu().numpy(), want[k]), k
 
 
 def test_corrupt_streams_fail_cleanly_on_the_device(ctx, seed_stream):

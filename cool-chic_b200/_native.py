@@ -185,8 +185,8 @@ class Context:
                     latent_bytes: Sequence[bytes], want_latents: bool = False, finish=None):
         """Decode n independent Cool-chics concurrently.  Returns (outputs, latents) where
         outputs[i] is a float32 CUDA tensor [1, C, H, W] (raw synthesis output).
-        ``finish[i] = (bitdepth, frame_data_type)`` (or None) asks for decode_frame's frame tail fused into the
-        synthesis kernel: outputs[i] is then the FINISHED frame in FrameData layout ([1, 3, H, W], or the
+        ``finish[i] = (bitdepth, frame_data_type)`` (or None) asks for decode_frame's frame tail (3-channel
+        outputs only): outputs[i] is then the FINISHED frame in FrameData layout ([1, 3, H, W], or the
         y / u / v dictionary for yuv420)."""
         n = len(descs)
         jobs = (CcdJob * n)()

@@ -101,8 +101,8 @@ class CoolChicDecoder:
 def decode_coolchics(headers: Sequence[CoolChicHeader], bytes_nn: Sequence[bytes], bytes_latent: Sequence[bytes],
                      device: int = 0, finish=None) -> List[Tensor]:
     """Decode several independent Cool-chics CONCURRENTLY (one persistent CTA per stream).  ``finish[i]`` =
-    (bitdepth, frame_data_type) for the Cool-chic of an I frame: the synthesis kernel then writes the finished
-    frame (decode.py:191-206 fused into its epilogue) instead of the raw output."""
+    (bitdepth, frame_data_type) for the Cool-chic of an I frame: libccdec then returns the finished frame
+    (decode.py:191-206 applied) instead of the raw output."""
     ctx = _native.get_context(device)
     descs = [desc_from_header(h) for h in headers]
     outs, _ = ctx.decode_many(descs, [bytes(b) for b in bytes_nn], [bytes(b) for b in bytes_latent], finish=finish)

@@ -44,12 +44,12 @@ def _parse_frame(bitstream_bytes: bytes):
 
 
 def _finish_request(frame_header: FrameHeader, ccs):
-    """(bitdepth, frame_data_type) when the frame tail can be fused into the synthesis of this frame's Cool-chic:
-    an I frame whose Cool-chic has 3 output channels at the image size (else None: separate kernel)."""
+    """(bitdepth, frame_data_type) for the Cool-chic of an I frame with 3 output channels: libccdec then returns the
+    finished frame (decode.py:191-206 applied) instead of the raw output.  None otherwise."""
     if frame_header.get_value("frame_type") != "I":
         return None
     p = ccs["residue"][0].get_coolchic_parameter()
-    if int(p.layers_synthesis[-1].split("-")[0]) != 3 or p.latent_resolution[0] != 0:
+    if int(p.layers_synthesis[-1].split("-")[0]) != 3:
         return None
     return (frame_header.get_value("bitdepth"), frame_header.get_value("frame_data_type"))
 
@@ -62,13 +62,10 @@ def _reconstruct(frame_header: FrameHeader, cc_out: Dict[str, torch.Tensor], ref
     bitdepth = frame_header.get_value("bitdepth")
     frame_data_type = frame_header.get_value("frame_data_type")
     if frame_type == "I":
-        decoded = cc_out["residue"]
-        if cc_out.get("finished"):
-            data = decoded  # the synthesis kernel already applied the frame tail
-        else:
-            if decoded.size(1) != 3:
-                raise ValueError(f"Frame reconstruction expects 3 channels, found {decoded.size(1)}")
-            data = ctx.finish_frame(decoded, bitdepth, frame_data_type)
+        # finished by libccdec when it has 3 channels (_finish_request): a tensor or, for yuv420, a dictionary
+        data = cc_out["residue"]
+        if torch.is_tensor(data) and data.size(1) != 3:
+            raise ValueError(f"Frame reconstruction expects 3 channels, found {data.size(1)}")
     else:
         # prediction + blending + residue + frame tail: one kernel, 4:2:0 references read in place
         refs = [r.to(ctx.torch_device) for r in reference_frames]
@@ -93,9 +90,7 @@ def decode_frame(bitstream_bytes: bytes, reference_frames: List[FrameData], verb
     if verbosity:
         for n in names:
             print(ccs[n][0].pretty_string())
-    cc_out = dict(zip(names, outs))
-    cc_out["finished"] = fin is not None
-    frame = _reconstruct(frame_header, cc_out, reference_frames, device)
+    frame = _reconstruct(frame_header, dict(zip(names, outs)), reference_frames, device)
     return frame, rest
 
 
@@ -111,26 +106,18 @@ def _decode_all_coolchics(parsed, device: int, decode_fn=None, frames_mine=None)
     """Pass 1 of decode_video: the Cool-chics of the frames in ``frames_mine`` (all frames by default), one
     concurrent batch (one persistent CTA per stream).  Under torch.distributed a rank only decodes the Cool-chics
     of the frames it OWNS (see decode_video_bytes)."""
-    single = decode_fn is None
     decode_fn = decode_fn or decode_coolchics
     if frames_mine is None:
         frames_mine = range(len(parsed))
     flat = [(i, name) for i in frames_mine for name in parsed[i][1]]
-    hdr = [parsed[i][1][n][0] for i, n in flat]
     cc_out: List[Dict[str, torch.Tensor]] = [dict() for _ in parsed]
     if not flat:
         return cc_out
-    args = ([hdr[k] for k in range(len(flat))], [parsed[i][1][n][1] for i, n in flat], [parsed[i][1][n][2] for i, n in flat])
-    if single:
-        fins = [_finish_request(parsed[i][0], parsed[i][1]) if n == "residue" else None for i, n in flat]
-        outs = decode_fn(*args, device=device, finish=fins)
-    else:
-        fins = [None] * len(flat)
-        outs = decode_fn(*args, device=device)
-    for k, ((i, name), o) in enumerate(zip(flat, outs)):
+    fins = [_finish_request(parsed[i][0], parsed[i][1]) if n == "residue" else None for i, n in flat]
+    outs = decode_fn([parsed[i][1][n][0] for i, n in flat], [parsed[i][1][n][1] for i, n in flat],
+                     [parsed[i][1][n][2] for i, n in flat], device=device, finish=fins)
+    for (i, name), o in zip(flat, outs):
         cc_out[i][name] = o
-        if fins[k] is not None:
-            cc_out[i]["finished"] = True
     return cc_out
 
 

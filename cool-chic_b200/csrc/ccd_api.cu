@@ -388,11 +388,11 @@ struct PreparedJob {
     bool pad_lat = false;   // latents owned by the library: every grid starts on a 16-byte boundary (TMA source)
     int64_t lat_bytes = 0;  // bytes of the latent buffer in that layout
     int nl = 0, gl[CCD_MAX_GRIDS];  // latent grids (not hyper), finest first
+    bool resized = false;   // the finest latent grid is smaller than the image: the output is computed at its size
     // float tail (plan_tail)
     bool tail = false;      // goes through the batched path
     int tail_cinp = 0, tail_C = 0;
     size_t off_tailP = 0, off_tailQ = 0, off_tailRaw = 0;  // inside the batched path's scratch
-    size_t off_rawtmp = 0;  // inside the per-stream path's scratch
     // device offsets inside the upload arena
     size_t off_words = 0, off_blob = 0, off_status = 0, off_syn = 0, off_lat = 0;
     std::vector<float> syn_f;  // dequantised synthesis weights, packed
@@ -490,6 +490,7 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
     P.nl = 0;
     for (int g = 0; g < d->n_grids; g++)
         if (!d->grid_is_hyper[g]) P.gl[P.nl++] = g;
+    P.resized = P.nl > 0 && (d->grid_h[P.gl[0]] != d->img_h || d->grid_w[P.gl[0]] != d->img_w);
     if (off >= ((int64_t)1 << 31)) return fail(CCD_ERR_UNSUPPORTED, "more than 2^31 latent symbols");
     // ---- ARM + IFCE integers
     const int dim = L.dim;
@@ -834,12 +835,22 @@ int run_synthesis(const PreparedJob &P, const int8_t *d_lat, const float *d_synw
 
 size_t synthesis_scratch_bytes(const CcdCoolChicDesc *d) { return syn_scratch_plan(d).total + 4096; }
 
+// decode_frame's frame tail (decode.py:191-206) of a job that asks for it, from its raw output at the image size: the
+// finished frame goes to the job's outputs.  (k_tail_syn finishes the full-size outputs it writes itself.)
+int finish_job(const CcdJob &job, const float *raw, cudaStream_t st) {
+    if (job.finish_bitdepth == 0) return CCD_OK;
+    const int ft = job.finish_type == 3 ? 2 : job.finish_type;  // flow: three full planes, as yuv444
+    if (ccd_finish(raw, job.desc->img_h, job.desc->img_w, job.finish_bitdepth, ft, job.d_out, job.d_out_u, job.d_out_v, st))
+        return fail(CCD_ERR_CUDA, "finish_frame launch failed");
+    return CCD_OK;
+}
+
 // ---- float tail planning -----------------------------------------------------------------------------------
 // A job takes the batched path when its upsampling uses the default kernel sizes (8 / 7), it has at least two
 // latent grids, no common randomness, and its synthesis is in the fused family.  All such jobs of a call share
 //   * one launch per cascade level (all but the last), and
-//   * one launch (per (cinp, C) pair) of the kernel that evaluates the last level, the synthesis and -- for I
-//     frames that ask for it -- the frame tail.
+//   * one launch (per (cinp, C) pair) of the kernel that evaluates the last level, the synthesis and -- for the
+//     full-size outputs of I frames that ask for it -- the frame tail.
 // Every other job takes the per-stream path (run_synthesis), one job after the other.
 bool tail_eligible(const PreparedJob &P) {
     const CcdCoolChicDesc *d = P.d;
@@ -874,7 +885,7 @@ TailScratch tail_scratch_plan(const PreparedJob &P) {
         o += al((size_t)(nl - 2) * d->grid_h[g2] * d->grid_w[g2] * 4);
     }
     const int g0 = P.gl[0];
-    if (d->grid_h[g0] != d->img_h || d->grid_w[g0] != d->img_w) {
+    if (P.resized) {
         T.raw = o;
         o += al((size_t)P.tail_C * d->grid_h[g0] * d->grid_w[g0] * 4);
     }
@@ -892,6 +903,7 @@ struct TailPlan {
     std::vector<std::pair<int, int>> lvl_jobs;  // (job, level) of every UpsLevelJob
     std::vector<LevelLaunch> levels;            // the batched path's k_ups_level_b launches
     size_t scratch_syn = 0, scratch_tail = 0;   // per-stream path (reused job after job), batched path
+    size_t scratch_fin = 0;                     // raw output for finish_job (jobs finished one after the other)
     size_t off_syn = 0, off_lvl = 0;            // job arrays in the upload arena
 };
 
@@ -909,13 +921,10 @@ void plan_tail(std::vector<PreparedJob> &P, const CcdJob *jobs, TailPlan &T) {
             T.scratch_tail += al(S.total);
             T.order.push_back(i);
         } else {
-            size_t need = synthesis_scratch_bytes(J.d);
-            if (jobs[i].finish_bitdepth != 0) {  // raw output first, then the frame tail kernel
-                J.off_rawtmp = al(need);
-                need = J.off_rawtmp + al((size_t)3 * J.d->img_h * J.d->img_w * 4);
-            }
-            T.scratch_syn = std::max(T.scratch_syn, need);
+            T.scratch_syn = std::max(T.scratch_syn, synthesis_scratch_bytes(J.d));
         }
+        if (jobs[i].finish_bitdepth != 0 && (!J.tail || J.resized))
+            T.scratch_fin = std::max(T.scratch_fin, al((size_t)3 * J.d->img_h * J.d->img_w * 4));
     }
     std::stable_sort(T.order.begin(), T.order.end(), [&](int a, int b) {
         const PreparedJob &A = P[(size_t)a], &B = P[(size_t)b];
@@ -989,7 +998,7 @@ void fill_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJo
         S.ot = N.ot;
         const size_t plane = (size_t)S.h * S.w;
         const CcdJob &job = jobs[i];
-        if (S.h != d->img_h || S.w != d->img_w) {
+        if (J.resized) {
             float *raw = reinterpret_cast<float *>(d_scr_tail + J.off_tailRaw);
             for (int c = 0; c < C; c++) S.out[c] = raw + (size_t)c * plane;
         } else if (job.finish_bitdepth != 0 && job.finish_type == 1) {
@@ -1009,9 +1018,10 @@ void fill_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJo
 }
 
 // The batched path's launches: every cascade level, then the last level + synthesis (+ frame tail) per group, then
-// the final resize of the outputs computed at a smaller size than the image (motion fields).
+// the final resize of the outputs computed at a smaller size than the image (motion fields, reduced-resolution I
+// frames), followed by the frame tail of those that ask for it.
 int launch_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJob *jobs, const unsigned char *dv,
-                const unsigned char *d_scr_tail, cudaStream_t st) {
+                const unsigned char *d_scr_tail, float *d_fin, cudaStream_t st) {
     const size_t lb = ccd_tail_level_job_bytes(), jb = ccd_tail_job_bytes();
     for (const TailPlan::LevelLaunch &LL : T.levels)
         if (ccd_tail_launch_level(dv + T.off_lvl + LL.first * lb, LL.count, LL.planes, LL.max_tw, LL.max_th, st))
@@ -1023,12 +1033,12 @@ int launch_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJ
     }
     for (int i : T.order) {
         const PreparedJob &J = P[(size_t)i];
+        if (!J.resized) continue;
         const CcdCoolChicDesc *d = J.d;
-        const int h0 = d->grid_h[J.gl[0]], w0 = d->grid_w[J.gl[0]];
-        if (h0 == d->img_h && w0 == d->img_w) continue;
-        if (jobs[i].finish_bitdepth != 0) return fail(CCD_ERR_UNSUPPORTED, "job %d: frame tail on a resized output", i);
-        const int rc = resize_output(d, reinterpret_cast<const float *>(d_scr_tail + J.off_tailRaw), J.tail_C, h0, w0,
-                                     jobs[i].d_out, st);
+        float *out = jobs[i].finish_bitdepth != 0 ? d_fin : jobs[i].d_out;
+        int rc = resize_output(d, reinterpret_cast<const float *>(d_scr_tail + J.off_tailRaw), J.tail_C,
+                               d->grid_h[J.gl[0]], d->grid_w[J.gl[0]], out, st);
+        if (!rc) rc = finish_job(jobs[i], out, st);
         if (rc) return rc;
     }
     return CCD_OK;
@@ -1213,10 +1223,11 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     int rc;
     if ((rc = ensure_pin(ctx, up))) return rc;
     if ((rc = ensure_dev(ctx->upload, up))) return rc;
-    if ((rc = ensure_dev(ctx->scratch, scratch_lat + al(T.scratch_syn) + T.scratch_tail + 4096))) return rc;
+    if ((rc = ensure_dev(ctx->scratch, scratch_lat + al(T.scratch_syn) + T.scratch_tail + T.scratch_fin + 4096))) return rc;
     unsigned char *h = ctx->h_pin, *dv = ctx->upload.p;
     unsigned char *d_scr_syn = ctx->scratch.p + scratch_lat;
     unsigned char *d_scr_tail = d_scr_syn + al(T.scratch_syn);
+    float *d_fin = reinterpret_cast<float *>(d_scr_tail + T.scratch_tail);
 
     // group jobs by kernel configuration so that each group is one launch
     std::vector<int> order((size_t)n_jobs);
@@ -1300,24 +1311,18 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     }
     CUDA_TRY(cudaEventRecord(ctx->ev[2], st));
     if (stages & 2) {
-        if ((rc = launch_tail(T, P, jobs, dv, d_scr_tail, st))) return rc;
+        if ((rc = launch_tail(T, P, jobs, dv, d_scr_tail, d_fin, st))) return rc;
         // everything else: one job after the other through the per-stream path
         for (int i = 0; i < n_jobs; i++) {
             const PreparedJob &J = P[(size_t)i];
             if (J.tail) continue;
-            const bool fin = jobs[i].finish_bitdepth != 0;
-            float *raw_dst = fin ? reinterpret_cast<float *>(d_scr_syn + J.off_rawtmp) : jobs[i].d_out;
-            rc = run_synthesis(J, d_lat[(size_t)i], reinterpret_cast<const float *>(dv + J.off_syn), raw_dst, d_scr_syn,
+            float *out = jobs[i].finish_bitdepth != 0 ? d_fin : jobs[i].d_out;
+            rc = run_synthesis(J, d_lat[(size_t)i], reinterpret_cast<const float *>(dv + J.off_syn), out, d_scr_syn,
                                T.scratch_syn, st);
+            if (!rc) rc = finish_job(jobs[i], out, st);
             if (rc) {
                 jobs[i].status = rc;
                 return rc;
-            }
-            if (fin) {
-                const int ft = jobs[i].finish_type == 3 ? 2 : jobs[i].finish_type;
-                if (ccd_finish(raw_dst, J.d->img_h, J.d->img_w, jobs[i].finish_bitdepth, ft, jobs[i].d_out, jobs[i].d_out_u,
-                               jobs[i].d_out_v, st))
-                    return fail(CCD_ERR_CUDA, "finish_frame launch failed");
             }
         }
     }

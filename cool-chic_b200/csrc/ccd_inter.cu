@@ -169,9 +169,6 @@ __device__ __forceinline__ void predict_pixel(const RefPlanes &ref, int cs, int 
         warp_pixel<N>(ref, cs, h, w, gx, gy, fx, fy, x, y, out);
 }
 
-__device__ __forceinline__ float quantf(float v, float M) { return __fdiv_rn(rintf(__fmul_rn(M, v)), M); }
-__device__ __forceinline__ float clamp01f(float v) { return v < 0.0f ? 0.0f : (v > 1.0f ? 1.0f : v); }
-
 // One thread per pixel; a warp covers a 16 x 2 patch (lane = lx + 16 ly), so that the 2 x 2 chroma blocks of a
 // 4:2:0 frame sit inside one warp and the frame tail of decode_frame (bitstream/decode.py:191-206: round ->
 // 2 x 2 average of U, V -> clamp -> round) is done with four shuffles instead of a second pass over HBM.
@@ -194,9 +191,9 @@ __global__ void __launch_bounds__(128)
     if (is_b) {
         predict_pixel<N>(ref1, ref_cs, h, w, g1x, g1y, motion[2 * plane + i], motion[3 * plane + i], x, y, p1);
         beta = __fadd_rn(residue[4 * plane + i], 0.5f);
-        beta = clamp01f(beta);
+        beta = clamp01(beta);
     }
-    float alpha = clamp01f(__fadd_rn(residue[3 * plane + i], 0.5f));
+    float alpha = clamp01(__fadd_rn(residue[3 * plane + i], 0.5f));
     float v[3];
 #pragma unroll
     for (int c = 0; c < 3; c++) {
@@ -213,15 +210,15 @@ __global__ void __launch_bounds__(128)
         return;
     }
 #pragma unroll
-    for (int c = 0; c < 3; c++) v[c] = quantf(v[c], M);
+    for (int c = 0; c < 3; c++) v[c] = quant(v[c], M);
     if (!out_420) {
         if (inside) {
 #pragma unroll
-            for (int c = 0; c < 3; c++) outp[c][i] = quantf(clamp01f(v[c]), M);
+            for (int c = 0; c < 3; c++) outp[c][i] = quant(clamp01(v[c]), M);
         }
         return;
     }
-    if (inside) o0[i] = quantf(clamp01f(v[0]), M);
+    if (inside) o0[i] = quant(clamp01(v[0]), M);
     // 2 x 2 average of the rounded chroma samples, in the order of F.avg_pool2d's reference loop (yuv.py:295)
     const int base = lane & ~17;
 #pragma unroll
@@ -232,7 +229,7 @@ __global__ void __launch_bounds__(128)
         s = __fadd_rn(s, __shfl_sync(0xffffffffu, v[c], base + 16));
         s = __fadd_rn(s, __shfl_sync(0xffffffffu, v[c], base + 17));
         if (lane == base && px + 1 < w && py + 1 < h)
-            outp[c][(size_t)(py >> 1) * (w >> 1) + (px >> 1)] = quantf(clamp01f(__fdiv_rn(s, 4.0f)), M);
+            outp[c][(size_t)(py >> 1) * (w >> 1) + (px >> 1)] = quant(clamp01(__fdiv_rn(s, 4.0f)), M);
     }
 }
 

@@ -155,6 +155,10 @@ int ccd_resize_torch(const float *d_in, int c, int h, int w, float *d_out, int H
 int ccd_cr_noise(float *d_out, size_t first, size_t n, cudaStream_t st);
 int ccd_finish(const float *d_in, int h, int w, int bitdepth, int data_type, float *a, float *b, float *c,
                cudaStream_t st);
+// The sample operations of decode_frame's frame tail (bitstream/decode.py:191-206), for k_finish_*, the epilogue of
+// k_tail_syn and that of k_inter_predict: round to the k / M grid (M = 2^bitdepth - 1), clamp to [0, 1].
+static __device__ __forceinline__ float quant(float v, float M) { return __fdiv_rn(rintf(__fmul_rn(M, v)), M); }
+static __device__ __forceinline__ float clamp01(float v) { return v < 0.0f ? 0.0f : (v > 1.0f ? 1.0f : v); }
 
 int ccd_pack(const float *const planes[3], int h, int w, int cs, int bitdepth, int sample_bytes, int interleaved,
              void *d_out, cudaStream_t st);

@@ -541,9 +541,6 @@ __host__ __device__ inline int ts_lh(int n3) { return SF_TH + 2 * n3 + 6; }
 __host__ __device__ inline int ts_sw(int n3) { return ((SF_TW + 2 * n3) / 2 + 5 + 3 + 3) & ~3; }
 __host__ __device__ inline int ts_sh(int n3) { return (SF_TH + 2 * n3) / 2 + 5; }
 
-__device__ __forceinline__ float quant(float v, float M);
-__device__ __forceinline__ float clamp01(float v);
-
 // ---------------------------------------------------------------------------------------------------------------
 // k_tail_syn (see the top of this section), laid out for instruction efficiency:
 //   * the halo of the stage-A region is rounded up to an even number of pixels, so that the region starts on even
@@ -1126,9 +1123,6 @@ __global__ void k_cr_noise(float *__restrict__ out, size_t first, size_t n) {
     // Box-Muller (noise.py:28-34) with the canonical log / cos of ccd_detmath.h: bit-identical to the oracle
     out[i] = (float)__dmul_rn(__dsqrt_rn(__dmul_rn(-2.0, ccdm_log(u1))), ccdm_cos(__dmul_rn(2 * 3.14159265359, u2)));
 }
-
-__device__ __forceinline__ float quant(float v, float M) { return __fdiv_rn(rintf(__fmul_rn(M, v)), M); }
-__device__ __forceinline__ float clamp01(float v) { return v < 0.0f ? 0.0f : (v > 1.0f ? 1.0f : v); }
 
 __global__ void k_finish_444(const float *__restrict__ in, size_t n, float M, float *__restrict__ out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

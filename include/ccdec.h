@@ -99,10 +99,11 @@ int64_t ccd_decode_nn(const CcdCoolChicDesc *desc, const uint8_t *nn_bytes, size
  * output (un-clamped, un-rounded -- what encode_decode_coolchic returns).  d_latents
  * (optional, may be NULL): int8 decoded latents in decode order (coarsest grid first, each
  * grid row-major).  status (out): per-job status written on completion.
- * Frame tail (optional, the Cool-chic of an I frame): finish_bitdepth != 0 asks for decode_frame's
- * round / (4:2:0 average) / clamp / round (bitstream/decode.py:191-206) fused into the synthesis
- * kernel's epilogue: d_out then receives the FINISHED frame -- [3][H][W] for finish_type 0 (rgb),
- * 2 (yuv444), 3 (flow); for finish_type 1 (yuv420) d_out = y [H][W], d_out_u, d_out_v [H/2][W/2]. */
+ * Frame tail (optional, the Cool-chic of an I frame, 3 output channels): finish_bitdepth != 0 asks
+ * for decode_frame's round / (4:2:0 average) / clamp / round (bitstream/decode.py:191-206), applied
+ * by the library -- fused into the synthesis kernel's epilogue where the batched path takes the job:
+ * d_out then receives the FINISHED frame -- [3][H][W] for finish_type 0 (rgb), 2 (yuv444),
+ * 3 (flow); for finish_type 1 (yuv420) d_out = y [H][W], d_out_u, d_out_v [H/2][W/2]. */
 typedef struct CcdJob {
     const CcdCoolChicDesc *desc;
     const uint8_t *nn_bytes;

@@ -77,7 +77,7 @@ def _gop_worker(rank, world, port, ret):
     data = broadcast_byte_strings([data] if rank == 0 else None, src=0)[0]
     decoded_here = []
 
-    def fake_decode(headers, nn, lat, device=0):
+    def fake_decode(headers, nn, lat, device=0, finish=None):
         outs = []
         for h, b in zip(headers, lat):
             decoded_here.append(len(b))
@@ -116,7 +116,7 @@ def test_gop_frames_are_owned_and_exchanged():
     data = open(os.path.join(ROOT, "tests", "golden", "gop5_64x96_yuv420.cool"), "rb").read()
     all_lens = []
 
-    def fake_decode(headers, nn, lat, device=0):
+    def fake_decode(headers, nn, lat, device=0, finish=None):
         all_lens.extend(len(b) for b in lat)
         return [torch.full(dec.output_shape(h), float(len(b) % 251), dtype=torch.float32) for h, b in zip(headers, lat)]
 

@@ -621,6 +621,10 @@ _FIVE_LAYERS = _syn("48-1-linear-relu", "3-1-linear-none", "3-3-residual-relu", 
     pytest.param((48, 80), (2, 5), "nearest", _syn("16-1-linear-relu", "2-1-linear-none"), None, 1 + 2 + 1 + 1,
                  id="motion_2ch_no_3x3_resize"),
     pytest.param((17, 9), (0, 2), None, None, None, 1 + 1 + 1, id="smaller_than_one_tile"),
+    # reduced latent resolution: k_tail_syn writes the raw output, the final resize, then ccd_finish (k_finish_444, and
+    # k_finish_420_uv for 4:2:0)
+    pytest.param((50, 70), (1, 5), "bicubic", None, (8, "rgb"), 1 + 3 + 1 + 1 + 1, id="resized_finish_rgb"),
+    pytest.param((44, 60), (1, 5), "bilinear", None, (10, "yuv420"), 1 + 3 + 1 + 1 + 2, id="resized_finish_yuv420"),
     # per-stream path
     # k_ups_first, k_ups_level per level, k_cr_noise + 3 noise resizes, k_syn_fused (8 inputs, stabiliser on 4)
     pytest.param((40, 56), (0, 3), None, {"flag_common_randomness": 1}, None, 1 + 1 + 3 + 1 + 3 + 1,
@@ -659,12 +663,13 @@ def test_synthesis_paths_vs_oracle(ctx, oracle, seed_stream, size, lat, fin_ups,
     nn = oracle.decode_nn(d, nnb)
     lat_o, _ = oracle.decode_latents(d, nn, lb)
     want = oracle.synthesize(d, nn, lat_o)
-    if finish is None:
-        assert np.array_equal(out[0][0].cpu().numpy(), want)
-    else:
+    if finish is not None:
         want = oracle.finish_frame(want, *finish)
+    if isinstance(want, dict):
         for k in "yuv":
             assert np.array_equal(out[0][k][0, 0].cpu().numpy(), want[k]), k
+    else:
+        assert np.array_equal(out[0][0].cpu().numpy(), want)
 
 
 def test_corrupt_streams_fail_cleanly_on_the_device(ctx, seed_stream):

@@ -29,7 +29,7 @@ EXPORTS = [
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
     "ccd_synthesize", "ccd_encode_latents", "ccd_finish_frame", "ccd_inter_predict", "ccd_reconstruct_frame",
     "ccd_pack_frame",
-    "ccd_pack_samples",
+    "ccd_pack_samples", "ccd_latent_rate",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
 ]
 
@@ -48,6 +48,21 @@ class CcdJob(ctypes.Structure):
         ("finish_type", ctypes.c_int32),
         ("d_out_u", ctypes.c_void_p),
         ("d_out_v", ctypes.c_void_p),
+    ]
+
+
+class CcdRateJob(ctypes.Structure):
+    _fields_ = [
+        ("desc", ctypes.POINTER(CcdCoolChicDesc)),
+        ("nn_ints", ctypes.c_void_p),
+        ("d_latents", ctypes.c_void_p),
+        ("d_bits", ctypes.c_void_p),
+        ("d_freq", ctypes.c_void_p),
+        ("d_mu_sc", ctypes.c_void_p),
+        ("d_spatial", ctypes.c_void_p),
+        ("grid_bits", ctypes.c_double * CCD_MAX_GRIDS),
+        ("bad_index", ctypes.c_int64),
+        ("status", ctypes.c_int32),
     ]
 
 
@@ -109,6 +124,8 @@ def load_library():
         L.ccd_pack_frame.argtypes = [vp, vp, ci, ci, ci, ci, ci, ci, vp, vp]
         L.ccd_pack_samples.restype = ci
         L.ccd_pack_samples.argtypes = [vp, vp, ctypes.c_size_t, ci, ci, vp, vp]
+        L.ccd_latent_rate.restype = ci
+        L.ccd_latent_rate.argtypes = [vp, ctypes.POINTER(CcdRateJob), ci, vp]
         L.ccd_debug_laplace_domain.restype = ci
         L.ccd_debug_laplace_domain.argtypes = [vp, ci, ci, vp, vp]
         L.ccd_debug_last_status.restype = ci
@@ -429,6 +446,50 @@ class Context:
         _check(self._lib.ccd_pack_samples(self._h, ctypes.c_void_p(base), total, int(bitdepth), sample_bytes, out.data_ptr(),
                                           self._stream()))
         return out
+
+    def latent_rate(self, descs: Sequence[CcdCoolChicDesc], nn_ints: Sequence[np.ndarray],
+                    latents: Sequence[torch.Tensor], want_freq: bool = False, want_mu_sc: bool = False,
+                    want_spatial: bool = False) -> List[dict]:
+        """Rate of decoded latents (``ccd_latent_rate``): one kernel launch for all Cool-chics, plus one for the
+        spatial maps.  ``latents[i]``: int8 CUDA tensor in decode order (what ``decode_many(want_latents=True)``
+        returns).  Per Cool-chic a dict with ``bits`` (float32 CUDA [n_symbols], decode order), ``grid_bits``
+        (list of f64, grid 0 = finest), and on request ``freq`` / ``mu_sc`` (int32 CUDA holding the uint32
+        values) and ``spatial`` ([1, 1, H, W] float32 CUDA)."""
+        n = len(descs)
+        jobs = (CcdRateJob * n)()
+        keep, res = [], []
+        dev = self.torch_device
+        for i in range(n):
+            d = descs[i]
+            nn = np.ascontiguousarray(nn_ints[i], dtype=np.int64)
+            lat = latents[i]
+            if not (lat.is_cuda and lat.dtype == torch.int8 and lat.is_contiguous() and lat.numel() == d.n_symbols()):
+                raise ValueError(f"latents[{i}] must be a contiguous int8 CUDA tensor of {d.n_symbols()} symbols")
+            r = {"bits": torch.empty((d.n_symbols(),), dtype=torch.float32, device=dev)}
+            if want_freq:
+                r["freq"] = torch.empty((d.n_symbols(),), dtype=torch.int32, device=dev)
+            if want_mu_sc:
+                r["mu_sc"] = torch.empty((d.n_symbols(),), dtype=torch.int32, device=dev)
+            if want_spatial:
+                r["spatial"] = torch.empty((1, 1, d.img_h, d.img_w), dtype=torch.float32, device=dev)
+            keep += [nn, lat]
+            jobs[i].desc = ctypes.pointer(d)
+            jobs[i].nn_ints = nn.ctypes.data
+            jobs[i].d_latents = lat.data_ptr()
+            jobs[i].d_bits = r["bits"].data_ptr()
+            jobs[i].d_freq = r["freq"].data_ptr() if want_freq else None
+            jobs[i].d_mu_sc = r["mu_sc"].data_ptr() if want_mu_sc else None
+            jobs[i].d_spatial = r["spatial"].data_ptr() if want_spatial else None
+            res.append(r)
+        rc = self._lib.ccd_latent_rate(self._h, jobs, n, self._stream())
+        if rc != CCD_OK:
+            msg = self._lib.ccd_last_error(None)
+            err = CcdError(rc, msg.decode() if msg else "")
+            err.bad_index = [int(jobs[i].bad_index) for i in range(n)]
+            raise err
+        for i in range(n):
+            res[i]["grid_bits"] = [float(jobs[i].grid_bits[g]) for g in range(descs[i].n_grids)]
+        return res
 
     def last_timing(self):
         ms = (ctypes.c_float * 4)()

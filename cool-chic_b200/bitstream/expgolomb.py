@@ -28,6 +28,16 @@ def encode_exp_golomb(data: Sequence[int], count: Sequence[int]) -> Tuple[bytes,
     return acc.to_bytes((n_bits + pad) // 8, "big"), pad
 
 
+def exp_golomb_bits(data: Sequence[int], count: Sequence[int]) -> List[int]:
+    """Length in bits of the exp-Golomb(k) codeword of each integer (the ``total`` of encode_exp_golomb)."""
+    out = []
+    for x, k in zip(data, count):
+        x = int(x)
+        u = -2 * x if x <= 0 else 2 * x - 1
+        out.append(2 * (u + (1 << k)).bit_length() - 1 - k)
+    return out
+
+
 def decode_exp_golomb(data_bytes: bytes, n_padding_bits: int, count: Sequence[int]) -> List[int]:
     if isinstance(n_padding_bits, float):
         raise TypeError(f"n_padding_bits must be an int. Found n_padding_bits={n_padding_bits}")

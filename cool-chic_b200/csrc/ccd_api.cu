@@ -1392,6 +1392,144 @@ int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
     return CCD_OK;
 }
 
+static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaStream_t st) {
+    std::vector<PreparedJob> P((size_t)n_jobs);
+    std::vector<RateTile> tiles;
+    // tiles of job i, decode-order grid gi: [tile_at[i][gi], tile_at[i][gi + 1])
+    std::vector<std::vector<size_t>> tile_at((size_t)n_jobs);
+    std::vector<size_t> off_blob((size_t)n_jobs), off_es((size_t)n_jobs), off_bad((size_t)n_jobs);
+    std::vector<RateSpatialDev> sp;
+    int64_t max_pixels = 0;
+    size_t up = 0, smem = 0;
+    for (int i = 0; i < n_jobs; i++) {
+        CcdRateJob &R = jobs[i];
+        R.status = CCD_OK;
+        R.bad_index = -1;
+        if (!R.desc || !R.nn_ints || !R.d_latents || !R.d_bits) return R.status = fail(CCD_ERR_ARG, "job %d: null pointer", i);
+        PreparedJob &J = P[(size_t)i];
+        J.d = R.desc;
+        int rc = prepare_job(J, R.nn_ints);  // the decoder's build_arm / pack_arm / pack_ifce and fast-path choice
+        if (rc) return R.status = rc;
+        off_blob[(size_t)i] = up;
+        up += al(J.blob.size());
+        off_es[(size_t)i] = up;
+        up += al(sizeof(EntStream));
+        off_bad[(size_t)i] = up;
+        up += al(8);
+        smem = std::max(smem, ccd_rate_smem_bytes(J.es.arm_blob_bytes, J.es.ifce_blob_max));
+        const CcdCoolChicDesc *d = J.d;
+        tile_at[(size_t)i].push_back(tiles.size());
+        for (int gi = 0; gi < d->n_grids; gi++) {
+            const EntGrid &G = J.es.grid[gi];
+            for (int y0 = 0; y0 < G.h; y0 += CCD_RATE_TH)
+                for (int x0 = 0; x0 < G.w; x0 += CCD_RATE_TW) tiles.push_back(RateTile{i, gi, y0, x0});
+            tile_at[(size_t)i].push_back(tiles.size());
+        }
+        if (R.d_spatial) {
+            RateSpatialDev S;
+            memset(&S, 0, sizeof(S));
+            S.bits = R.d_bits;
+            S.out = R.d_spatial;
+            S.H = d->img_h;
+            S.W = d->img_w;
+            S.n_grids = d->n_grids;
+            for (int g = 0; g < d->n_grids; g++) {
+                S.h[g] = d->grid_h[g];
+                S.w[g] = d->grid_w[g];
+                S.off[g] = J.lat_off_by_grid[g];
+                S.ratio[g] = (float)(((double)d->img_h * d->img_w) / ((double)d->grid_h[g] * d->grid_w[g]));
+                S.sy[g] = (float)d->grid_h[g] / (float)d->img_h;
+                S.sx[g] = (float)d->grid_w[g] / (float)d->img_w;
+            }
+            sp.push_back(S);
+            max_pixels = std::max(max_pixels, (int64_t)d->img_h * d->img_w);
+        }
+    }
+    if (tiles.size() > (size_t)INT32_MAX) return fail(CCD_ERR_UNSUPPORTED, "too many rate tiles");
+    if (smem > 227 * 1024) return fail(CCD_ERR_UNSUPPORTED, "rate pass needs %zu bytes of shared memory", smem);
+    const size_t off_jobs = up;
+    up += al(sizeof(RateJobDev) * (size_t)n_jobs);
+    const size_t off_tiles = up;
+    up += al(sizeof(RateTile) * tiles.size());
+    const size_t off_sp = up;
+    up += al(sizeof(RateSpatialDev) * sp.size());
+    const size_t off_part = up;
+    up += al(sizeof(double) * tiles.size());
+    int rc;
+    if ((rc = ensure_pin(ctx, up))) return rc;
+    if ((rc = ensure_dev(ctx->upload, up))) return rc;
+    unsigned char *h = ctx->h_pin, *dv = ctx->upload.p;
+    for (int i = 0; i < n_jobs; i++) {
+        PreparedJob &J = P[(size_t)i];
+        memcpy(h + off_blob[(size_t)i], J.blob.data(), J.blob.size());
+        J.es.latents = const_cast<int8_t *>(jobs[i].d_latents);
+        J.es.blob = dv + off_blob[(size_t)i];
+        memcpy(h + off_es[(size_t)i], &J.es, sizeof(EntStream));
+        memset(h + off_bad[(size_t)i], 0xff, 8);
+        RateJobDev D;
+        D.es = reinterpret_cast<const EntStream *>(dv + off_es[(size_t)i]);
+        D.bits = jobs[i].d_bits;
+        D.freq = jobs[i].d_freq;
+        D.mu_sc = jobs[i].d_mu_sc;
+        D.bad = reinterpret_cast<unsigned long long *>(dv + off_bad[(size_t)i]);
+        D.kind = ccd_rate_kind(J.d->n_ctx, J.es.cf, J.fast);
+        memcpy(h + off_jobs + sizeof(RateJobDev) * (size_t)i, &D, sizeof(D));
+    }
+    memcpy(h + off_tiles, tiles.data(), sizeof(RateTile) * tiles.size());
+    if (!sp.empty()) memcpy(h + off_sp, sp.data(), sizeof(RateSpatialDev) * sp.size());
+    CUDA_TRY(cudaMemcpyAsync(dv, h, off_part, cudaMemcpyHostToDevice, st));
+    double *d_part = reinterpret_cast<double *>(dv + off_part);
+    int e = ccd_rate_launch(reinterpret_cast<const RateTile *>(dv + off_tiles), (int)tiles.size(),
+                            reinterpret_cast<const RateJobDev *>(dv + off_jobs), smem, ctx->d_cdf, ctx->d_scale, d_part, st);
+    if (e != 0) return fail(CCD_ERR_CUDA, "rate kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    if (!sp.empty()) {
+        e = ccd_rate_spatial_launch(reinterpret_cast<const RateSpatialDev *>(dv + off_sp), (int)sp.size(), max_pixels, st);
+        if (e != 0) return fail(CCD_ERR_CUDA, "spatial rate launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    }
+    CUDA_TRY(cudaMemcpyAsync(h + off_part, d_part, sizeof(double) * tiles.size(), cudaMemcpyDeviceToHost, st));
+    for (int i = 0; i < n_jobs; i++) CUDA_TRY(cudaMemcpyAsync(h + off_bad[(size_t)i], dv + off_bad[(size_t)i], 8, cudaMemcpyDeviceToHost, st));
+    cudaError_t se = cudaStreamSynchronize(st);
+    if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "rate kernel execution failed: %s", cudaGetErrorString(se));
+    const double *part = reinterpret_cast<const double *>(h + off_part);
+    int first = CCD_OK;
+    for (int i = 0; i < n_jobs; i++) {
+        CcdRateJob &R = jobs[i];
+        const int n_grids = P[(size_t)i].d->n_grids;
+        for (int g = 0; g < CCD_MAX_GRIDS; g++) R.grid_bits[g] = 0.0;
+        for (int gi = 0; gi < n_grids; gi++) {
+            double s = 0.0;  // tiles in order: a fixed-order sum
+            for (size_t t = tile_at[(size_t)i][(size_t)gi]; t < tile_at[(size_t)i][(size_t)gi + 1]; t++) s += part[t];
+            R.grid_bits[n_grids - 1 - gi] = s;
+        }
+        unsigned long long bad;
+        memcpy(&bad, h + off_bad[(size_t)i], 8);
+        if (bad != ~0ull) {
+            R.bad_index = (int64_t)bad;
+            R.status = CCD_ERR_ARG;
+            if (!first) first = fail(CCD_ERR_ARG, "job %d: latent %lld is outside [-64, 63]", i, (long long)bad);
+        }
+    }
+    return first;
+}
+
+int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_stream) {
+    if (!ctx) return fail(CCD_ERR_ARG, "null context");
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
+    if (n_jobs == 0) return CCD_OK;
+    DeviceGuard guard(ctx->device);
+    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const int rc = latent_rate_body(ctx, jobs, n_jobs, st);
+    if (rc != CCD_OK) {
+        // leave the context quiescent: the staging buffers may be reused by the next call
+        const std::string keep = g_err;
+        cudaStreamSynchronize(st);
+        cudaGetLastError();
+        g_err = keep;
+    }
+    return rc;
+}
+
 int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitdepth, int data_type, float *d_out_a,
                      float *d_out_b, float *d_out_c, void *cuda_stream) {
     if (!ctx || !d_in || !d_out_a || h < 1 || w < 1 || bitdepth < 8 || bitdepth > 16 || data_type < 0 || data_type > 2)

@@ -1396,6 +1396,168 @@ int launch_t(const EntStream *d_streams, int n, size_t smem, int threads, const 
     return (int)cudaGetLastError();
 }
 
+// =======================================================================================
+// Rate pass: k_latent_rate evaluates the ARM of every decoded symbol again -- with the decoder's own QuadArm /
+// GenericArm on the same row-ring layout, fed from a staged tile instead of the wavefront -- and turns the
+// symbol's cumulative window into freq = left(s+1) - left(s) and bits = 24 - log2(freq).
+// =======================================================================================
+// One symbol: clamp (latent.py:165, rangecoder.py:89-91), then the exact interval the range coder used: the
+// table window for s_lo <= s < s_lo + 31 (what the coder reads), the f64 model outside it.  Returns the f64 bits.
+__device__ __forceinline__ double rate_symbol(long long o0, long long o1, int sym, long long idx, const RateJobDev &J,
+                                              const uint32_t *__restrict__ cdf, const float *__restrict__ scale_tab) {
+    long long im = o0 + 16384, is = o1 + 1280;
+    im = im < 0 ? 0 : (im > 32767 ? 32767 : im);
+    is = is < 0 ? 0 : (is > 2560 ? 2560 : is);
+    const int mu_idx = (int)im, sc_idx = (int)is;
+    if (sym < kSymMin || sym > kSymMax) {
+        atomicMin(J.bad, (unsigned long long)idx);
+        return 0.0;
+    }
+    const int mu_int = ((mu_idx + 128) >> 8) - 64;
+    const int fr = (mu_idx + 128) & 255;
+    const int t = sym - (mu_int - CCD_WIN_HALF);
+    uint32_t l0, l1;
+    if (t >= 0 && t < CCD_WIN - 1) {
+        const uint32_t *row = cdf + (((size_t)sc_idx << 8 | (size_t)fr) << 5);
+        l0 = fix_left(__ldg(row + t), sym);
+        l1 = fix_left(__ldg(row + t + 1), sym + 1);
+    } else {
+        const double mu = (double)(mu_idx - 16384) * (1.0 / 256.0);
+        const double b = (double)scale_tab[sc_idx];
+        l0 = laplace_left_exact(sym, mu, b);
+        l1 = laplace_left_exact(sym + 1, mu, b);
+    }
+    const uint32_t freq = l1 - l0;
+    const double bits = 24.0 - log2((double)freq);
+    J.bits[idx] = (float)bits;
+    if (J.freq) J.freq[idx] = freq;
+    if (J.mu_sc) J.mu_sc[idx] = (uint32_t)mu_idx | ((uint32_t)sc_idx << 16);
+    return bits;
+}
+
+// One tile: rows y0-4 .. y0+nr-1 and columns x0-4 .. x0+59 of the grid are staged in the 32 x 64 row ring (the
+// causal neighbourhood is dy -4..0, dx -4..4), then every symbol of the tile is evaluated.  FAST: a quad of lanes
+// per symbol (64 symbols per pass of the CTA), GENERIC: a thread per symbol.
+template <int NCTX, int CF, bool FAST>
+__device__ __forceinline__ void rate_tile(const RateTile &t, const RateJobDev &J, unsigned char *smem,
+                                          const uint32_t *__restrict__ cdf, const float *__restrict__ scale_tab,
+                                          double *__restrict__ part) {
+    const EntStream &G = *J.es;
+    const EntGrid &Gg = G.grid[t.grid];
+    const int tid = threadIdx.x, nthr = blockDim.x;
+    EntGrid *g = reinterpret_cast<EntGrid *>(smem);
+    unsigned char *arm = smem + align16(sizeof(EntGrid));
+    unsigned char *ifce = arm + align16((size_t)G.arm_blob_bytes);
+    const uint32_t rows = (uint32_t)__cvta_generic_to_shared(ifce + align16((size_t)G.ifce_blob_max));
+    const int8_t *lat = G.latents;
+    const int h = Gg.h, w = Gg.w, n_hidden = G.n_hidden;
+    const long long base = Gg.lat_off;
+    {
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(&Gg);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(g);
+        for (int i = tid; i < (int)(sizeof(EntGrid) / 4); i += nthr) dst[i] = src[i];
+        for (int i = tid * 4; i < G.arm_blob_bytes; i += nthr * 4)
+            *reinterpret_cast<uint32_t *>(arm + i) = *reinterpret_cast<const uint32_t *>(G.blob + i);
+        for (int i = tid * 4; i < Gg.ifce_blob_bytes; i += nthr * 4)
+            *reinterpret_cast<uint32_t *>(ifce + i) = *reinterpret_cast<const uint32_t *>(G.blob + Gg.ifce_blob_off + i);
+    }
+    const int nr = min(CCD_RATE_TH, h - t.y0), nc = min(CCD_RATE_TW, w - t.x0);
+    for (int i = tid; i < (nr + 4) * CCD_ROW_COLS; i += nthr) {
+        const int yy = t.y0 - 4 + (i >> 6), xx = t.x0 - 4 + (i & (CCD_ROW_COLS - 1));
+        int v = 0;
+        if (yy >= 0 && xx >= 0 && xx < w) v = lat[base + (long long)yy * w + xx];
+        sts_u8(rows + ((((uint32_t)yy & (CCD_RATE_ROWS - 1)) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))), v);
+    }
+    __syncthreads();
+    const uint32_t row_mask = CCD_RATE_ROWS - 1;
+    const int n = nr * nc;
+    double acc = 0.0;
+    if constexpr (FAST) {
+        const int member = tid & 3;
+        for (int s0 = 0; s0 < n; s0 += nthr >> 2) {
+            // uniform trip count: every lane of a warp takes part in the quad shuffles
+            const int s = s0 + (tid >> 2);
+            const bool valid = s < n;
+            const int ty = valid ? s / nc : 0, tx = valid ? s - ty * nc : 0;
+            const int y = t.y0 + ty, x = t.x0 + tx;
+            int ifv[CCD_IFCE_FAST_MAX];
+            QuadArm<NCTX, CF>::ifce_prefetch(g, lat, y, x, member, ifv);
+            long long o0, o1;
+            QuadArm<NCTX, CF>::run(g, arm, ifce, ifv, rows, row_mask, n_hidden, y, x, member, o0, o1);
+            if (valid && member == 0) {
+                const int sym = lds_s8(rows + (((uint32_t)y & row_mask) << 6 | ((uint32_t)x & (CCD_ROW_COLS - 1))));
+                acc += rate_symbol(o0, o1, sym, base + (long long)y * w + x, J, cdf, scale_tab);
+            }
+        }
+    } else {
+        const int n_ctx = G.n_ctx, cf = G.cf;
+        for (int s = tid; s < n; s += nthr) {
+            const int ty = s / nc, tx = s - ty * nc;
+            const int y = t.y0 + ty, x = t.x0 + tx;
+            long long xin[CCD_MAX_DIM];
+            for (int c = 0; c < n_ctx; c++) {
+                const int yy = y + c_ctx_dy[c], xx = x + c_ctx_dx[c];
+                int v = 0;
+                if (yy >= 0 && xx >= 0 && xx < w)
+                    v = lds_s8(rows + ((((uint32_t)yy & row_mask) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))));
+                xin[c] = v;
+            }
+            if (cf > 0) GenericArm::ifce(g, ifce, lat, cf, y >> 1, x >> 1, xin + n_ctx);
+            long long o0, o1;
+            GenericArm::arm(arm, n_ctx + cf, n_hidden, xin, o0, o1);
+            const int sym = lds_s8(rows + (((uint32_t)y & row_mask) << 6 | ((uint32_t)x & (CCD_ROW_COLS - 1))));
+            acc += rate_symbol(o0, o1, sym, base + (long long)y * w + x, J, cdf, scale_tab);
+        }
+    }
+    // fixed-order reduction: lanes (butterfly), then the warps in order -- the same sum on every run
+    __shared__ double wsum[CCD_RATE_THREADS / 32];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
+    if ((tid & 31) == 0) wsum[tid >> 5] = acc;
+    __syncthreads();
+    if (tid == 0) {
+        double s = 0.0;
+        for (int i = 0; i < (nthr >> 5); i++) s += wsum[i];
+        part[blockIdx.x] = s;
+    }
+}
+
+// ONE launch for every grid of every job; the ARM variant is chosen per CTA (uniform branch).
+__global__ void __launch_bounds__(CCD_RATE_THREADS)
+    k_latent_rate(const RateTile *__restrict__ tiles, const RateJobDev *__restrict__ jobs, const uint32_t *__restrict__ cdf,
+                  const float *__restrict__ scale_tab, double *__restrict__ part) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const RateTile t = tiles[blockIdx.x];
+    const RateJobDev &J = jobs[t.job];
+    switch (J.kind) {
+        case 0: rate_tile<6, 2, true>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 1: rate_tile<10, 2, true>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 2: rate_tile<10, 4, true>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 3: rate_tile<14, 6, true>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 4: rate_tile<20, 6, true>(t, J, smem_raw, cdf, scale_tab, part); break;
+        default: rate_tile<0, 0, false>(t, J, smem_raw, cdf, scale_tab, part); break;
+    }
+}
+
+// Spatial rate map (training/test.py:217-235 in a canonical order): per pixel, acc = 0, then for every grid,
+// finest first, acc += bits[nearest(y), nearest(x)] / ((H*W) / (h*w)), all in fp32.  blockIdx.y = job.
+__global__ void k_rate_spatial(const RateSpatialDev *__restrict__ jobs) {
+    const RateSpatialDev &J = jobs[blockIdx.y];
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= (long long)J.H * J.W) return;
+    const int Y = (int)(p / J.W), X = (int)(p - (long long)Y * J.W);
+    float acc = 0.0f;
+    for (int g = 0; g < J.n_grids; g++) {
+        // F.interpolate(mode="nearest") index, as k_resize_nearest
+        int yy = (int)floorf(__fmul_rn((float)Y, J.sy[g]));
+        int xx = (int)floorf(__fmul_rn((float)X, J.sx[g]));
+        yy = yy > J.h[g] - 1 ? J.h[g] - 1 : yy;
+        xx = xx > J.w[g] - 1 ? J.w[g] - 1 : xx;
+        acc = __fadd_rn(acc, __fdiv_rn(J.bits[J.off[g] + (long long)yy * J.w[g] + xx], J.ratio[g]));
+    }
+    J.out[p] = acc;
+}
+
 }  // namespace
 
 unsigned long long g_ccd_launches = 0;
@@ -1434,5 +1596,37 @@ int ccd_laplace_domain(const float *d_scale, int sc_lo, int sc_hi, uint32_t *d_l
                        cudaStream_t st) {
     size_t total = (size_t)(sc_hi - sc_lo) * 32641;
     k_laplace_domain<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(d_scale, sc_lo, sc_hi, d_lo, d_hi);
+    return (int)cudaGetLastError();
+}
+
+int ccd_rate_kind(int n_ctx, int cf, bool fast) {
+    if (fast) {
+        if (n_ctx == 6 && cf == 2) return 0;
+        if (n_ctx == 10 && cf == 2) return 1;
+        if (n_ctx == 10 && cf == 4) return 2;
+        if (n_ctx == 14 && cf == 6) return 3;
+        if (n_ctx == 20 && cf == 6) return 4;
+    }
+    return 5;
+}
+
+size_t ccd_rate_smem_bytes(int arm_blob_bytes, int ifce_blob_max) {
+    return align16(sizeof(EntGrid)) + align16((size_t)arm_blob_bytes) + align16((size_t)ifce_blob_max) +
+           (size_t)CCD_RATE_ROWS * CCD_ROW_COLS;
+}
+
+int ccd_rate_launch(const RateTile *d_tiles, int n_tiles, const RateJobDev *d_jobs, size_t smem, const uint32_t *d_cdf,
+                    const float *d_scale, double *d_part, cudaStream_t st) {
+    cudaError_t e = cudaFuncSetAttribute(k_latent_rate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    k_latent_rate<<<n_tiles, CCD_RATE_THREADS, smem, st>>>(d_tiles, d_jobs, d_cdf, d_scale, d_part);
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
+
+int ccd_rate_spatial_launch(const RateSpatialDev *d_jobs, int n_jobs, int64_t max_pixels, cudaStream_t st) {
+    const dim3 grid((unsigned)((max_pixels + 255) / 256), (unsigned)n_jobs);
+    k_rate_spatial<<<grid, 256, 0, st>>>(d_jobs);
+    g_ccd_launches++;
     return (int)cudaGetLastError();
 }

@@ -92,6 +92,44 @@ int ccd_laplace_domain(const float *d_scale, int sc_lo, int sc_hi, uint32_t *d_l
                        cudaStream_t st);
 
 // --------------------------------------------------------------------------------------
+// Rate pass (ccd_entropy.cu, after the entropy kernel): the information content of every decoded latent under the
+// model the range coder used.  All latents are known, so every symbol's context is known: no wavefront, one CTA
+// per tile of CCD_RATE_TH x CCD_RATE_TW symbols of one grid of one job, all jobs in one launch.
+// --------------------------------------------------------------------------------------
+#define CCD_RATE_THREADS 256
+#define CCD_RATE_TH 28               // tile rows; + 4 causal halo rows = the 32-row ring
+#define CCD_RATE_TW 56               // tile columns; + 4 halo columns each side = the 64 ring columns
+#define CCD_RATE_ROWS 32
+
+struct RateJobDev {
+    const EntStream *es;      // device: the job's stream descriptor (grids, ARM blob, latents in decode order)
+    float *bits;              // [n_symbols] 24 - log2(freq), decode order
+    uint32_t *freq;           // optional
+    uint32_t *mu_sc;          // optional: mu_idx | sc_idx << 16
+    unsigned long long *bad;  // smallest decode-order index of a latent outside [-64, 63] (~0 if none)
+    int32_t kind;             // ARM variant (ccd_rate_kind)
+};
+struct RateTile {
+    int32_t job, grid, y0, x0;  // grid: decode-order index (0 = coarsest)
+};
+// spatial rate map of one job (finest grid first, canonical fp32 order)
+struct RateSpatialDev {
+    const float *bits;
+    float *out;               // [H][W]
+    int32_t H, W, n_grids;
+    int32_t h[CCD_MAX_GRIDS], w[CCD_MAX_GRIDS];
+    int64_t off[CCD_MAX_GRIDS];   // decode-order offset of the grid in bits
+    float ratio[CCD_MAX_GRIDS];   // fp32((H * W) / (h * w))
+    float sy[CCD_MAX_GRIDS], sx[CCD_MAX_GRIDS];  // nearest-resize scales h / H, w / W (fp32)
+};
+
+int ccd_rate_kind(int n_ctx, int cf, bool fast);
+size_t ccd_rate_smem_bytes(int arm_blob_bytes, int ifce_blob_max);
+int ccd_rate_launch(const RateTile *d_tiles, int n_tiles, const RateJobDev *d_jobs, size_t smem, const uint32_t *d_cdf,
+                    const float *d_scale, double *d_part, cudaStream_t st);
+int ccd_rate_spatial_launch(const RateSpatialDev *d_jobs, int n_jobs, int64_t max_pixels, cudaStream_t st);
+
+// --------------------------------------------------------------------------------------
 // Synthesis stage (ccd_synth.cu)
 // --------------------------------------------------------------------------------------
 struct SynLayerDev {

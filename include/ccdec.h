@@ -154,6 +154,35 @@ int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
                        uint64_t seed, int8_t *d_latents, uint32_t *d_out_words, int64_t out_cap_words,
                        int64_t *n_words_out, int32_t *slow_path_count_out, void *cuda_stream);
 
+/* Rate analysis of decoded latents: the information content of every latent symbol under the model the
+ * range coder used -- the ARM + IFCE evaluated exactly as decoding does, (mu_idx, sc_idx) clamped like
+ * latent.py:165 / rangecoder.py:89-91, freq = left(s+1) - left(s) of constriction's leaky quantised Laplace
+ * on the 2^24 scale (an integer in [1, 2^24]), bits = 24 - log2(freq).  This is not the encoder's training
+ * rate proxy.  Inputs: desc, the host NN integers (ccd_decode_nn) and d_latents in decode order (what
+ * ccd_decode_many writes to CcdJob.d_latents).  Outputs: d_bits float32 [n_symbols] in decode order
+ * (required); d_freq uint32 and d_mu_sc (mu_idx | sc_idx << 16) uint32, same layout (optional);
+ * d_spatial float32 [img_h][img_w] (optional): the per-pixel map of training/test.py:217-235 -- every
+ * grid's bits divided by fp32((H*W)/(h*w)), taken to the image size by nearest (F.interpolate index),
+ * summed over grids in fp32, finest grid first, starting from 0; grid_bits (out): f64 sum per grid
+ * (grid 0 = finest), a fixed-order reduction (the same value on every run).  A latent outside [-64, 63]
+ * makes the job CCD_ERR_ARG with bad_index = its decode-order index (else -1). */
+typedef struct CcdRateJob {
+    const CcdCoolChicDesc *desc;
+    const int64_t *nn_ints;
+    const int8_t *d_latents;
+    float *d_bits;
+    uint32_t *d_freq;
+    uint32_t *d_mu_sc;
+    float *d_spatial;
+    double grid_bits[CCD_MAX_GRIDS];
+    int64_t bad_index;
+    int32_t status;
+} CcdRateJob;
+
+/* All jobs in ONE kernel launch (plus one for the spatial maps, if any job asks for one).  Synchronous
+ * like ccd_decode_many.  Returns CCD_OK or the first failing job's status. */
+int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_stream);
+
 /* Tail of decode_frame for every frame type (bitstream/decode.py:191-206 with
  * io/format/yuv.py:239-256,274-300): round to the 2^b-1 grid -> (444->420 2x2 average of
  * U,V) -> clamp [0,1] -> round again.  data_type: 0 rgb, 1 yuv420, 2 yuv444.

@@ -1,0 +1,49 @@
+"""Quality analysis of a Cool-chic bitstream against its source: PSNR per plane and per frame, rate, and the
+prediction statistics of P / B frames, with the reference encoder's column names.
+
+    python cc_eval.py -i <bitstream.cool> --original <src.yuv|png|ppm> [--frame_offset N] [--maps out.npz] [--device N]
+
+Display frame i is compared with source frame frame_offset + i.  ``--maps`` writes, per frame, the error map
+(sum over planes of the squared integer errors / (2^b - 1)^2, chroma at (y >> 1, x >> 1) for 4:2:0) and for P / B
+frames the alpha, beta and prediction maps.
+"""
+import argparse
+
+import numpy as np
+
+import coolchic_b200  # noqa: F401  (import alias of the cool-chic_b200/ package)
+from coolchic_b200.bitstream.quality import video_quality
+
+COLUMNS = ["frame_idx", "frame_type", "psnr_db", "psnr_y_db", "psnr_u_db", "psnr_v_db", "rate_bpp", "alpha_mean",
+           "beta_mean", "pred_psnr_db", "dummy_pred_psnr_db"]
+
+
+if __name__ == "__main__":
+    parser = argparse.ArgumentParser()
+    parser.add_argument("--input", "-i", type=str, required=True, help="Bitstream path.")
+    parser.add_argument("--original", type=str, required=True, help="Source file (.yuv, .png, .ppm).")
+    parser.add_argument("--frame_offset", type=int, default=0, help="Source frame of the first displayed frame.")
+    parser.add_argument("--maps", type=str, default=None, help="Write the error / alpha / beta / prediction maps here (.npz).")
+    parser.add_argument("--device", type=int, help="CUDA device ordinal.", default=0)
+    args = parser.parse_args()
+
+    with open(args.input, "rb") as f_in:
+        frames = video_quality(f_in.read(), args.original, frame_offset=args.frame_offset, device=args.device,
+                               want_maps=args.maps is not None)
+    print(" ".join(f"{c:<18}" for c in COLUMNS))
+    for key, q in frames.items():
+        vals = [key, q.frame_type] + [f"{getattr(q, c):.6f}" for c in COLUMNS[2:]]
+        print(" ".join(f"{v:<18}" for v in vals))
+    n_bits = 8 * sum(q.n_bytes for q in frames.values())
+    n_pixels = sum(q.img_size[0] * q.img_size[1] for q in frames.values())
+    mean_psnr = sum(q.psnr_db for q in frames.values()) / len(frames)
+    print(f"mean psnr_db {mean_psnr:.6f}  total rate_bpp {n_bits / n_pixels:.6f}  ({len(frames)} frames)")
+    if args.maps:
+        maps = {}
+        for key, q in frames.items():
+            maps[f"frame{key}_error"] = q.error_map.cpu().numpy()
+            for name in ("alpha", "beta", "pred"):
+                t = getattr(q, f"{name}_map")
+                if t is not None:
+                    maps[f"frame{key}_{name}"] = t.cpu().numpy()
+        np.savez_compressed(args.maps, **maps)

@@ -29,7 +29,7 @@ EXPORTS = [
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
     "ccd_synthesize", "ccd_encode_latents", "ccd_finish_frame", "ccd_inter_predict", "ccd_reconstruct_frame",
     "ccd_pack_frame",
-    "ccd_pack_samples", "ccd_latent_rate",
+    "ccd_pack_samples", "ccd_latent_rate", "ccd_frame_distortion", "ccd_inter_stats",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
 ]
 
@@ -64,6 +64,26 @@ class CcdRateJob(ctypes.Structure):
         ("bad_index", ctypes.c_int64),
         ("status", ctypes.c_int32),
     ]
+
+
+class CcdDistJob(ctypes.Structure):
+    _fields_ = [
+        ("d_planes", ctypes.c_void_p * 3),
+        ("d_src", ctypes.c_void_p),
+        ("h", ctypes.c_int32),
+        ("w", ctypes.c_int32),
+        ("chroma_shift", ctypes.c_int32),
+        ("bitdepth", ctypes.c_int32),
+        ("src_layout", ctypes.c_int32),
+        ("d_map", ctypes.c_void_p),
+        ("sse", ctypes.c_uint64 * 3),
+        ("max_abs", ctypes.c_uint32 * 3),
+        ("bad_index", ctypes.c_int64),
+        ("status", ctypes.c_int32),
+    ]
+
+
+SOURCE_LAYOUTS = {"planar": 0, "hwc": 1}
 
 
 class CcdError(RuntimeError):
@@ -126,6 +146,11 @@ def load_library():
         L.ccd_pack_samples.argtypes = [vp, vp, ctypes.c_size_t, ci, ci, vp, vp]
         L.ccd_latent_rate.restype = ci
         L.ccd_latent_rate.argtypes = [vp, ctypes.POINTER(CcdRateJob), ci, vp]
+        L.ccd_frame_distortion.restype = ci
+        L.ccd_frame_distortion.argtypes = [vp, ctypes.POINTER(CcdDistJob), ci, vp]
+        L.ccd_inter_stats.restype = ci
+        L.ccd_inter_stats.argtypes = [vp, vp, ci, vp, ci, vp, vp, ci, ci, ci, ci, ci, vp, ci, vp, ci, vp, vp, vp,
+                                      ctypes.POINTER(ctypes.c_double), vp]
         L.ccd_debug_laplace_domain.restype = ci
         L.ccd_debug_laplace_domain.argtypes = [vp, ci, ci, vp, vp]
         L.ccd_debug_last_status.restype = ci
@@ -490,6 +515,90 @@ class Context:
         for i in range(n):
             res[i]["grid_bits"] = [float(jobs[i].grid_bits[g]) for g in range(descs[i].n_grids)]
         return res
+
+    @staticmethod
+    def _frame_planes(data, frame_data_type):
+        """(keep-alive tensors, [h, w], chroma shift) of a finished frame in FrameData layout."""
+        if frame_data_type == "yuv420":
+            ts = [data[k].contiguous() for k in ("y", "u", "v")]
+            cs = 1
+        else:
+            t = data.contiguous()
+            ts = [t[0, c] for c in range(3)]
+            cs = 0
+        assert all(t.is_cuda and t.dtype == torch.float32 for t in ts)
+        return ts, tuple(ts[0].shape[-2:]), cs
+
+    def frame_distortion(self, frames, sources: Sequence[torch.Tensor], layouts: Sequence[str],
+                         want_maps: bool = False) -> List[dict]:
+        """Distortion of finished frames against their source samples (``ccd_frame_distortion``), one launch for all.
+        ``frames[i]``: a FrameData on this device; ``sources[i]``: its source samples on this device as read from the
+        file (uint8, or int16 holding the uint16 samples), in layout ``layouts[i]`` ("planar" or "hwc").  Per frame a
+        dict with ``sse`` and ``max_abs`` (three ints, one per plane) and on request ``map`` ([H, W] float32 CUDA,
+        fp32(sum_c d_c^2) / fp32(M^2)).  An off-grid decoded sample raises CcdError with ``bad_index`` per frame."""
+        n = len(frames)
+        jobs = (CcdDistJob * n)()
+        keep, res = [], []
+        for i, (fd, src, lay) in enumerate(zip(frames, sources, layouts)):
+            ts, (h, w), cs = self._frame_planes(fd.data, fd.frame_data_type)
+            if not (src.is_cuda and src.is_contiguous() and src.dtype == (torch.uint8 if fd.bitdepth <= 8 else torch.int16)):
+                raise ValueError(f"sources[{i}] must be a contiguous {'uint8' if fd.bitdepth <= 8 else 'int16'} CUDA tensor")
+            if src.numel() != h * w + 2 * (h >> cs) * (w >> cs):
+                raise ValueError(f"sources[{i}] holds {src.numel()} samples, a {h}x{w} {fd.frame_data_type} frame has "
+                                 f"{h * w + 2 * (h >> cs) * (w >> cs)}")
+            r = {}
+            if want_maps:
+                r["map"] = torch.empty((h, w), dtype=torch.float32, device=self.torch_device)
+            keep += [ts, src]
+            for c in range(3):
+                jobs[i].d_planes[c] = ts[c].data_ptr()
+            jobs[i].d_src = src.data_ptr()
+            jobs[i].h, jobs[i].w, jobs[i].chroma_shift, jobs[i].bitdepth = h, w, cs, int(fd.bitdepth)
+            jobs[i].src_layout = SOURCE_LAYOUTS[lay]
+            jobs[i].d_map = r["map"].data_ptr() if want_maps else None
+            res.append(r)
+        rc = self._lib.ccd_frame_distortion(self._h, jobs, n, self._stream())
+        if rc != CCD_OK:
+            msg = self._lib.ccd_last_error(None)
+            err = CcdError(rc, msg.decode() if msg else "")
+            err.bad_index = [int(jobs[i].bad_index) for i in range(n)]
+            raise err
+        for i in range(n):
+            res[i]["sse"] = [int(jobs[i].sse[c]) for c in range(3)]
+            res[i]["max_abs"] = [int(jobs[i].max_abs[c]) for c in range(3)]
+        return res
+
+    def inter_stats(self, residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow, warp_filter_size,
+                    source: Optional[torch.Tensor] = None, layout: str = "planar", want_maps: bool = False) -> dict:
+        """Statistics of a P/B frame's prediction (``ccd_inter_stats``), from the arguments of reconstruct_frame and
+        optionally the frame's source samples (as for frame_distortion).  Returns ``sums``: [sum alpha, sum beta,
+        sum (pred - orig)^2, sum (dummy - orig)^2] (f64; the last two 0 without a source) and on request the maps
+        ``alpha``, ``beta`` ([H, W]) and ``pred`` ([3, H, W]), float32 CUDA."""
+        h, w = self._check_inter_shapes(residue, motion, refs, is_b, frame_data_type)
+        residue, motion = residue.contiguous(), motion.contiguous()
+        keep0, p0 = self._ref_planes(refs[0], frame_data_type)
+        keep1, p1 = self._ref_planes(refs[1], frame_data_type) if is_b else (None, None)
+        if source is not None:
+            cs = 1 if frame_data_type == "yuv420" else 0
+            if not (source.is_cuda and source.is_contiguous() and source.dtype == (torch.uint8 if bitdepth <= 8 else torch.int16)
+                    and source.numel() == h * w + 2 * (h >> cs) * (w >> cs)):
+                raise ValueError(f"source must hold the {h}x{w} {frame_data_type} frame's samples, contiguous on the device")
+        dev = self.torch_device
+        out = {}
+        if want_maps:
+            out = {"alpha": torch.empty((h, w), dtype=torch.float32, device=dev),
+                   "beta": torch.empty((h, w), dtype=torch.float32, device=dev),
+                   "pred": torch.empty((3, h, w), dtype=torch.float32, device=dev)}
+        gf = (ctypes.c_int32 * 4)(*(list(global_flow) + [0, 0, 0, 0])[:4])
+        sums = (ctypes.c_double * 4)()
+        _check(self._lib.ccd_inter_stats(
+            self._h, residue.data_ptr(), residue.size(1), motion.data_ptr(), motion.size(1), p0, p1,
+            _frame_type_code(frame_data_type), int(bitdepth), h, w, int(is_b), gf, int(warp_filter_size),
+            source.data_ptr() if source is not None else None, SOURCE_LAYOUTS[layout],
+            *[out[k].data_ptr() if want_maps else None for k in ("alpha", "beta", "pred")], sums, self._stream()))
+        del keep0, keep1
+        out["sums"] = [float(s) for s in sums]
+        return out
 
     def last_timing(self):
         ms = (ctypes.c_float * 4)()

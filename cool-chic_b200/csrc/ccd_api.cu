@@ -1530,6 +1530,92 @@ int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_st
     return rc;
 }
 
+static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, cudaStream_t st) {
+    // pinned / device staging: the job array, then per job sse[3] (u64), bad (u64), max_abs[3] (u32)
+    const size_t off_res = al(sizeof(DistJobDev) * (size_t)n_jobs), res_bytes = 48;
+    const size_t up = off_res + res_bytes * (size_t)n_jobs;
+    int64_t max_pixels = 1;
+    for (int i = 0; i < n_jobs; i++) {
+        CcdDistJob &J = jobs[i];
+        J.status = CCD_OK;
+        J.bad_index = -1;
+        if (!J.d_planes[0] || !J.d_planes[1] || !J.d_planes[2] || !J.d_src || J.h < 1 || J.w < 1)
+            return J.status = fail(CCD_ERR_ARG, "job %d: bad argument", i);
+        if (J.bitdepth < 1 || J.bitdepth > 16) return J.status = fail(CCD_ERR_ARG, "job %d: bad bitdepth %d", i, J.bitdepth);
+        if (J.chroma_shift < 0 || J.chroma_shift > 1 || J.src_layout < 0 || J.src_layout > 1 || (J.src_layout && J.chroma_shift))
+            return J.status = fail(CCD_ERR_ARG, "job %d: bad layout", i);
+        if (J.chroma_shift && ((J.h | J.w) & 1))
+            return J.status = fail(CCD_ERR_ARG, "job %d: 4:2:0 needs even frame sizes, got %dx%d", i, J.h, J.w);
+        if ((int64_t)J.h * J.w > (int64_t)INT32_MAX / 3) return J.status = fail(CCD_ERR_UNSUPPORTED, "job %d: frame too large", i);
+        max_pixels = std::max(max_pixels, (int64_t)J.h * J.w);
+    }
+    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
+    int rc;
+    if ((rc = ensure_pin(ctx, up))) return rc;
+    if ((rc = ensure_dev(ctx->upload, up))) return rc;
+    unsigned char *h = ctx->h_pin, *dv = ctx->upload.p;
+    memset(h + off_res, 0, res_bytes * (size_t)n_jobs);
+    for (int i = 0; i < n_jobs; i++) {
+        const CcdDistJob &J = jobs[i];
+        unsigned char *res = dv + off_res + res_bytes * (size_t)i;
+        memset(h + off_res + res_bytes * (size_t)i + 24, 0xff, 8);
+        DistJobDev D;
+        for (int c = 0; c < 3; c++) D.p[c] = J.d_planes[c];
+        D.src = J.d_src;
+        D.map = J.d_map;
+        D.h = J.h;
+        D.w = J.w;
+        D.cs = J.chroma_shift;
+        D.hwc = J.src_layout;
+        const double M = (double)((1 << J.bitdepth) - 1);
+        D.M = (float)M;
+        D.M2 = (float)(M * M);
+        D.wide = J.bitdepth > 8;
+        D.sse = reinterpret_cast<unsigned long long *>(res);
+        D.bad = reinterpret_cast<unsigned long long *>(res + 24);
+        D.max_abs = reinterpret_cast<unsigned int *>(res + 32);
+        memcpy(h + sizeof(DistJobDev) * (size_t)i, &D, sizeof(D));
+    }
+    CUDA_TRY(cudaMemcpyAsync(dv, h, up, cudaMemcpyHostToDevice, st));
+    int e = ccd_dist_launch(reinterpret_cast<const DistJobDev *>(dv), n_jobs, max_pixels, ctx->n_sm, st);
+    if (e != 0) return fail(CCD_ERR_CUDA, "frame distortion launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    CUDA_TRY(cudaMemcpyAsync(h + off_res, dv + off_res, res_bytes * (size_t)n_jobs, cudaMemcpyDeviceToHost, st));
+    cudaError_t se = cudaStreamSynchronize(st);
+    if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "frame distortion execution failed: %s", cudaGetErrorString(se));
+    int first = CCD_OK;
+    for (int i = 0; i < n_jobs; i++) {
+        CcdDistJob &J = jobs[i];
+        const unsigned char *res = h + off_res + res_bytes * (size_t)i;
+        unsigned long long bad;
+        memcpy(J.sse, res, 24);
+        memcpy(&bad, res + 24, 8);
+        memcpy(J.max_abs, res + 32, 12);
+        if (bad != ~0ull) {
+            J.bad_index = (int64_t)bad;
+            J.status = CCD_ERR_ARG;
+            if (!first) first = fail(CCD_ERR_ARG, "job %d: decoded sample %lld is off the k / (2^%d - 1) grid", i, (long long)bad, J.bitdepth);
+        }
+    }
+    return first;
+}
+
+int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cuda_stream) {
+    if (!ctx) return fail(CCD_ERR_ARG, "null context");
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
+    if (n_jobs == 0) return CCD_OK;
+    DeviceGuard guard(ctx->device);
+    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const int rc = frame_distortion_body(ctx, jobs, n_jobs, st);
+    if (rc != CCD_OK) {
+        const std::string keep = g_err;
+        cudaStreamSynchronize(st);
+        cudaGetLastError();
+        g_err = keep;
+    }
+    return rc;
+}
+
 int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitdepth, int data_type, float *d_out_a,
                      float *d_out_b, float *d_out_c, void *cuda_stream) {
     if (!ctx || !d_in || !d_out_a || h < 1 || w < 1 || bitdepth < 8 || bitdepth > 16 || data_type < 0 || data_type > 2)
@@ -1543,9 +1629,9 @@ int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitde
 }
 
 namespace {
-int inter_common(CcdContext *ctx, InterLaunch &L, int n_res_ch, int n_mot_ch, void *cuda_stream) {
-    if (!ctx || !L.residue || !L.motion || !L.ref0[0] || !L.ref0[1] || !L.ref0[2] || !L.out[0] || !L.out[1] || !L.out[2] ||
-        L.h < 1 || L.w < 1)
+// argument checks shared by the reconstruction (ccd_inter_predict, ccd_reconstruct_frame) and ccd_inter_stats
+int inter_check(CcdContext *ctx, const InterLaunch &L, int n_res_ch, int n_mot_ch) {
+    if (!ctx || !L.residue || !L.motion || !L.ref0[0] || !L.ref0[1] || !L.ref0[2] || L.h < 1 || L.w < 1)
         return fail(CCD_ERR_ARG, "bad argument");
     if (L.is_b && (!L.ref1[0] || !L.ref1[1] || !L.ref1[2])) return fail(CCD_ERR_ARG, "B frame without a second reference");
     // decode.py:171-189 reads residue channels 0..3 (P) / 0..4 (B) and motion channels 0..1 (P) / 0..3 (B)
@@ -1555,6 +1641,12 @@ int inter_common(CcdContext *ctx, InterLaunch &L, int n_res_ch, int n_mot_ch, vo
         return fail(CCD_ERR_ARG, "%s-frame motion has %d channels, expected %d", L.is_b ? "B" : "P", n_mot_ch, L.is_b ? 4 : 2);
     if ((L.ref_cs || L.out_420) && ((L.h | L.w) & 1)) return fail(CCD_ERR_ARG, "4:2:0 needs even frame sizes, got %dx%d", L.h, L.w);
     if (L.filter_size < 2 || (L.filter_size & 1)) return fail(CCD_ERR_ARG, "bad warp filter size %d", L.filter_size);
+    return CCD_OK;
+}
+
+int inter_common(CcdContext *ctx, InterLaunch &L, int n_res_ch, int n_mot_ch, void *cuda_stream) {
+    if (!L.out[0] || !L.out[1] || !L.out[2]) return fail(CCD_ERR_ARG, "bad argument");
+    if (int rc = inter_check(ctx, L, n_res_ch, n_mot_ch)) return rc;
     DeviceGuard guard(ctx->device);
     if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice failed");
     if (!L.is_b) L.gf[2] = L.gf[3] = 0;
@@ -1606,6 +1698,59 @@ int ccd_reconstruct_frame(CcdContext *ctx, const float *d_residue, int n_res_ch,
     L.filter_size = warp_filter_size;
     L.M = (float)((1 << bitdepth) - 1);
     return inter_common(ctx, L, n_res_ch, n_mot_ch, cuda_stream);
+}
+
+int ccd_inter_stats(CcdContext *ctx, const float *d_residue, int n_res_ch, const float *d_motion, int n_mot_ch,
+                    const float *const ref0_planes[3], const float *const ref1_planes[3], int frame_data_type,
+                    int bitdepth, int h, int w, int is_b, const int32_t *global_flow, int warp_filter_size,
+                    const void *d_src, int src_layout, float *d_alpha, float *d_beta, float *d_pred, double sums[4],
+                    void *cuda_stream) {
+    if (!global_flow || !ref0_planes || !sums) return fail(CCD_ERR_ARG, "bad argument");
+    if (bitdepth < 1 || bitdepth > 16) return fail(CCD_ERR_ARG, "bad bitdepth %d", bitdepth);
+    if (frame_data_type < 0 || frame_data_type > 3) return fail(CCD_ERR_ARG, "bad frame_data_type %d", frame_data_type);
+    if (src_layout < 0 || src_layout > 1 || (src_layout == 1 && frame_data_type == 1))
+        return fail(CCD_ERR_ARG, "bad source layout %d for frame_data_type %d", src_layout, frame_data_type);
+    InterLaunch L{};
+    L.residue = d_residue;
+    L.motion = d_motion;
+    for (int c = 0; c < 3; c++) {
+        L.ref0[c] = ref0_planes[c];
+        L.ref1[c] = (is_b && ref1_planes) ? ref1_planes[c] : nullptr;
+    }
+    L.ref_cs = (frame_data_type == 1);
+    L.h = h; L.w = w; L.is_b = is_b;
+    for (int i = 0; i < 4; i++) L.gf[i] = (i < 2 || is_b) ? global_flow[i] : 0;
+    L.filter_size = warp_filter_size;
+    int rc = inter_check(ctx, L, n_res_ch, n_mot_ch);
+    if (rc) return rc;
+    DeviceGuard guard(ctx->device);
+    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice failed");
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    const int64_t n_ctas = ccd_inter_stats_ctas(h, w);
+    const size_t bytes = sizeof(double) * 4 * (size_t)n_ctas;
+    if ((rc = ensure_pin(ctx, bytes))) return rc;
+    if ((rc = ensure_dev(ctx->upload, bytes))) return rc;
+    InterStatsOut o{};
+    o.src = d_src;
+    o.src_hwc = src_layout;
+    o.src_wide = bitdepth > 8;
+    o.src_M = (float)((1 << bitdepth) - 1);
+    o.alpha = d_alpha;
+    o.beta = d_beta;
+    o.pred = d_pred;
+    o.part = reinterpret_cast<double *>(ctx->upload.p);
+    rc = ccd_inter_stats_launch(L, o, st);
+    if (rc == -1)
+        return fail(CCD_ERR_UNSUPPORTED, "warp filter size %d is not supported (2, 4: frames of at least 2x2; 6 .. 14)", warp_filter_size);
+    if (rc) return fail(CCD_ERR_CUDA, "inter_stats launch failed: %s", cudaGetErrorString((cudaError_t)rc));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_pin, o.part, bytes, cudaMemcpyDeviceToHost, st));
+    cudaError_t se = cudaStreamSynchronize(st);
+    if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "inter_stats execution failed: %s", cudaGetErrorString(se));
+    const double *part = reinterpret_cast<const double *>(ctx->h_pin);
+    for (int k = 0; k < 4; k++) sums[k] = 0.0;
+    for (int64_t b = 0; b < n_ctas; b++)  // tiles in order: a fixed-order sum
+        for (int k = 0; k < 4; k++) sums[k] += part[4 * b + k];
+    return CCD_OK;
 }
 
 int ccd_pack_frame(CcdContext *ctx, const float *const planes[3], int h, int w, int chroma_shift, int bitdepth,

@@ -233,7 +233,102 @@ __global__ void __launch_bounds__(128)
     }
 }
 
+// Statistics of the P/B prediction (training/test.py:169-199), one thread per pixel of a 32 x 4 tile: p0, p1, beta,
+// alpha and pred with exactly the fp32 operations of k_inter_predict, and with a source orig = ks / M (4:2:0 chroma
+// read at >> 1, convert_420_to_444) and dummy = ((0 + r0) + r1) / n_refs.  Per-pixel f64 terms, then a fixed-order
+// tree over the CTA: one partial per CTA and per sum, added by the host in tile order (the same value on every run).
+template <int N>
+__global__ void __launch_bounds__(128)
+    k_inter_stats(const float *__restrict__ residue, const float *__restrict__ motion, RefPlanes ref0, RefPlanes ref1,
+                  int ref_cs, int h, int w, int is_b, int g0x, int g0y, int g1x, int g1y, InterStatsOut o) {
+    __shared__ double red[4][128];
+    const int t = threadIdx.x;
+    const int x = blockIdx.x * 32 + (t & 31), y = blockIdx.y * 4 + (t >> 5);
+    double acc[4] = {0.0, 0.0, 0.0, 0.0};
+    if (x < w && y < h) {
+        const size_t plane = (size_t)h * w, i = (size_t)y * w + x;
+        float p0[3], p1[3] = {0.0f, 0.0f, 0.0f};
+        predict_pixel<N>(ref0, ref_cs, h, w, g0x, g0y, motion[i], motion[plane + i], x, y, p0);
+        float beta = 0.0f;
+        if (is_b) {
+            predict_pixel<N>(ref1, ref_cs, h, w, g1x, g1y, motion[2 * plane + i], motion[3 * plane + i], x, y, p1);
+            beta = __fadd_rn(residue[4 * plane + i], 0.5f);
+            beta = clamp01(beta);
+        }
+        const float alpha = clamp01(__fadd_rn(residue[3 * plane + i], 0.5f));
+        float pred[3];
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            pred[c] = p0[c];
+            if (is_b) pred[c] = __fadd_rn(__fmul_rn(beta, pred[c]), __fmul_rn(__fsub_rn(1.0f, beta), p1[c]));
+        }
+        acc[0] = alpha;
+        acc[1] = beta;
+        if (o.src) {
+            const size_t wc = (size_t)(w >> ref_cs), nc = (size_t)(h >> ref_cs) * wc;
+#pragma unroll
+            for (int c = 0; c < 3; c++) {
+                const size_t k = o.src_hwc ? 3 * i + c
+                                           : (c == 0 ? i : plane + (c - 1) * nc + (size_t)(y >> ref_cs) * wc + (x >> ref_cs));
+                const int ks = o.src_wide ? (int)__ldg(static_cast<const uint16_t *>(o.src) + k)
+                                          : (int)__ldg(static_cast<const uint8_t *>(o.src) + k);
+                const float orig = __fdiv_rn((float)ks, o.src_M);
+                float dummy = __fadd_rn(0.0f, ref_at(ref0, c, ref_cs, w, y, x));
+                if (is_b) dummy = __fadd_rn(dummy, ref_at(ref1, c, ref_cs, w, y, x));
+                dummy = __fdiv_rn(dummy, is_b ? 2.0f : 1.0f);
+                const float e = __fsub_rn(pred[c], orig), f = __fsub_rn(dummy, orig);
+                acc[2] += (double)__fmul_rn(e, e);
+                acc[3] += (double)__fmul_rn(f, f);
+            }
+        }
+        if (o.alpha) o.alpha[i] = alpha;
+        if (o.beta) o.beta[i] = beta;
+        if (o.pred) {
+#pragma unroll
+            for (int c = 0; c < 3; c++) o.pred[c * plane + i] = pred[c];
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++) red[k][t] = acc[k];
+    __syncthreads();
+    for (int s = 64; s > 0; s >>= 1) {
+        if (t < s) {
+#pragma unroll
+            for (int k = 0; k < 4; k++) red[k][t] += red[k][t + s];
+        }
+        __syncthreads();
+    }
+    if (t < 4) o.part[4 * ((size_t)blockIdx.y * gridDim.x + blockIdx.x) + t] = red[t][0];
+}
+
 }  // namespace
+
+int64_t ccd_inter_stats_ctas(int h, int w) { return (int64_t)((w + 31) / 32) * ((h + 3) / 4); }
+
+int ccd_inter_stats_launch(const InterLaunch &a, const InterStatsOut &o, cudaStream_t st) {
+    const dim3 block(128, 1, 1), grid((a.w + 31) / 32, (a.h + 3) / 4, 1);
+    RefPlanes r0, r1;
+    for (int c = 0; c < 3; c++) {
+        r0.p[c] = a.ref0[c];
+        r1.p[c] = a.ref1[c] ? a.ref1[c] : a.ref0[c];
+    }
+#define LAUNCH(N)                                                                                                  \
+    k_inter_stats<N><<<grid, block, 0, st>>>(a.residue, a.motion, r0, r1, a.ref_cs, a.h, a.w, a.is_b, a.gf[0], a.gf[1], \
+                                             a.gf[2], a.gf[3], o)
+    switch (a.filter_size) {
+        case 2: if (a.h < 2 || a.w < 2) return -1; LAUNCH(2); break;
+        case 4: if (a.h < 2 || a.w < 2) return -1; LAUNCH(4); break;
+        case 6: LAUNCH(6); break;
+        case 8: LAUNCH(8); break;
+        case 10: LAUNCH(10); break;
+        case 12: LAUNCH(12); break;
+        case 14: LAUNCH(14); break;
+        default: return -1;
+    }
+#undef LAUNCH
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
 
 int ccd_inter_launch(const InterLaunch &a, cudaStream_t st) {
     const dim3 block(128, 1, 1), grid((a.w + 31) / 32, (a.h + 3) / 4, 1);

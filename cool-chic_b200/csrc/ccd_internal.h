@@ -202,6 +202,21 @@ int ccd_pack(const float *const planes[3], int h, int w, int cs, int bitdepth, i
              void *d_out, cudaStream_t st);
 int ccd_pack_flat(const float *d_in, size_t n, int bitdepth, int sample_bytes, void *d_out, cudaStream_t st);
 
+// Distortion of finished frames against their source samples (ccd_synth.cu, next to the packing kernels): one launch
+// for every job of a call, blockIdx.y = job.
+struct DistJobDev {
+    const float *p[3];          // finished planes (FrameData layout); planes 1, 2 are [h >> cs][w >> cs]
+    const void *src;            // source samples, uint8 (bitdepth <= 8) or uint16: planar, or [h][w][3] when hwc
+    float *map;                 // optional [h][w] error map
+    int32_t h, w, cs, hwc;
+    float M, M2;                // 2^b - 1 and fp32(M^2)
+    int32_t wide;               // 2-byte source samples
+    unsigned long long *sse;    // [3], zeroed by the host
+    unsigned int *max_abs;      // [3], zeroed by the host
+    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
+};
+int ccd_dist_launch(const DistJobDev *d_jobs, int n_jobs, int64_t max_pixels, int n_sm, cudaStream_t st);
+
 // P/B reconstruction (ccd_inter.cu); returns -1 for an unsupported filter size
 struct InterLaunch {
     const float *residue, *motion;  // [4|5][h][w], [2|4][h][w]
@@ -215,3 +230,15 @@ struct InterLaunch {
     float *out[3];
 };
 int ccd_inter_launch(const InterLaunch &a, cudaStream_t st);
+// P/B prediction statistics (k_inter_stats): the prediction of k_inter_predict, its blending weights and, with a
+// source, the squared errors of the prediction and of the reference average.  One f64 partial per CTA and per sum
+// (alpha, beta, pred SSE, dummy SSE) in d_part[4 * n_ctas]; ccd_inter_stats_ctas gives n_ctas.
+struct InterStatsOut {
+    const void *src;                // optional source samples (planar or [h][w][3]), layout of the frame
+    int src_hwc, src_wide;
+    float src_M;
+    float *alpha, *beta, *pred;     // optional maps: [h][w], [h][w], [3][h][w]
+    double *part;
+};
+int64_t ccd_inter_stats_ctas(int h, int w);
+int ccd_inter_stats_launch(const InterLaunch &a, const InterStatsOut &o, cudaStream_t st);

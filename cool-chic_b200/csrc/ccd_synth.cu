@@ -1521,6 +1521,69 @@ int ccd_pack_flat(const float *d_in, size_t n, int bitdepth, int sample_bytes, v
     return (int)cudaGetLastError();
 }
 
+// ---- distortion against the source, the mirror image of the packing above: each decoded sample goes back to its
+// integer kd = rint(x * M) and is compared with the source sample ks as it was uploaded (uint8 / uint16, planar or
+// [H][W][3], never widened on the host).  A thread owns pixels of the luma grid; with 4:2:0 chroma only the thread of
+// the even (x, y) counts the chroma sample, the others read it only for the error map.  Sums are integers: exact, and
+// the same whatever the order of the atomics.
+__global__ void __launch_bounds__(256) k_frame_dist(const DistJobDev *__restrict__ jobs) {
+    const DistJobDev &J = jobs[blockIdx.y];
+    const unsigned w = (unsigned)J.w, cs = (unsigned)J.cs, n0 = (unsigned)J.h * w;
+    const unsigned wc = w >> cs, n1 = ((unsigned)J.h >> cs) * wc;
+    const float M = J.M;
+    const bool want_map = J.map != nullptr;
+    unsigned long long s[3] = {0ull, 0ull, 0ull}, bad = ~0ull;
+    unsigned mx[3] = {0u, 0u, 0u};
+    for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n0; i += gridDim.x * blockDim.x) {
+        const unsigned y = i / w, x = i - y * w;
+        const bool own = ((x | y) & cs) == 0;  // counts the chroma sample (always, without subsampling)
+        unsigned long long e = 0ull;
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            if (c > 0 && !own && !want_map) continue;
+            const unsigned j = c == 0 ? i : (y >> cs) * wc + (x >> cs);
+            const unsigned pidx = c == 0 ? i : n0 + (unsigned)(c - 1) * n1 + j;  // planar (FrameData) sample index
+            const size_t k = J.hwc ? (size_t)i * 3 + c : (size_t)pidx;
+            const float v = __ldg(J.p[c] + j);
+            const float vm = __fmul_rn(v, M), kd = rintf(vm);
+            const int ks = J.wide ? (int)__ldg(static_cast<const uint16_t *>(J.src) + k)
+                                  : (int)__ldg(static_cast<const uint8_t *>(J.src) + k);
+            const unsigned a = (unsigned)abs((int)kd - ks);
+            const unsigned long long d2 = (unsigned long long)a * a;
+            e += d2;
+            if (c == 0 || own) {
+                s[c] += d2;
+                mx[c] = max(mx[c], a);
+                if (!(v >= 0.0f && v <= 1.0f) || fabsf(__fsub_rn(vm, kd)) > 0.0625f) bad = min(bad, (unsigned long long)pidx);
+            }
+        }
+        if (want_map) J.map[i] = __fdiv_rn(__ull2float_rn(e), J.M2);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        for (int o = 16; o > 0; o >>= 1) s[c] += __shfl_down_sync(0xffffffffu, s[c], o);
+        mx[c] = __reduce_max_sync(0xffffffffu, mx[c]);
+    }
+    for (int o = 16; o > 0; o >>= 1) bad = min(bad, __shfl_down_sync(0xffffffffu, bad, o));
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            if (s[c]) atomicAdd(J.sse + c, s[c]);
+            if (mx[c]) atomicMax(J.max_abs + c, mx[c]);
+        }
+        if (bad != ~0ull) atomicMin(J.bad, bad);
+    }
+}
+
+int ccd_dist_launch(const DistJobDev *d_jobs, int n_jobs, int64_t max_pixels, int n_sm, cudaStream_t st) {
+    // about 16 CTAs per SM over the whole call, at least one per job
+    const int64_t want = (max_pixels + 255) / 256, cap = ((int64_t)n_sm * 16 + n_jobs - 1) / n_jobs;
+    const int64_t per_job = want < cap ? want : cap;
+    k_frame_dist<<<dim3((unsigned)per_job, (unsigned)n_jobs, 1), 256, 0, st>>>(d_jobs);
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
+
 int ccd_finish(const float *d_in, int h, int w, int bitdepth, int data_type, float *a, float *b, float *c,
                cudaStream_t st) {
     const float M = (float)((1 << bitdepth) - 1);

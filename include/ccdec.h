@@ -231,6 +231,43 @@ int ccd_pack_frame(CcdContext *ctx, const float *const planes[3], int h, int w, 
 int ccd_pack_samples(CcdContext *ctx, const float *d_samples, size_t n, int bitdepth, int sample_bytes,
                      void *d_out, void *cuda_stream);
 
+/* Distortion of finished frames against their source (training/loss.py:88-118 restated on integers): every decoded
+ * sample x goes back to kd = rint(x * M), M = 2^bitdepth - 1, and d = kd - ks with ks the source sample.
+ * d_planes: the finished frame in FrameData layout (three [H][W] planes; chroma_shift 1: planes 1, 2 are
+ * [H/2][W/2], H and W even).  d_src: the source samples as read from the file, uint8 when bitdepth <= 8 else
+ * native-endian uint16; src_layout 0: planar (Y, U, V one after the other), 1: [H][W][3] (chroma_shift 0 only).
+ * d_map (optional): float32 [H][W], fp32(sum_c d_c^2) / fp32(M^2), 4:2:0 chroma read at (y >> 1, x >> 1).
+ * Outputs: sse[c] = sum of d^2 over plane c (exact), max_abs[c] = max |d|.  A decoded value off the k / M grid
+ * (|x * M - kd| > 1/16, or x outside [0, 1]) makes the job CCD_ERR_ARG with bad_index = the smallest such
+ * sample's planar index (plane after plane, each row-major; else -1). */
+typedef struct CcdDistJob {
+    const float *d_planes[3];
+    const void *d_src;
+    int32_t h, w, chroma_shift, bitdepth, src_layout;
+    float *d_map;
+    uint64_t sse[3];
+    uint32_t max_abs[3];
+    int64_t bad_index;
+    int32_t status;
+} CcdDistJob;
+
+/* All jobs in ONE kernel launch; synchronous.  Returns CCD_OK or the first failing job's status. */
+int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cuda_stream);
+
+/* Statistics of a P/B frame's prediction (training/test.py:169-199), from the arguments of
+ * ccd_reconstruct_frame (checked by the same rules): the prediction pred (beta * p0 + (1 - beta) * p1 for B),
+ * alpha and beta, with the fp32 operations of the reconstruction.  d_src (optional): the frame's source samples
+ * in the layout of ccd_frame_distortion (src_layout 1 for frame types other than yuv420 only); orig = ks / M
+ * with 4:2:0 chroma read at >> 1, dummy = ((0 + r0) + r1) / n_refs.  Maps (each optional): d_alpha, d_beta
+ * float32 [H][W], d_pred float32 [3][H][W].  sums (out): sum of alpha, sum of beta (0 for P), and with a source
+ * the sums of fp32((pred - orig)^2) and fp32((dummy - orig)^2) over the 3 H W samples (else 0): f64 partials
+ * per CTA added in tile order, the same on every run.  One launch; synchronous. */
+int ccd_inter_stats(CcdContext *ctx, const float *d_residue, int n_res_ch, const float *d_motion, int n_mot_ch,
+                    const float *const ref0_planes[3], const float *const ref1_planes[3], int frame_data_type,
+                    int bitdepth, int h, int w, int is_b, const int32_t *global_flow, int warp_filter_size,
+                    const void *d_src, int src_layout, float *d_alpha, float *d_beta, float *d_pred,
+                    double sums[4], void *cuda_stream);
+
 /* Device-side evaluation of the quantised-Laplace left cumulative for testing the f64
  * exp() agreement with the host (SURVEY Appendix C.3): for sc in [sc_lo, sc_hi) and every
  * numerator index n in [0, 32641) (|d| = n/256), writes to host arrays

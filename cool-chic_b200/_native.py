@@ -27,9 +27,8 @@ ERROR_NAMES = {
 EXPORTS = [
     "ccd_version", "ccd_sizeof_desc", "ccd_last_error", "ccd_create", "ccd_destroy", "ccd_nn_count",
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
-    "ccd_synthesize", "ccd_encode_latents", "ccd_finish_frame", "ccd_inter_predict", "ccd_reconstruct_frame",
-    "ccd_pack_frame",
-    "ccd_pack_samples", "ccd_latent_rate", "ccd_frame_distortion", "ccd_inter_stats",
+    "ccd_encode_latents", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
+    "ccd_latent_rate", "ccd_frame_distortion", "ccd_inter_stats",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
 ]
 
@@ -83,6 +82,35 @@ class CcdDistJob(ctypes.Structure):
     ]
 
 
+class CcdInterFrame(ctypes.Structure):
+    _fields_ = [
+        ("d_residue", ctypes.c_void_p),
+        ("n_res_ch", ctypes.c_int32),
+        ("d_motion", ctypes.c_void_p),
+        ("n_mot_ch", ctypes.c_int32),
+        ("ref0", ctypes.c_void_p * 3),
+        ("ref1", ctypes.c_void_p * 3),
+        ("frame_data_type", ctypes.c_int32),
+        ("bitdepth", ctypes.c_int32),
+        ("h", ctypes.c_int32),
+        ("w", ctypes.c_int32),
+        ("is_b", ctypes.c_int32),
+        ("global_flow", ctypes.c_int32 * 4),
+        ("warp_filter_size", ctypes.c_int32),
+    ]
+
+
+class CcdInterStats(ctypes.Structure):
+    _fields_ = [
+        ("d_src", ctypes.c_void_p),
+        ("src_layout", ctypes.c_int32),
+        ("d_alpha", ctypes.c_void_p),
+        ("d_beta", ctypes.c_void_p),
+        ("d_pred", ctypes.c_void_p),
+        ("sums", ctypes.c_double * 4),
+    ]
+
+
 SOURCE_LAYOUTS = {"planar": 0, "hwc": 1}
 
 
@@ -130,16 +158,12 @@ def load_library():
         L.ccd_decode_coolchic.argtypes = [vp, pd, ctypes.c_char_p, sz, ctypes.c_char_p, sz, vp, vp, vp]
         L.ccd_decode_latents.restype = ci
         L.ccd_decode_latents.argtypes = [vp, pd, vp, ctypes.c_char_p, sz, vp, vp]
-        L.ccd_synthesize.restype = ci
-        L.ccd_synthesize.argtypes = [vp, pd, vp, vp, vp, vp]
         L.ccd_encode_latents.restype = ci
         L.ccd_encode_latents.argtypes = [vp, pd, vp, ci, ctypes.c_uint64, vp, vp, i64, vp, vp, vp]
         L.ccd_finish_frame.restype = ci
         L.ccd_finish_frame.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp]
-        L.ccd_inter_predict.restype = ci
-        L.ccd_inter_predict.argtypes = [vp, vp, ci, vp, ci, vp, vp, ci, ci, ci, vp, ci, vp, vp]
         L.ccd_reconstruct_frame.restype = ci
-        L.ccd_reconstruct_frame.argtypes = [vp, vp, ci, vp, ci, vp, vp, ci, ci, ci, ci, ci, vp, ci, vp, vp]
+        L.ccd_reconstruct_frame.argtypes = [vp, ctypes.POINTER(CcdInterFrame), vp, vp]
         L.ccd_pack_frame.restype = ci
         L.ccd_pack_frame.argtypes = [vp, vp, ci, ci, ci, ci, ci, ci, vp, vp]
         L.ccd_pack_samples.restype = ci
@@ -149,8 +173,7 @@ def load_library():
         L.ccd_frame_distortion.restype = ci
         L.ccd_frame_distortion.argtypes = [vp, ctypes.POINTER(CcdDistJob), ci, vp]
         L.ccd_inter_stats.restype = ci
-        L.ccd_inter_stats.argtypes = [vp, vp, ci, vp, ci, vp, vp, ci, ci, ci, ci, ci, vp, ci, vp, ci, vp, vp, vp,
-                                      ctypes.POINTER(ctypes.c_double), vp]
+        L.ccd_inter_stats.argtypes = [vp, ctypes.POINTER(CcdInterFrame), ctypes.POINTER(CcdInterStats), vp]
         L.ccd_debug_laplace_domain.restype = ci
         L.ccd_debug_laplace_domain.argtypes = [vp, ci, ci, vp, vp]
         L.ccd_debug_last_status.restype = ci
@@ -292,15 +315,6 @@ class Context:
                                             latent_bytes, len(latent_bytes), lat.data_ptr(), self._stream()))
         return lat
 
-    def synthesize(self, desc, nn_ints: np.ndarray, latents: torch.Tensor) -> torch.Tensor:
-        nn_ints = np.ascontiguousarray(nn_ints, dtype=np.int64)
-        assert latents.dtype == torch.int8 and latents.is_cuda and latents.is_contiguous()
-        out = torch.empty((1, desc.n_out_channels, desc.img_h, desc.img_w), dtype=torch.float32,
-                          device=self.torch_device)
-        _check(self._lib.ccd_synthesize(self._h, ctypes.byref(desc), nn_ints.ctypes.data_as(ctypes.c_void_p),
-                                        latents.data_ptr(), out.data_ptr(), self._stream()))
-        return out
-
     def encode_latents(self, desc, nn_ints: np.ndarray, latents: Optional[torch.Tensor] = None,
                        seed: Optional[int] = None):
         """Range-encode ``latents`` (mode 1) or draw them from the ARM with ``seed`` (mode 2).
@@ -330,17 +344,21 @@ class Context:
         raw = raw.contiguous()
         h, w = raw.shape[-2:]
         code = _frame_type_code(frame_data_type)
-        if code == 1:
-            y = torch.empty((1, 1, h, w), dtype=torch.float32, device=raw.device)
-            u = torch.empty((1, 1, h // 2, w // 2), dtype=torch.float32, device=raw.device)
-            v = torch.empty_like(u)
-            _check(self._lib.ccd_finish_frame(self._h, raw.data_ptr(), h, w, bitdepth, code, y.data_ptr(),
-                                              u.data_ptr(), v.data_ptr(), self._stream()))
-            return {"y": y, "u": u, "v": v}
-        out = torch.empty_like(raw)
+        out = self._empty_frame(h, w, frame_data_type)
+        planes, _ = _planes(out, frame_data_type)
+        u, v = (planes[1].data_ptr(), planes[2].data_ptr()) if code == 1 else (None, None)
         _check(self._lib.ccd_finish_frame(self._h, raw.data_ptr(), h, w, bitdepth, 2 if code == 3 else code,
-                                          out.data_ptr(), None, None, self._stream()))
+                                          planes[0].data_ptr(), u, v, self._stream()))
         return out
+
+    def _empty_frame(self, h: int, w: int, frame_data_type: str):
+        """FrameData.data of an h x w frame on this device: [1, 3, H, W], or the y / u / v dictionary for yuv420."""
+        dev = self.torch_device
+        if frame_data_type == "yuv420":
+            return {"y": torch.empty((1, 1, h, w), dtype=torch.float32, device=dev),
+                    "u": torch.empty((1, 1, h // 2, w // 2), dtype=torch.float32, device=dev),
+                    "v": torch.empty((1, 1, h // 2, w // 2), dtype=torch.float32, device=dev)}
+        return torch.empty((1, 3, h, w), dtype=torch.float32, device=dev)
 
     @staticmethod
     def _check_inter_shapes(residue, motion, refs, is_b, frame_data_type):
@@ -369,72 +387,49 @@ class Context:
                 raise ValueError(f"reference is {tuple(r.data.shape)}, frame is {(1, 3, h, w)}")
         return h, w
 
-    @staticmethod
-    def _ref_planes(r, frame_data_type):
-        """(keep-alive tensors, c_void_p[3]) of a reference frame's planes."""
-        if frame_data_type == "yuv420":
-            ts = [r.data[k].contiguous() for k in ("y", "u", "v")]
-        else:
-            t = r.data.contiguous()
-            ts = [t[0, c] for c in range(3)]
-        assert all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in ts)
-        return ts, (ctypes.c_void_p * 3)(*[t.data_ptr() for t in ts])
-
-    def inter_predict(self, residue, motion, refs, is_b, frame_data_type, global_flow, warp_filter_size):
-        """decode_frame P/B branch (bitstream/decode.py:156-189) -> PRE-ROUNDING frame [1,3,H,W] (stage entry
-        point for tests; decode_frame uses reconstruct_frame).  References are 4:4:4 here."""
-        if frame_data_type == "yuv420":
-            raise ValueError("inter_predict takes 4:4:4 references; use reconstruct_frame for yuv420 frames")
+    def _inter_frame(self, residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow, warp_filter_size):
+        """(CcdInterFrame, the tensors it points into, h, w) of a P/B frame; bitdepth None: the pre-rounding frame."""
         h, w = self._check_inter_shapes(residue, motion, refs, is_b, frame_data_type)
         residue, motion = residue.contiguous(), motion.contiguous()
-        r0 = refs[0].data.contiguous()
-        r1 = refs[1].data.contiguous() if is_b else None
-        out = torch.empty((1, 3, h, w), dtype=torch.float32, device=self.torch_device)
-        gf = (ctypes.c_int32 * 4)(*(list(global_flow) + [0, 0, 0, 0])[:4])
-        _check(self._lib.ccd_inter_predict(
-            self._h, residue.data_ptr(), residue.size(1), motion.data_ptr(), motion.size(1), r0.data_ptr(),
-            r1.data_ptr() if is_b else None, h, w, int(is_b), gf, int(warp_filter_size), out.data_ptr(), self._stream()))
-        return out
+        f = CcdInterFrame(d_residue=residue.data_ptr(), n_res_ch=residue.size(1), d_motion=motion.data_ptr(),
+                          n_mot_ch=motion.size(1), frame_data_type=_frame_type_code(frame_data_type),
+                          bitdepth=int(bitdepth or 0), h=h, w=w, is_b=int(is_b),
+                          warp_filter_size=int(warp_filter_size))
+        keep = [residue, motion]
+        for dst, r in zip((f.ref0, f.ref1), refs[:2 if is_b else 1]):
+            ts, _ = _planes(r.data, frame_data_type)
+            keep += ts
+            dst[:] = [t.data_ptr() for t in ts]
+        f.global_flow[:] = (list(global_flow) + [0, 0, 0, 0])[:4]
+        return f, keep, h, w
 
     def reconstruct_frame(self, residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow, warp_filter_size):
         """Whole P/B reconstruction in one kernel (bitstream/decode.py:156-206): prediction from the finished
         reference frames (4:2:0 planes read in place), blending, residue, frame tail.  Returns the finished frame
-        in FrameData layout ([1,3,H,W], or the y / u / v dictionary)."""
-        h, w = self._check_inter_shapes(residue, motion, refs, is_b, frame_data_type)
-        residue, motion = residue.contiguous(), motion.contiguous()
-        keep0, p0 = self._ref_planes(refs[0], frame_data_type)
-        keep1, p1 = self._ref_planes(refs[1], frame_data_type) if is_b else (None, None)
-        dev = self.torch_device
-        if frame_data_type == "yuv420":
-            data = {"y": torch.empty((1, 1, h, w), dtype=torch.float32, device=dev),
-                    "u": torch.empty((1, 1, h // 2, w // 2), dtype=torch.float32, device=dev),
-                    "v": torch.empty((1, 1, h // 2, w // 2), dtype=torch.float32, device=dev)}
-            outs = [data[k] for k in ("y", "u", "v")]
-        else:
-            data = torch.empty((1, 3, h, w), dtype=torch.float32, device=dev)
-            outs = [data[0, c] for c in range(3)]
-        po = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in outs])
-        gf = (ctypes.c_int32 * 4)(*(list(global_flow) + [0, 0, 0, 0])[:4])
-        _check(self._lib.ccd_reconstruct_frame(
-            self._h, residue.data_ptr(), residue.size(1), motion.data_ptr(), motion.size(1), p0, p1,
-            _frame_type_code(frame_data_type), int(bitdepth), h, w, int(is_b), gf, int(warp_filter_size), po,
-            self._stream()))
-        del keep0, keep1
+        in FrameData layout ([1,3,H,W], or the y / u / v dictionary).  ``bitdepth=None`` stops before the frame tail
+        (decode.py:156-189): the PRE-ROUNDING frame [1,3,H,W], from 4:4:4 references."""
+        if bitdepth is None and frame_data_type == "yuv420":
+            raise ValueError("the pre-rounding frame takes 4:4:4 references; yuv420 frames need a bitdepth")
+        f, keep, h, w = self._inter_frame(residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow,
+                                          warp_filter_size)
+        data = self._empty_frame(h, w, frame_data_type)
+        outs, _ = _planes(data, frame_data_type)
+        _check(self._lib.ccd_reconstruct_frame(self._h, ctypes.byref(f), (ctypes.c_void_p * 3)(*[t.data_ptr() for t in outs]),
+                                               self._stream()))
+        del keep
         return data
+
+    def inter_predict(self, residue, motion, refs, is_b, frame_data_type, global_flow, warp_filter_size):
+        """decode_frame's P/B branch (bitstream/decode.py:156-189) -> PRE-ROUNDING frame [1,3,H,W] from 4:4:4
+        references (stage entry point for tests): reconstruct_frame without the frame tail."""
+        return self.reconstruct_frame(residue, motion, refs, is_b, frame_data_type, None, global_flow, warp_filter_size)
 
     def pack_frame(self, data, bitdepth: int, frame_data_type: str, interleaved: bool = False,
                    sample_bytes: Optional[int] = None) -> torch.Tensor:
         """Finished frame (FrameData.data on the device) -> integer samples on the device, uint8 / uint16:
         planar (y, u, v one after the other: the .yuv file order) or pixel-interleaved HWC (PPM / PNG order)."""
-        if frame_data_type == "yuv420":
-            planes = [data[k].contiguous() for k in ("y", "u", "v")]
-            h, w = planes[0].shape[-2:]
-            cs = 1
-        else:
-            t = data.contiguous()
-            h, w = t.shape[-2:]
-            planes = [t[0, c] for c in range(3)]
-            cs = 0
+        planes, cs = _planes(data, frame_data_type)
+        h, w = planes[0].shape[-2:]
         if sample_bytes is None:
             sample_bytes = 1 if bitdepth <= 8 else 2
         n = h * w + 2 * (h >> cs) * (w >> cs)
@@ -516,19 +511,6 @@ class Context:
             res[i]["grid_bits"] = [float(jobs[i].grid_bits[g]) for g in range(descs[i].n_grids)]
         return res
 
-    @staticmethod
-    def _frame_planes(data, frame_data_type):
-        """(keep-alive tensors, [h, w], chroma shift) of a finished frame in FrameData layout."""
-        if frame_data_type == "yuv420":
-            ts = [data[k].contiguous() for k in ("y", "u", "v")]
-            cs = 1
-        else:
-            t = data.contiguous()
-            ts = [t[0, c] for c in range(3)]
-            cs = 0
-        assert all(t.is_cuda and t.dtype == torch.float32 for t in ts)
-        return ts, tuple(ts[0].shape[-2:]), cs
-
     def frame_distortion(self, frames, sources: Sequence[torch.Tensor], layouts: Sequence[str],
                          want_maps: bool = False) -> List[dict]:
         """Distortion of finished frames against their source samples (``ccd_frame_distortion``), one launch for all.
@@ -540,7 +522,8 @@ class Context:
         jobs = (CcdDistJob * n)()
         keep, res = [], []
         for i, (fd, src, lay) in enumerate(zip(frames, sources, layouts)):
-            ts, (h, w), cs = self._frame_planes(fd.data, fd.frame_data_type)
+            ts, cs = _planes(fd.data, fd.frame_data_type)
+            h, w = ts[0].shape[-2:]
             if not (src.is_cuda and src.is_contiguous() and src.dtype == (torch.uint8 if fd.bitdepth <= 8 else torch.int16)):
                 raise ValueError(f"sources[{i}] must be a contiguous {'uint8' if fd.bitdepth <= 8 else 'int16'} CUDA tensor")
             if src.numel() != h * w + 2 * (h >> cs) * (w >> cs):
@@ -574,10 +557,8 @@ class Context:
         optionally the frame's source samples (as for frame_distortion).  Returns ``sums``: [sum alpha, sum beta,
         sum (pred - orig)^2, sum (dummy - orig)^2] (f64; the last two 0 without a source) and on request the maps
         ``alpha``, ``beta`` ([H, W]) and ``pred`` ([3, H, W]), float32 CUDA."""
-        h, w = self._check_inter_shapes(residue, motion, refs, is_b, frame_data_type)
-        residue, motion = residue.contiguous(), motion.contiguous()
-        keep0, p0 = self._ref_planes(refs[0], frame_data_type)
-        keep1, p1 = self._ref_planes(refs[1], frame_data_type) if is_b else (None, None)
+        f, keep, h, w = self._inter_frame(residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow,
+                                          warp_filter_size)
         if source is not None:
             cs = 1 if frame_data_type == "yuv420" else 0
             if not (source.is_cuda and source.is_contiguous() and source.dtype == (torch.uint8 if bitdepth <= 8 else torch.int16)
@@ -589,15 +570,12 @@ class Context:
             out = {"alpha": torch.empty((h, w), dtype=torch.float32, device=dev),
                    "beta": torch.empty((h, w), dtype=torch.float32, device=dev),
                    "pred": torch.empty((3, h, w), dtype=torch.float32, device=dev)}
-        gf = (ctypes.c_int32 * 4)(*(list(global_flow) + [0, 0, 0, 0])[:4])
-        sums = (ctypes.c_double * 4)()
-        _check(self._lib.ccd_inter_stats(
-            self._h, residue.data_ptr(), residue.size(1), motion.data_ptr(), motion.size(1), p0, p1,
-            _frame_type_code(frame_data_type), int(bitdepth), h, w, int(is_b), gf, int(warp_filter_size),
-            source.data_ptr() if source is not None else None, SOURCE_LAYOUTS[layout],
-            *[out[k].data_ptr() if want_maps else None for k in ("alpha", "beta", "pred")], sums, self._stream()))
-        del keep0, keep1
-        out["sums"] = [float(s) for s in sums]
+        st = CcdInterStats(d_src=source.data_ptr() if source is not None else None, src_layout=SOURCE_LAYOUTS[layout])
+        if want_maps:
+            st.d_alpha, st.d_beta, st.d_pred = (out[k].data_ptr() for k in ("alpha", "beta", "pred"))
+        _check(self._lib.ccd_inter_stats(self._h, ctypes.byref(f), ctypes.byref(st), self._stream()))
+        del keep
+        out["sums"] = [float(s) for s in st.sums]
         return out
 
     def last_timing(self):
@@ -620,6 +598,18 @@ class Context:
         _check(self._lib.ccd_debug_laplace_domain(self._h, sc_lo, sc_hi, lo.ctypes.data_as(ctypes.c_void_p),
                                                   hi.ctypes.data_as(ctypes.c_void_p)))
         return lo, hi
+
+
+def _planes(data, frame_data_type: str):
+    """(the three contiguous float32 CUDA planes, chroma shift) of FrameData.data: y, u, v for yuv420 (chroma shift
+    1), else the channels of the [1, 3, H, W] tensor."""
+    if frame_data_type == "yuv420":
+        ts, cs = [data[k].contiguous() for k in ("y", "u", "v")], 1
+    else:
+        t = data.contiguous()
+        ts, cs = [t[0, c] for c in range(3)], 0
+    assert all(t.is_cuda and t.dtype == torch.float32 for t in ts)
+    return ts, cs
 
 
 def _frame_type_code(frame_data_type: str) -> int:

@@ -461,6 +461,36 @@ int ensure_pin(CcdContext *c, size_t bytes) {
     return CCD_OK;
 }
 
+// n bytes of pinned staging (h) and of the upload arena (dv)
+int stage(CcdContext *c, size_t n, unsigned char *&h, unsigned char *&dv) {
+    int rc;
+    if ((rc = ensure_pin(c, n)) || (rc = ensure_dev(c->upload, n))) return rc;
+    h = c->h_pin;
+    dv = c->upload.p;
+    return CCD_OK;
+}
+
+// The body of every entry point that takes a context: body(stream) runs on the context's device, and a failing call
+// leaves the context quiescent -- the pinned staging buffer, the upload arena and the scratch may be reused (or
+// re-allocated) by the next call -- with its own message kept.
+template <class F>
+int guarded(CcdContext *ctx, void *cuda_stream, F &&body) {
+    if (!ctx) return fail(CCD_ERR_ARG, "null context");
+    DeviceGuard guard(ctx->device);
+    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+    const cudaStream_t st = (cudaStream_t)cuda_stream;
+    const int rc = body(st);
+    if (rc != CCD_OK) {
+        const std::string keep = g_err;
+        cudaStreamSynchronize(st);
+        for (int a = 0; a < 3; a++)
+            if (ctx->aux[a]) cudaStreamSynchronize(ctx->aux[a]);
+        cudaGetLastError();
+        g_err = keep;
+    }
+    return rc;
+}
+
 inline size_t al(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
 // Host preparation of one job: NN decode, ARM/IFCE packing, stream descriptor.
@@ -1140,40 +1170,15 @@ int64_t ccd_decode_nn(const CcdCoolChicDesc *desc, const uint8_t *nn_bytes, size
     return decode_nn_host(desc, L, nn_bytes, nn_nbytes, out_ints);
 }
 
-// stages: bit 0 entropy, bit 1 synthesis
-static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int64_t *const *nn_ints, int stages,
-                            const int8_t *const *d_lat_in, int mode, uint64_t seed, uint32_t *const *d_out_words,
-                            int64_t out_cap, int32_t (*statuses)[16], cudaStream_t st);
-
-static int decode_impl(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int64_t *const *nn_ints, int stages,
-                       const int8_t *const *d_lat_in, int mode, uint64_t seed, uint32_t *const *d_out_words,
-                       int64_t out_cap, int32_t (*statuses)[16], void *cuda_stream) {
-    if (!ctx) return fail(CCD_ERR_ARG, "null context");
+// The entropy stage of every job, then (tail) its float tail: upsampling, synthesis and the frame tail it asks for.
+static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int64_t *const *nn_ints, bool tail,
+                            int mode, uint64_t seed, uint32_t *const *d_out_words, int64_t out_cap,
+                            int32_t (*statuses)[16], cudaStream_t st) {
     if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
     if (n_jobs == 0) return CCD_OK;
-    if (stages & 2)
+    if (tail)
         for (int i = 0; i < n_jobs; i++)
             if (!jobs[i].d_out) return fail(CCD_ERR_ARG, "job %d: null output pointer", i);
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    const int rc = decode_impl_body(ctx, jobs, n_jobs, nn_ints, stages, d_lat_in, mode, seed, d_out_words, out_cap, statuses, st);
-    if (rc != CCD_OK) {
-        // every exit path leaves the context quiescent: the pinned staging buffer, the upload arena and the scratch
-        // may be reused (or re-allocated) by the next call
-        const std::string keep = g_err;
-        cudaStreamSynchronize(st);
-        for (int a = 0; a < 3; a++)
-            if (ctx->aux[a]) cudaStreamSynchronize(ctx->aux[a]);
-        cudaGetLastError();
-        g_err = keep;
-    }
-    return rc;
-}
-
-static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int64_t *const *nn_ints, int stages,
-                            const int8_t *const *d_lat_in, int mode, uint64_t seed, uint32_t *const *d_out_words,
-                            int64_t out_cap, int32_t (*statuses)[16], cudaStream_t st) {
     CUDA_TRY(cudaEventRecord(ctx->ev[0], st));
 
     std::vector<PreparedJob> P((size_t)n_jobs);
@@ -1182,7 +1187,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         P[(size_t)i].job = &jobs[i];
         P[(size_t)i].d = jobs[i].desc;
         jobs[i].status = CCD_OK;
-        const bool own_lat = !(jobs[i].d_latents || (d_lat_in && d_lat_in[i]));
+        const bool own_lat = !jobs[i].d_latents;
         P[(size_t)i].pad_lat = own_lat && mode == 0;
         int rc = prepare_job(P[(size_t)i], nn_ints ? nn_ints[i] : nullptr);
         if (rc) {
@@ -1190,9 +1195,9 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
             return rc;
         }
         PreparedJob &J = P[(size_t)i];
-        if ((stages & 1) && mode == 0 && (!jobs[i].latent_bytes && jobs[i].latent_nbytes))
+        if (mode == 0 && (!jobs[i].latent_bytes && jobs[i].latent_nbytes))
             return fail(CCD_ERR_ARG, "job %d: null latent bytes", i);
-        const size_t nwords = (stages & 1) && mode == 0 ? jobs[i].latent_nbytes / 4 : 0;
+        const size_t nwords = mode == 0 ? jobs[i].latent_nbytes / 4 : 0;
         J.off_words = up;
         up += al(nwords * 4 + 16);
         J.off_blob = up;
@@ -1201,7 +1206,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         up += al(64);
         J.off_syn = up;
         up += al(J.syn_f.size() * 4);
-        if ((stages & 2) && jobs[i].finish_bitdepth != 0) {
+        if (tail && jobs[i].finish_bitdepth != 0) {
             if (jobs[i].finish_bitdepth < 1 || jobs[i].finish_bitdepth > 16 || jobs[i].finish_type < 0 || jobs[i].finish_type > 3)
                 return fail(CCD_ERR_ARG, "job %d: bad frame tail request (bitdepth %d, type %d)", i, jobs[i].finish_bitdepth, jobs[i].finish_type);
             if (J.L.syn_c != 3) return fail(CCD_ERR_ARG, "job %d: the frame tail needs a 3-channel output, found %d", i, J.L.syn_c);
@@ -1212,7 +1217,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         if (own_lat) scratch_lat += al((size_t)J.lat_bytes);
     }
     TailPlan T;
-    if (stages & 2) plan_tail(P, jobs, T);
+    if (tail) plan_tail(P, jobs, T);
     // device-resident job arrays of the float tail (filled below, uploaded with everything else)
     T.off_syn = up;
     up += al(T.order.size() * ccd_tail_job_bytes());
@@ -1220,11 +1225,10 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     up += al(T.lvl_jobs.size() * ccd_tail_level_job_bytes());
     const size_t off_streams = up;
     up += al(sizeof(EntStream) * (size_t)n_jobs);
+    unsigned char *h, *dv;
     int rc;
-    if ((rc = ensure_pin(ctx, up))) return rc;
-    if ((rc = ensure_dev(ctx->upload, up))) return rc;
+    if ((rc = stage(ctx, up, h, dv))) return rc;
     if ((rc = ensure_dev(ctx->scratch, scratch_lat + al(T.scratch_syn) + T.scratch_tail + T.scratch_fin + 4096))) return rc;
-    unsigned char *h = ctx->h_pin, *dv = ctx->upload.p;
     unsigned char *d_scr_syn = ctx->scratch.p + scratch_lat;
     unsigned char *d_scr_tail = d_scr_syn + al(T.scratch_syn);
     float *d_fin = reinterpret_cast<float *>(d_scr_tail + T.scratch_tail);
@@ -1241,14 +1245,13 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     std::vector<int8_t *> d_lat((size_t)n_jobs);
     for (int i = 0; i < n_jobs; i++) {
         PreparedJob &J = P[(size_t)i];
-        const size_t nbytes4 = (stages & 1) && mode == 0 ? jobs[i].latent_nbytes / 4 * 4 : 0;
+        const size_t nbytes4 = mode == 0 ? jobs[i].latent_nbytes / 4 * 4 : 0;
         memset(h + J.off_words, 0, al(nbytes4 + 16));
         if (nbytes4) memcpy(h + J.off_words, jobs[i].latent_bytes, nbytes4);
         memcpy(h + J.off_blob, J.blob.data(), J.blob.size());
         memset(h + J.off_status, 0, 64);
         if (!J.syn_f.empty()) memcpy(h + J.off_syn, J.syn_f.data(), J.syn_f.size() * 4);
         int8_t *lat = jobs[i].d_latents;
-        if (!lat && d_lat_in && d_lat_in[i]) lat = const_cast<int8_t *>(d_lat_in[i]);
         if (!lat) lat = reinterpret_cast<int8_t *>(ctx->scratch.p + J.off_lat);
         d_lat[(size_t)i] = lat;
         EntStream &S = J.es;
@@ -1266,51 +1269,49 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     for (int t = 0; t < n_jobs; t++)
         memcpy(h + off_streams + sizeof(EntStream) * (size_t)t, &P[(size_t)order[(size_t)t]].es, sizeof(EntStream));
 
-    if (stages & 2) fill_tail(T, P, jobs, d_lat, h, dv, d_scr_tail);
+    if (tail) fill_tail(T, P, jobs, d_lat, h, dv, d_scr_tail);
     CUDA_TRY(cudaMemcpyAsync(dv, h, up, cudaMemcpyHostToDevice, st));
     ctx->last_upload_bytes = up;
     CUDA_TRY(cudaEventRecord(ctx->ev[1], st));
 
-    if (stages & 1) {
-        int t = 0, g = 0;
-        while (t < n_jobs) {
-            int u = t;
-            size_t smem = 0;
-            while (u < n_jobs && key(order[(size_t)u]) == key(order[(size_t)t])) {
-                smem = std::max(smem, P[(size_t)order[(size_t)u]].smem);
-                u++;
-            }
-            const PreparedJob &J0 = P[(size_t)order[(size_t)t]];
-            // more streams than SMs: 8-warp CTAs, two per SM (registers: 2 x 256 x 128; shared memory permitting)
-            const bool narrow = mode == 0 && (u - t) > ctx->n_sm &&
-                                2 * (smem + 1024) <= (size_t)227 * 1024;
-            EntLaunchCfg cfg{J0.d->n_ctx, J0.d->flag_ifce ? J0.d->n_ifce_out : 0, J0.fast, smem,
-                             narrow ? CCD_ENT_THREADS_NARROW : CCD_ENT_THREADS};
-            // group 0 on the caller's stream, the next ones on auxiliary streams forked after the upload
-            cudaStream_t sg = st;
-            if (g > 0) {
-                const int a = (g - 1) % 3;
-                if (!ctx->aux[a]) {
-                    CUDA_TRY(cudaStreamCreateWithFlags(&ctx->aux[a], cudaStreamNonBlocking));
-                    CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_join[a], cudaEventDisableTiming));
-                }
-                sg = ctx->aux[a];
-                CUDA_TRY(cudaStreamWaitEvent(sg, ctx->ev[1], 0));  // the upload (recorded on st before any launch)
-            }
-            int e = ccd_entropy_launch(reinterpret_cast<const EntStream *>(dv + off_streams) + t, u - t, cfg, ctx->d_cdf,
-                                       ctx->d_scale, sg);
-            if (e != 0) return fail(CCD_ERR_CUDA, "entropy kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
-            if (g > 0) {
-                const int a = (g - 1) % 3;
-                CUDA_TRY(cudaEventRecord(ctx->ev_join[a], sg));
-                CUDA_TRY(cudaStreamWaitEvent(st, ctx->ev_join[a], 0));
-            }
-            t = u;
-            g++;
+    int t = 0, g = 0;
+    while (t < n_jobs) {
+        int u = t;
+        size_t smem = 0;
+        while (u < n_jobs && key(order[(size_t)u]) == key(order[(size_t)t])) {
+            smem = std::max(smem, P[(size_t)order[(size_t)u]].smem);
+            u++;
         }
+        const PreparedJob &J0 = P[(size_t)order[(size_t)t]];
+        // more streams than SMs: 8-warp CTAs, two per SM (registers: 2 x 256 x 128; shared memory permitting)
+        const bool narrow = mode == 0 && (u - t) > ctx->n_sm &&
+                            2 * (smem + 1024) <= (size_t)227 * 1024;
+        EntLaunchCfg cfg{J0.d->n_ctx, J0.d->flag_ifce ? J0.d->n_ifce_out : 0, J0.fast, smem,
+                         narrow ? CCD_ENT_THREADS_NARROW : CCD_ENT_THREADS};
+        // group 0 on the caller's stream, the next ones on auxiliary streams forked after the upload
+        cudaStream_t sg = st;
+        if (g > 0) {
+            const int a = (g - 1) % 3;
+            if (!ctx->aux[a]) {
+                CUDA_TRY(cudaStreamCreateWithFlags(&ctx->aux[a], cudaStreamNonBlocking));
+                CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_join[a], cudaEventDisableTiming));
+            }
+            sg = ctx->aux[a];
+            CUDA_TRY(cudaStreamWaitEvent(sg, ctx->ev[1], 0));  // the upload (recorded on st before any launch)
+        }
+        int e = ccd_entropy_launch(reinterpret_cast<const EntStream *>(dv + off_streams) + t, u - t, cfg, ctx->d_cdf,
+                                   ctx->d_scale, sg);
+        if (e != 0) return fail(CCD_ERR_CUDA, "entropy kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+        if (g > 0) {
+            const int a = (g - 1) % 3;
+            CUDA_TRY(cudaEventRecord(ctx->ev_join[a], sg));
+            CUDA_TRY(cudaStreamWaitEvent(st, ctx->ev_join[a], 0));
+        }
+        t = u;
+        g++;
     }
     CUDA_TRY(cudaEventRecord(ctx->ev[2], st));
-    if (stages & 2) {
+    if (tail) {
         if ((rc = launch_tail(T, P, jobs, dv, d_scr_tail, d_fin, st))) return rc;
         // everything else: one job after the other through the per-stream path
         for (int i = 0; i < n_jobs; i++) {
@@ -1340,7 +1341,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         const int32_t *s = reinterpret_cast<const int32_t *>(h + P[(size_t)i].off_status);
         if (statuses) memcpy(statuses[i], s, 64);
         memcpy(ctx->last_status, s, 64);
-        if ((stages & 1) && s[0] != 0) {
+        if (s[0] != 0) {
             jobs[i].status = s[0];
             if (!first) first = fail(s[0], "job %d: corrupt latent payload (range decoder desynchronised)", i);
         }
@@ -1348,8 +1349,16 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     return first;
 }
 
+static int decode_impl(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int64_t *const *nn_ints, bool tail, int mode,
+                       uint64_t seed, uint32_t *const *d_out_words, int64_t out_cap, int32_t (*statuses)[16],
+                       void *cuda_stream) {
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        return decode_impl_body(ctx, jobs, n_jobs, nn_ints, tail, mode, seed, d_out_words, out_cap, statuses, st);
+    });
+}
+
 int ccd_decode_many(CcdContext *ctx, CcdJob *jobs, int n_jobs, void *cuda_stream) {
-    return decode_impl(ctx, jobs, n_jobs, nullptr, 3, nullptr, 0, 0, nullptr, 0, nullptr, cuda_stream);
+    return decode_impl(ctx, jobs, n_jobs, nullptr, true, 0, 0, nullptr, 0, nullptr, cuda_stream);
 }
 
 int ccd_decode_coolchic(CcdContext *ctx, const CcdCoolChicDesc *desc, const uint8_t *nn_bytes, size_t nn_nbytes,
@@ -1364,16 +1373,7 @@ int ccd_decode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
     if (!d_latents || !nn_ints) return fail(CCD_ERR_ARG, "null pointer");
     CcdJob j{desc, nullptr, 0, latent_bytes, latent_nbytes, nullptr, d_latents, 0, 0, 0, nullptr, nullptr};
     const int64_t *nn[1] = {nn_ints};
-    return decode_impl(ctx, &j, 1, nn, 1, nullptr, 0, 0, nullptr, 0, nullptr, cuda_stream);
-}
-
-int ccd_synthesize(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints, const int8_t *d_latents,
-                   float *d_out, void *cuda_stream) {
-    if (!d_latents || !nn_ints || !d_out) return fail(CCD_ERR_ARG, "null pointer");
-    CcdJob j{desc, nullptr, 0, nullptr, 0, d_out, nullptr, 0, 0, 0, nullptr, nullptr};
-    const int64_t *nn[1] = {nn_ints};
-    const int8_t *lat[1] = {d_latents};
-    return decode_impl(ctx, &j, 1, nn, 2, lat, 0, 0, nullptr, 0, nullptr, cuda_stream);
+    return decode_impl(ctx, &j, 1, nn, false, 0, 0, nullptr, 0, nullptr, cuda_stream);
 }
 
 int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints, int mode, uint64_t seed,
@@ -1384,7 +1384,7 @@ int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
     const int64_t *nn[1] = {nn_ints};
     uint32_t *ow[1] = {d_out_words};
     int32_t stt[1][16];
-    int rc = decode_impl(ctx, &j, 1, nn, 1, nullptr, mode, seed, ow, out_cap_words, stt, cuda_stream);
+    int rc = decode_impl(ctx, &j, 1, nn, false, mode, seed, ow, out_cap_words, stt, cuda_stream);
     if (rc) return rc;
     if (n_words_out) *n_words_out = stt[0][3];
     if (slow_out) *slow_out = stt[0][2];
@@ -1393,6 +1393,8 @@ int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
 }
 
 static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaStream_t st) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
+    if (n_jobs == 0) return CCD_OK;
     std::vector<PreparedJob> P((size_t)n_jobs);
     std::vector<RateTile> tiles;
     // tiles of job i, decode-order grid gi: [tile_at[i][gi], tile_at[i][gi + 1])
@@ -1455,10 +1457,8 @@ static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaS
     up += al(sizeof(RateSpatialDev) * sp.size());
     const size_t off_part = up;
     up += al(sizeof(double) * tiles.size());
-    int rc;
-    if ((rc = ensure_pin(ctx, up))) return rc;
-    if ((rc = ensure_dev(ctx->upload, up))) return rc;
-    unsigned char *h = ctx->h_pin, *dv = ctx->upload.p;
+    unsigned char *h, *dv;
+    if (int rc = stage(ctx, up, h, dv)) return rc;
     for (int i = 0; i < n_jobs; i++) {
         PreparedJob &J = P[(size_t)i];
         memcpy(h + off_blob[(size_t)i], J.blob.data(), J.blob.size());
@@ -1513,24 +1513,12 @@ static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaS
 }
 
 int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_stream) {
-    if (!ctx) return fail(CCD_ERR_ARG, "null context");
-    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
-    if (n_jobs == 0) return CCD_OK;
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    const int rc = latent_rate_body(ctx, jobs, n_jobs, st);
-    if (rc != CCD_OK) {
-        // leave the context quiescent: the staging buffers may be reused by the next call
-        const std::string keep = g_err;
-        cudaStreamSynchronize(st);
-        cudaGetLastError();
-        g_err = keep;
-    }
-    return rc;
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int { return latent_rate_body(ctx, jobs, n_jobs, st); });
 }
 
 static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, cudaStream_t st) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
+    if (n_jobs == 0) return CCD_OK;
     // pinned / device staging: the job array, then per job sse[3] (u64), bad (u64), max_abs[3] (u32)
     const size_t off_res = al(sizeof(DistJobDev) * (size_t)n_jobs), res_bytes = 48;
     const size_t up = off_res + res_bytes * (size_t)n_jobs;
@@ -1550,10 +1538,8 @@ static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, 
         max_pixels = std::max(max_pixels, (int64_t)J.h * J.w);
     }
     if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
-    int rc;
-    if ((rc = ensure_pin(ctx, up))) return rc;
-    if ((rc = ensure_dev(ctx->upload, up))) return rc;
-    unsigned char *h = ctx->h_pin, *dv = ctx->upload.p;
+    unsigned char *h, *dv;
+    if (int rc = stage(ctx, up, h, dv)) return rc;
     memset(h + off_res, 0, res_bytes * (size_t)n_jobs);
     for (int i = 0; i < n_jobs; i++) {
         const CcdDistJob &J = jobs[i];
@@ -1600,196 +1586,143 @@ static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, 
 }
 
 int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cuda_stream) {
-    if (!ctx) return fail(CCD_ERR_ARG, "null context");
-    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
-    if (n_jobs == 0) return CCD_OK;
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    const int rc = frame_distortion_body(ctx, jobs, n_jobs, st);
-    if (rc != CCD_OK) {
-        const std::string keep = g_err;
-        cudaStreamSynchronize(st);
-        cudaGetLastError();
-        g_err = keep;
-    }
-    return rc;
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int { return frame_distortion_body(ctx, jobs, n_jobs, st); });
 }
 
 int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitdepth, int data_type, float *d_out_a,
                      float *d_out_b, float *d_out_c, void *cuda_stream) {
-    if (!ctx || !d_in || !d_out_a || h < 1 || w < 1 || bitdepth < 8 || bitdepth > 16 || data_type < 0 || data_type > 2)
-        return fail(CCD_ERR_ARG, "bad argument");
-    if (data_type == 1 && (!d_out_b || !d_out_c)) return fail(CCD_ERR_ARG, "yuv420 needs u and v outputs");
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice failed");
-    if (ccd_finish(d_in, h, w, bitdepth, data_type, d_out_a, d_out_b, d_out_c, (cudaStream_t)cuda_stream))
-        return fail(CCD_ERR_CUDA, "finish_frame launch failed");
-    return CCD_OK;
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        if (!d_in || !d_out_a || h < 1 || w < 1 || bitdepth < 8 || bitdepth > 16 || data_type < 0 || data_type > 2)
+            return fail(CCD_ERR_ARG, "bad argument");
+        if (data_type == 1 && (!d_out_b || !d_out_c)) return fail(CCD_ERR_ARG, "yuv420 needs u and v outputs");
+        if (ccd_finish(d_in, h, w, bitdepth, data_type, d_out_a, d_out_b, d_out_c, st))
+            return fail(CCD_ERR_CUDA, "finish_frame launch failed");
+        return CCD_OK;
+    });
 }
 
 namespace {
-// argument checks shared by the reconstruction (ccd_inter_predict, ccd_reconstruct_frame) and ccd_inter_stats
-int inter_check(CcdContext *ctx, const InterLaunch &L, int n_res_ch, int n_mot_ch) {
-    if (!ctx || !L.residue || !L.motion || !L.ref0[0] || !L.ref0[1] || !L.ref0[2] || L.h < 1 || L.w < 1)
+// The launch arguments of a P/B frame, with every check of the reconstruction and of the statistics (outputs aside).
+int inter_launch_args(const CcdInterFrame *f, InterLaunch &L) {
+    if (!f || !f->d_residue || !f->d_motion || !f->ref0[0] || !f->ref0[1] || !f->ref0[2] || f->h < 1 || f->w < 1)
         return fail(CCD_ERR_ARG, "bad argument");
-    if (L.is_b && (!L.ref1[0] || !L.ref1[1] || !L.ref1[2])) return fail(CCD_ERR_ARG, "B frame without a second reference");
+    const int is_b = f->is_b;
+    if (f->bitdepth < 0 || f->bitdepth > 16) return fail(CCD_ERR_ARG, "bad bitdepth %d", f->bitdepth);
+    if (f->frame_data_type < 0 || f->frame_data_type > 3) return fail(CCD_ERR_ARG, "bad frame_data_type %d", f->frame_data_type);
+    if (f->bitdepth == 0 && f->frame_data_type == 1) return fail(CCD_ERR_ARG, "the pre-rounding frame takes 4:4:4 references");
+    if (is_b && (!f->ref1[0] || !f->ref1[1] || !f->ref1[2])) return fail(CCD_ERR_ARG, "B frame without a second reference");
     // decode.py:171-189 reads residue channels 0..3 (P) / 0..4 (B) and motion channels 0..1 (P) / 0..3 (B)
-    if (n_res_ch != (L.is_b ? 5 : 4))
-        return fail(CCD_ERR_ARG, "%s-frame residue has %d channels, expected %d", L.is_b ? "B" : "P", n_res_ch, L.is_b ? 5 : 4);
-    if (n_mot_ch != (L.is_b ? 4 : 2))
-        return fail(CCD_ERR_ARG, "%s-frame motion has %d channels, expected %d", L.is_b ? "B" : "P", n_mot_ch, L.is_b ? 4 : 2);
-    if ((L.ref_cs || L.out_420) && ((L.h | L.w) & 1)) return fail(CCD_ERR_ARG, "4:2:0 needs even frame sizes, got %dx%d", L.h, L.w);
-    if (L.filter_size < 2 || (L.filter_size & 1)) return fail(CCD_ERR_ARG, "bad warp filter size %d", L.filter_size);
+    if (f->n_res_ch != (is_b ? 5 : 4))
+        return fail(CCD_ERR_ARG, "%s-frame residue has %d channels, expected %d", is_b ? "B" : "P", f->n_res_ch, is_b ? 5 : 4);
+    if (f->n_mot_ch != (is_b ? 4 : 2))
+        return fail(CCD_ERR_ARG, "%s-frame motion has %d channels, expected %d", is_b ? "B" : "P", f->n_mot_ch, is_b ? 4 : 2);
+    if (f->frame_data_type == 1 && ((f->h | f->w) & 1)) return fail(CCD_ERR_ARG, "4:2:0 needs even frame sizes, got %dx%d", f->h, f->w);
+    if (f->warp_filter_size < 2 || (f->warp_filter_size & 1)) return fail(CCD_ERR_ARG, "bad warp filter size %d", f->warp_filter_size);
+    L = InterLaunch{};
+    L.residue = f->d_residue;
+    L.motion = f->d_motion;
+    for (int c = 0; c < 3; c++) {
+        L.ref0[c] = f->ref0[c];
+        L.ref1[c] = is_b ? f->ref1[c] : nullptr;
+    }
+    L.ref_cs = L.out_420 = (f->frame_data_type == 1);
+    L.h = f->h;
+    L.w = f->w;
+    L.is_b = is_b;
+    for (int i = 0; i < 4; i++) L.gf[i] = (i < 2 || is_b) ? f->global_flow[i] : 0;
+    L.filter_size = f->warp_filter_size;
+    L.M = f->bitdepth ? (float)((1 << f->bitdepth) - 1) : 0.0f;
     return CCD_OK;
 }
 
-int inter_common(CcdContext *ctx, InterLaunch &L, int n_res_ch, int n_mot_ch, void *cuda_stream) {
-    if (!L.out[0] || !L.out[1] || !L.out[2]) return fail(CCD_ERR_ARG, "bad argument");
-    if (int rc = inter_check(ctx, L, n_res_ch, n_mot_ch)) return rc;
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice failed");
-    if (!L.is_b) L.gf[2] = L.gf[3] = 0;
-    int rc = ccd_inter_launch(L, (cudaStream_t)cuda_stream);
+// status of a P/B kernel launch (ccd_inter_launch, ccd_inter_stats_launch)
+int inter_launched(int rc, int filter_size) {
     if (rc == -1)
-        return fail(CCD_ERR_UNSUPPORTED, "warp filter size %d is not supported (2, 4: frames of at least 2x2; 6 .. 14)", L.filter_size);
-    if (rc) return fail(CCD_ERR_CUDA, "inter_predict launch failed: %s", cudaGetErrorString((cudaError_t)rc));
+        return fail(CCD_ERR_UNSUPPORTED, "warp filter size %d is not supported (2, 4: frames of at least 2x2; 6 .. 14)", filter_size);
+    if (rc) return fail(CCD_ERR_CUDA, "P/B kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc));
     return CCD_OK;
 }
 }  // namespace
 
-int ccd_inter_predict(CcdContext *ctx, const float *d_residue, int n_res_ch, const float *d_motion, int n_mot_ch,
-                      const float *d_ref0, const float *d_ref1, int h, int w, int is_b, const int32_t *global_flow,
-                      int warp_filter_size, float *d_out, void *cuda_stream) {
-    if (!global_flow || !d_ref0 || !d_out) return fail(CCD_ERR_ARG, "bad argument");
-    const size_t plane = (size_t)h * w;
-    InterLaunch L{};
-    L.residue = d_residue;
-    L.motion = d_motion;
-    for (int c = 0; c < 3; c++) {
-        L.ref0[c] = d_ref0 + c * plane;
-        L.ref1[c] = d_ref1 ? d_ref1 + c * plane : nullptr;
-        L.out[c] = d_out + c * plane;
-    }
-    L.h = h; L.w = w; L.is_b = is_b;
-    for (int i = 0; i < 4; i++) L.gf[i] = (i < 2 || is_b) ? global_flow[i] : 0;
-    L.filter_size = warp_filter_size;
-    return inter_common(ctx, L, n_res_ch, n_mot_ch, cuda_stream);
+int ccd_reconstruct_frame(CcdContext *ctx, const CcdInterFrame *frame, float *const out_planes[3], void *cuda_stream) {
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        InterLaunch L;
+        if (int rc = inter_launch_args(frame, L)) return rc;
+        if (!out_planes || !out_planes[0] || !out_planes[1] || !out_planes[2]) return fail(CCD_ERR_ARG, "bad argument");
+        for (int c = 0; c < 3; c++) L.out[c] = out_planes[c];
+        return inter_launched(ccd_inter_launch(L, st), L.filter_size);
+    });
 }
 
-int ccd_reconstruct_frame(CcdContext *ctx, const float *d_residue, int n_res_ch, const float *d_motion, int n_mot_ch,
-                          const float *const ref0_planes[3], const float *const ref1_planes[3], int frame_data_type,
-                          int bitdepth, int h, int w, int is_b, const int32_t *global_flow, int warp_filter_size,
-                          float *const out_planes[3], void *cuda_stream) {
-    if (!global_flow || !ref0_planes || !out_planes) return fail(CCD_ERR_ARG, "bad argument");
-    if (bitdepth < 1 || bitdepth > 16) return fail(CCD_ERR_ARG, "bad bitdepth %d", bitdepth);
-    if (frame_data_type < 0 || frame_data_type > 3) return fail(CCD_ERR_ARG, "bad frame_data_type %d", frame_data_type);
-    InterLaunch L{};
-    L.residue = d_residue;
-    L.motion = d_motion;
-    for (int c = 0; c < 3; c++) {
-        L.ref0[c] = ref0_planes[c];
-        L.ref1[c] = (is_b && ref1_planes) ? ref1_planes[c] : nullptr;
-        L.out[c] = out_planes[c];
-    }
-    L.ref_cs = L.out_420 = (frame_data_type == 1);
-    L.h = h; L.w = w; L.is_b = is_b;
-    for (int i = 0; i < 4; i++) L.gf[i] = (i < 2 || is_b) ? global_flow[i] : 0;
-    L.filter_size = warp_filter_size;
-    L.M = (float)((1 << bitdepth) - 1);
-    return inter_common(ctx, L, n_res_ch, n_mot_ch, cuda_stream);
-}
-
-int ccd_inter_stats(CcdContext *ctx, const float *d_residue, int n_res_ch, const float *d_motion, int n_mot_ch,
-                    const float *const ref0_planes[3], const float *const ref1_planes[3], int frame_data_type,
-                    int bitdepth, int h, int w, int is_b, const int32_t *global_flow, int warp_filter_size,
-                    const void *d_src, int src_layout, float *d_alpha, float *d_beta, float *d_pred, double sums[4],
-                    void *cuda_stream) {
-    if (!global_flow || !ref0_planes || !sums) return fail(CCD_ERR_ARG, "bad argument");
-    if (bitdepth < 1 || bitdepth > 16) return fail(CCD_ERR_ARG, "bad bitdepth %d", bitdepth);
-    if (frame_data_type < 0 || frame_data_type > 3) return fail(CCD_ERR_ARG, "bad frame_data_type %d", frame_data_type);
-    if (src_layout < 0 || src_layout > 1 || (src_layout == 1 && frame_data_type == 1))
-        return fail(CCD_ERR_ARG, "bad source layout %d for frame_data_type %d", src_layout, frame_data_type);
-    InterLaunch L{};
-    L.residue = d_residue;
-    L.motion = d_motion;
-    for (int c = 0; c < 3; c++) {
-        L.ref0[c] = ref0_planes[c];
-        L.ref1[c] = (is_b && ref1_planes) ? ref1_planes[c] : nullptr;
-    }
-    L.ref_cs = (frame_data_type == 1);
-    L.h = h; L.w = w; L.is_b = is_b;
-    for (int i = 0; i < 4; i++) L.gf[i] = (i < 2 || is_b) ? global_flow[i] : 0;
-    L.filter_size = warp_filter_size;
-    int rc = inter_check(ctx, L, n_res_ch, n_mot_ch);
-    if (rc) return rc;
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice failed");
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    const int64_t n_ctas = ccd_inter_stats_ctas(h, w);
-    const size_t bytes = sizeof(double) * 4 * (size_t)n_ctas;
-    if ((rc = ensure_pin(ctx, bytes))) return rc;
-    if ((rc = ensure_dev(ctx->upload, bytes))) return rc;
-    InterStatsOut o{};
-    o.src = d_src;
-    o.src_hwc = src_layout;
-    o.src_wide = bitdepth > 8;
-    o.src_M = (float)((1 << bitdepth) - 1);
-    o.alpha = d_alpha;
-    o.beta = d_beta;
-    o.pred = d_pred;
-    o.part = reinterpret_cast<double *>(ctx->upload.p);
-    rc = ccd_inter_stats_launch(L, o, st);
-    if (rc == -1)
-        return fail(CCD_ERR_UNSUPPORTED, "warp filter size %d is not supported (2, 4: frames of at least 2x2; 6 .. 14)", warp_filter_size);
-    if (rc) return fail(CCD_ERR_CUDA, "inter_stats launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_pin, o.part, bytes, cudaMemcpyDeviceToHost, st));
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "inter_stats execution failed: %s", cudaGetErrorString(se));
-    const double *part = reinterpret_cast<const double *>(ctx->h_pin);
-    for (int k = 0; k < 4; k++) sums[k] = 0.0;
-    for (int64_t b = 0; b < n_ctas; b++)  // tiles in order: a fixed-order sum
-        for (int k = 0; k < 4; k++) sums[k] += part[4 * b + k];
-    return CCD_OK;
+int ccd_inter_stats(CcdContext *ctx, const CcdInterFrame *frame, CcdInterStats *stats, void *cuda_stream) {
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        InterLaunch L;
+        if (int rc = inter_launch_args(frame, L)) return rc;
+        if (!stats) return fail(CCD_ERR_ARG, "bad argument");
+        if (frame->bitdepth < 1) return fail(CCD_ERR_ARG, "bad bitdepth %d", frame->bitdepth);
+        const int layout = stats->src_layout;
+        if (layout < 0 || layout > 1 || (layout == 1 && frame->frame_data_type == 1))
+            return fail(CCD_ERR_ARG, "bad source layout %d for frame_data_type %d", layout, frame->frame_data_type);
+        const int64_t n_ctas = ccd_inter_stats_ctas(L.h, L.w);
+        const size_t bytes = sizeof(double) * 4 * (size_t)n_ctas;
+        unsigned char *h, *dv;
+        if (int rc = stage(ctx, bytes, h, dv)) return rc;
+        InterStatsOut o{};
+        o.src = stats->d_src;
+        o.src_hwc = layout;
+        o.src_wide = frame->bitdepth > 8;
+        o.src_M = L.M;
+        o.alpha = stats->d_alpha;
+        o.beta = stats->d_beta;
+        o.pred = stats->d_pred;
+        o.part = reinterpret_cast<double *>(dv);
+        if (int rc = inter_launched(ccd_inter_stats_launch(L, o, st), L.filter_size)) return rc;
+        CUDA_TRY(cudaMemcpyAsync(h, dv, bytes, cudaMemcpyDeviceToHost, st));
+        cudaError_t se = cudaStreamSynchronize(st);
+        if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "inter_stats execution failed: %s", cudaGetErrorString(se));
+        const double *part = reinterpret_cast<const double *>(h);
+        for (int k = 0; k < 4; k++) stats->sums[k] = 0.0;
+        for (int64_t b = 0; b < n_ctas; b++)  // tiles in order: a fixed-order sum
+            for (int k = 0; k < 4; k++) stats->sums[k] += part[4 * b + k];
+        return CCD_OK;
+    });
 }
 
 int ccd_pack_frame(CcdContext *ctx, const float *const planes[3], int h, int w, int chroma_shift, int bitdepth,
                    int sample_bytes, int interleaved, void *d_out, void *cuda_stream) {
-    if (!ctx || !planes || !planes[0] || !planes[1] || !planes[2] || !d_out || h < 1 || w < 1) return fail(CCD_ERR_ARG, "bad argument");
-    if (bitdepth < 1 || bitdepth > 16 || (sample_bytes != 1 && sample_bytes != 2) || (sample_bytes == 1 && bitdepth > 8))
-        return fail(CCD_ERR_ARG, "bitdepth %d does not fit %d-byte samples", bitdepth, sample_bytes);
-    if (chroma_shift < 0 || chroma_shift > 1 || (interleaved && chroma_shift)) return fail(CCD_ERR_ARG, "bad layout");
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice failed");
-    if (ccd_pack(planes, h, w, chroma_shift, bitdepth, sample_bytes, interleaved, d_out, (cudaStream_t)cuda_stream))
-        return fail(CCD_ERR_CUDA, "pack_frame launch failed");
-    return CCD_OK;
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        if (!planes || !planes[0] || !planes[1] || !planes[2] || !d_out || h < 1 || w < 1) return fail(CCD_ERR_ARG, "bad argument");
+        if (bitdepth < 1 || bitdepth > 16 || (sample_bytes != 1 && sample_bytes != 2) || (sample_bytes == 1 && bitdepth > 8))
+            return fail(CCD_ERR_ARG, "bitdepth %d does not fit %d-byte samples", bitdepth, sample_bytes);
+        if (chroma_shift < 0 || chroma_shift > 1 || (interleaved && chroma_shift)) return fail(CCD_ERR_ARG, "bad layout");
+        if (ccd_pack(planes, h, w, chroma_shift, bitdepth, sample_bytes, interleaved, d_out, st))
+            return fail(CCD_ERR_CUDA, "pack_frame launch failed");
+        return CCD_OK;
+    });
 }
 
 int ccd_pack_samples(CcdContext *ctx, const float *d_samples, size_t n, int bitdepth, int sample_bytes, void *d_out,
                      void *cuda_stream) {
-    if (!ctx || !d_samples || !d_out || n == 0) return fail(CCD_ERR_ARG, "bad argument");
-    if (bitdepth < 1 || bitdepth > 16 || (sample_bytes != 1 && sample_bytes != 2) || (sample_bytes == 1 && bitdepth > 8))
-        return fail(CCD_ERR_ARG, "bitdepth %d does not fit %d-byte samples", bitdepth, sample_bytes);
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice failed");
-    if (ccd_pack_flat(d_samples, n, bitdepth, sample_bytes, d_out, (cudaStream_t)cuda_stream))
-        return fail(CCD_ERR_CUDA, "pack_samples launch failed");
-    return CCD_OK;
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        if (!d_samples || !d_out || n == 0) return fail(CCD_ERR_ARG, "bad argument");
+        if (bitdepth < 1 || bitdepth > 16 || (sample_bytes != 1 && sample_bytes != 2) || (sample_bytes == 1 && bitdepth > 8))
+            return fail(CCD_ERR_ARG, "bitdepth %d does not fit %d-byte samples", bitdepth, sample_bytes);
+        if (ccd_pack_flat(d_samples, n, bitdepth, sample_bytes, d_out, st)) return fail(CCD_ERR_CUDA, "pack_samples launch failed");
+        return CCD_OK;
+    });
 }
 
 int ccd_debug_laplace_domain(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *out_lo, uint32_t *out_hi) {
-    if (!ctx || sc_lo < 0 || sc_hi > CCD_N_SCALE || sc_lo >= sc_hi || !out_lo || !out_hi) return fail(CCD_ERR_ARG, "bad argument");
-    DeviceGuard guard(ctx->device);
-    if (!guard.ok) return fail(CCD_ERR_CUDA, "cudaSetDevice failed");
-    const size_t n = (size_t)(sc_hi - sc_lo) * 32641;
-    int rc;
-    if ((rc = ensure_dev(ctx->scratch, n * 8))) return rc;
-    uint32_t *lo = reinterpret_cast<uint32_t *>(ctx->scratch.p), *hi = lo + n;
-    if (ccd_laplace_domain(ctx->d_scale, sc_lo, sc_hi, lo, hi, 0)) return fail(CCD_ERR_CUDA, "launch failed");
-    CUDA_TRY(cudaMemcpy(out_lo, lo, n * 4, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(out_hi, hi, n * 4, cudaMemcpyDeviceToHost));
-    return CCD_OK;
+    return guarded(ctx, nullptr, [&](cudaStream_t st) -> int {
+        if (sc_lo < 0 || sc_hi > CCD_N_SCALE || sc_lo >= sc_hi || !out_lo || !out_hi) return fail(CCD_ERR_ARG, "bad argument");
+        const size_t n = (size_t)(sc_hi - sc_lo) * 32641;
+        if (int rc = ensure_dev(ctx->scratch, n * 8)) return rc;
+        uint32_t *lo = reinterpret_cast<uint32_t *>(ctx->scratch.p), *hi = lo + n;
+        if (ccd_laplace_domain(ctx->d_scale, sc_lo, sc_hi, lo, hi, st)) return fail(CCD_ERR_CUDA, "launch failed");
+        CUDA_TRY(cudaMemcpy(out_lo, lo, n * 4, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(out_hi, hi, n * 4, cudaMemcpyDeviceToHost));
+        return CCD_OK;
+    });
 }
 
 uint64_t ccd_debug_launch_count(void) { return g_ccd_launches; }

@@ -13,6 +13,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "ccd_detmath.h"
 #include "ccd_internal.h"
 
@@ -169,6 +171,29 @@ __device__ __forceinline__ void predict_pixel(const RefPlanes &ref, int cs, int 
         warp_pixel<N>(ref, cs, h, w, gx, gy, fx, fy, x, y, out);
 }
 
+// The two predictions of pixel (x, y) and its blending weights (decode.py:171-189): p0, p1 (zero for P), beta (0 for
+// P) and the returned alpha, residue channels 4 and 3 plus 0.5, clamped to [0, 1].
+template <int N>
+__device__ __forceinline__ float predict_refs(const float *__restrict__ residue, const float *__restrict__ motion,
+                                              const RefPlanes &ref0, const RefPlanes &ref1, int ref_cs, int h, int w,
+                                              int is_b, int g0x, int g0y, int g1x, int g1y, int x, int y,
+                                              float (&p0)[3], float (&p1)[3], float &beta) {
+    const size_t plane = (size_t)h * w, i = (size_t)y * w + x;
+    p1[0] = p1[1] = p1[2] = 0.0f;
+    predict_pixel<N>(ref0, ref_cs, h, w, g0x, g0y, motion[i], motion[plane + i], x, y, p0);
+    beta = 0.0f;
+    if (is_b) {
+        predict_pixel<N>(ref1, ref_cs, h, w, g1x, g1y, motion[2 * plane + i], motion[3 * plane + i], x, y, p1);
+        beta = __fadd_rn(residue[4 * plane + i], 0.5f);
+        beta = clamp01(beta);
+    }
+    return clamp01(__fadd_rn(residue[3 * plane + i], 0.5f));
+}
+// the prediction: p0 for P, beta * p0 + (1 - beta) * p1 for B
+__device__ __forceinline__ float blend(int is_b, float beta, float p0, float p1) {
+    return is_b ? __fadd_rn(__fmul_rn(beta, p0), __fmul_rn(__fsub_rn(1.0f, beta), p1)) : p0;
+}
+
 // One thread per pixel; a warp covers a 16 x 2 patch (lane = lx + 16 ly), so that the 2 x 2 chroma blocks of a
 // 4:2:0 frame sit inside one warp and the frame tail of decode_frame (bitstream/decode.py:191-206: round ->
 // 2 x 2 average of U, V -> clamp -> round) is done with four shuffles instead of a second pass over HBM.
@@ -185,22 +210,12 @@ __global__ void __launch_bounds__(128)
     const bool inside = px < w && py < h;
     const int x = px < w ? px : w - 1, y = py < h ? py : h - 1;  // every lane computes (shuffles below)
     const size_t plane = (size_t)h * w, i = (size_t)y * w + x;
-    float p0[3], p1[3] = {0.0f, 0.0f, 0.0f};
-    predict_pixel<N>(ref0, ref_cs, h, w, g0x, g0y, motion[i], motion[plane + i], x, y, p0);
-    float beta = 0.0f;
-    if (is_b) {
-        predict_pixel<N>(ref1, ref_cs, h, w, g1x, g1y, motion[2 * plane + i], motion[3 * plane + i], x, y, p1);
-        beta = __fadd_rn(residue[4 * plane + i], 0.5f);
-        beta = clamp01(beta);
-    }
-    float alpha = clamp01(__fadd_rn(residue[3 * plane + i], 0.5f));
+    float p0[3], p1[3], beta;
+    const float alpha = predict_refs<N>(residue, motion, ref0, ref1, ref_cs, h, w, is_b, g0x, g0y, g1x, g1y, x, y, p0,
+                                        p1, beta);
     float v[3];
 #pragma unroll
-    for (int c = 0; c < 3; c++) {
-        float pred = p0[c];
-        if (is_b) pred = __fadd_rn(__fmul_rn(beta, pred), __fmul_rn(__fsub_rn(1.0f, beta), p1[c]));
-        v[c] = __fadd_rn(__fmul_rn(alpha, pred), residue[c * plane + i]);
-    }
+    for (int c = 0; c < 3; c++) v[c] = __fadd_rn(__fmul_rn(alpha, blend(is_b, beta, p0[c], p1[c])), residue[c * plane + i]);
     float *const outp[3] = {o0, o1, o2};
     if (M == 0.0f) {
         if (inside) {
@@ -247,21 +262,12 @@ __global__ void __launch_bounds__(128)
     double acc[4] = {0.0, 0.0, 0.0, 0.0};
     if (x < w && y < h) {
         const size_t plane = (size_t)h * w, i = (size_t)y * w + x;
-        float p0[3], p1[3] = {0.0f, 0.0f, 0.0f};
-        predict_pixel<N>(ref0, ref_cs, h, w, g0x, g0y, motion[i], motion[plane + i], x, y, p0);
-        float beta = 0.0f;
-        if (is_b) {
-            predict_pixel<N>(ref1, ref_cs, h, w, g1x, g1y, motion[2 * plane + i], motion[3 * plane + i], x, y, p1);
-            beta = __fadd_rn(residue[4 * plane + i], 0.5f);
-            beta = clamp01(beta);
-        }
-        const float alpha = clamp01(__fadd_rn(residue[3 * plane + i], 0.5f));
+        float p0[3], p1[3], beta;
+        const float alpha = predict_refs<N>(residue, motion, ref0, ref1, ref_cs, h, w, is_b, g0x, g0y, g1x, g1y, x, y,
+                                            p0, p1, beta);
         float pred[3];
 #pragma unroll
-        for (int c = 0; c < 3; c++) {
-            pred[c] = p0[c];
-            if (is_b) pred[c] = __fadd_rn(__fmul_rn(beta, pred[c]), __fmul_rn(__fsub_rn(1.0f, beta), p1[c]));
-        }
+        for (int c = 0; c < 3; c++) pred[c] = blend(is_b, beta, p0[c], p1[c]);
         acc[0] = alpha;
         acc[1] = beta;
         if (o.src) {
@@ -301,56 +307,46 @@ __global__ void __launch_bounds__(128)
     if (t < 4) o.part[4 * ((size_t)blockIdx.y * gridDim.x + blockIdx.x) + t] = red[t][0];
 }
 
+// One launch of a P/B kernel: launch(std::integral_constant<int, N>, grid, block, ref0, ref1) for the warp filter
+// size N of a, on one thread per pixel in CTAs of 128.  Returns -1 for a size no kernel is built for.
+template <class F>
+int launch_inter(const InterLaunch &a, F &&launch) {
+    const dim3 block(128, 1, 1), grid((a.w + 31) / 32, (a.h + 3) / 4, 1);
+    RefPlanes r0, r1;
+    for (int c = 0; c < 3; c++) {
+        r0.p[c] = a.ref0[c];
+        r1.p[c] = a.ref1[c] ? a.ref1[c] : a.ref0[c];
+    }
+    switch (a.filter_size) {
+        case 2: if (a.h < 2 || a.w < 2) return -1; launch(std::integral_constant<int, 2>{}, grid, block, r0, r1); break;
+        case 4: if (a.h < 2 || a.w < 2) return -1; launch(std::integral_constant<int, 4>{}, grid, block, r0, r1); break;
+        case 6: launch(std::integral_constant<int, 6>{}, grid, block, r0, r1); break;
+        case 8: launch(std::integral_constant<int, 8>{}, grid, block, r0, r1); break;
+        case 10: launch(std::integral_constant<int, 10>{}, grid, block, r0, r1); break;
+        case 12: launch(std::integral_constant<int, 12>{}, grid, block, r0, r1); break;
+        // the largest size the 4-bit header field can carry (header.py:217)
+        case 14: launch(std::integral_constant<int, 14>{}, grid, block, r0, r1); break;
+        default: return -1;
+    }
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
+
 }  // namespace
 
 int64_t ccd_inter_stats_ctas(int h, int w) { return (int64_t)((w + 31) / 32) * ((h + 3) / 4); }
 
 int ccd_inter_stats_launch(const InterLaunch &a, const InterStatsOut &o, cudaStream_t st) {
-    const dim3 block(128, 1, 1), grid((a.w + 31) / 32, (a.h + 3) / 4, 1);
-    RefPlanes r0, r1;
-    for (int c = 0; c < 3; c++) {
-        r0.p[c] = a.ref0[c];
-        r1.p[c] = a.ref1[c] ? a.ref1[c] : a.ref0[c];
-    }
-#define LAUNCH(N)                                                                                                  \
-    k_inter_stats<N><<<grid, block, 0, st>>>(a.residue, a.motion, r0, r1, a.ref_cs, a.h, a.w, a.is_b, a.gf[0], a.gf[1], \
-                                             a.gf[2], a.gf[3], o)
-    switch (a.filter_size) {
-        case 2: if (a.h < 2 || a.w < 2) return -1; LAUNCH(2); break;
-        case 4: if (a.h < 2 || a.w < 2) return -1; LAUNCH(4); break;
-        case 6: LAUNCH(6); break;
-        case 8: LAUNCH(8); break;
-        case 10: LAUNCH(10); break;
-        case 12: LAUNCH(12); break;
-        case 14: LAUNCH(14); break;
-        default: return -1;
-    }
-#undef LAUNCH
-    g_ccd_launches++;
-    return (int)cudaGetLastError();
+    return launch_inter(a, [&](auto n, dim3 grid, dim3 block, const RefPlanes &r0, const RefPlanes &r1) {
+        k_inter_stats<decltype(n)::value><<<grid, block, 0, st>>>(a.residue, a.motion, r0, r1, a.ref_cs, a.h, a.w, a.is_b,
+                                                                  a.gf[0], a.gf[1], a.gf[2], a.gf[3], o);
+    });
 }
 
 int ccd_inter_launch(const InterLaunch &a, cudaStream_t st) {
-    const dim3 block(128, 1, 1), grid((a.w + 31) / 32, (a.h + 3) / 4, 1);
-    RefPlanes r0, r1;
-    for (int c = 0; c < 3; c++) {
-        r0.p[c] = a.ref0[c];
-        r1.p[c] = a.ref1[c] ? a.ref1[c] : a.ref0[c];
-    }
-#define LAUNCH(N)                                                                                                  \
-    k_inter_predict<N><<<grid, block, 0, st>>>(a.residue, a.motion, r0, r1, a.ref_cs, a.h, a.w, a.is_b, a.gf[0],    \
-                                               a.gf[1], a.gf[2], a.gf[3], a.M, a.out_420, a.out[0], a.out[1], a.out[2])
-    switch (a.filter_size) {
-        case 2: if (a.h < 2 || a.w < 2) return -1; LAUNCH(2); break;
-        case 4: if (a.h < 2 || a.w < 2) return -1; LAUNCH(4); break;
-        case 6: LAUNCH(6); break;
-        case 8: LAUNCH(8); break;
-        case 10: LAUNCH(10); break;
-        case 12: LAUNCH(12); break;
-        case 14: LAUNCH(14); break;  // the largest size the 4-bit header field can carry (header.py:217)
-        default: return -1;
-    }
-#undef LAUNCH
-    g_ccd_launches++;
-    return (int)cudaGetLastError();
+    return launch_inter(a, [&](auto n, dim3 grid, dim3 block, const RefPlanes &r0, const RefPlanes &r1) {
+        k_inter_predict<decltype(n)::value><<<grid, block, 0, st>>>(a.residue, a.motion, r0, r1, a.ref_cs, a.h, a.w,
+                                                                    a.is_b, a.gf[0], a.gf[1], a.gf[2], a.gf[3], a.M,
+                                                                    a.out_420, a.out[0], a.out[1], a.out[2]);
+    });
 }

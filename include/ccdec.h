@@ -136,12 +136,10 @@ int ccd_decode_coolchic(CcdContext *ctx, const CcdCoolChicDesc *desc, const uint
                         size_t nn_nbytes, const uint8_t *latent_bytes, size_t latent_nbytes,
                         float *d_out, int8_t *d_latents, void *cuda_stream);
 
-/* Stage entry points (used by tests / profiling; same semantics as the stages above). */
+/* Stage entry point (used by tests / tools; same semantics as the entropy stage above). */
 int ccd_decode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints,
                        const uint8_t *latent_bytes, size_t latent_nbytes, int8_t *d_latents,
                        void *cuda_stream);
-int ccd_synthesize(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints,
-                   const int8_t *d_latents, float *d_out, void *cuda_stream);
 
 /* Range ENcoder on the device: the mode="encode" branch of the same reference functions
  * (component/coolchic.py:152-170,194-195, latent.py:166-170, rangecoder.py:46-78 ->
@@ -191,30 +189,28 @@ int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_st
 int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitdepth, int data_type,
                      float *d_out_a, float *d_out_b, float *d_out_c, void *cuda_stream);
 
-/* P/B-frame prediction + residue (bitstream/decode.py:156-189: apply_global_translation
- * globalmotion.py:151-160, Warper.forward warp.py:294-397 in its training branch, alpha/beta
- * blending).  d_residue [n_res_ch][H][W], d_motion [n_mot_ch][H][W]: raw synthesis outputs; the
- * channel counts are checked against what the path reads (P: 4 / 2, B: 5 / 4; the reference raises a
- * shape error otherwise).  d_ref0/d_ref1 [3][H][W] (444).  global_flow: (x,y) per reference.
- * d_out [3][H][W] pre-rounding frame.  warp_filter_size 2 / 4: grid_sample bilinear / bicubic (border,
- * align_corners); 6, 8, 10, 12, 14: windowed sinc (14 is the largest value of the 4-bit header field,
- * header/header.py:217); odd sizes are an argument error. */
-int ccd_inter_predict(CcdContext *ctx, const float *d_residue, int n_res_ch, const float *d_motion,
-                      int n_mot_ch, const float *d_ref0, const float *d_ref1, int h, int w, int is_b,
-                      const int32_t *global_flow, int warp_filter_size, float *d_out,
-                      void *cuda_stream);
+/* One P/B frame (bitstream/decode.py:156-206: apply_global_translation globalmotion.py:151-160, Warper.forward
+ * warp.py:294-397 in its training branch, alpha/beta blending, residue, frame tail).  d_residue [n_res_ch][H][W],
+ * d_motion [n_mot_ch][H][W]: raw synthesis outputs, channel counts checked (P: 4 / 2, B: 5 / 4; the reference raises a
+ * shape error otherwise).  ref0, ref1 (ignored for P): planes in the frame's layout -- frame_data_type 1 (yuv420):
+ * y [H][W], u, v [H/2][W/2], read through convert_420_to_444 (io/format/yuv.py:303-316) folded into the gather index;
+ * else three [H][W] planes.  bitdepth 1 .. 16: the finished frame; 0: the pre-rounding frame, three [H][W] planes
+ * (4:4:4 references only).  global_flow: (x, y) per reference.  warp_filter_size 2 / 4: grid_sample bilinear / bicubic
+ * (border, align_corners; frames of at least 2x2); 6 .. 14 even: windowed sinc (14: the largest value of the 4-bit
+ * header field, header/header.py:217). */
+typedef struct CcdInterFrame {
+    const float *d_residue;
+    int32_t n_res_ch;
+    const float *d_motion;
+    int32_t n_mot_ch;
+    const float *ref0[3], *ref1[3];
+    int32_t frame_data_type, bitdepth, h, w, is_b;
+    int32_t global_flow[4];
+    int32_t warp_filter_size;
+} CcdInterFrame;
 
-/* Whole reconstruction of a P/B frame in ONE kernel: the prediction above + the frame tail of
- * ccd_finish_frame (bitstream/decode.py:156-206).  The references are given as three plane pointers
- * each, in the layout of the frames this function (or ccd_finish_frame) produced: frame_data_type 1
- * (yuv420): y [H][W], u, v [H/2][W/2] -- read through the nearest x2 up-conversion of
- * convert_420_to_444 (io/format/yuv.py:303-316) folded into the gather index; otherwise three [H][W]
- * planes.  out_planes: the finished frame in the same layout.  ref1_planes may be NULL for a P frame. */
-int ccd_reconstruct_frame(CcdContext *ctx, const float *d_residue, int n_res_ch, const float *d_motion,
-                          int n_mot_ch, const float *const ref0_planes[3],
-                          const float *const ref1_planes[3], int frame_data_type, int bitdepth, int h,
-                          int w, int is_b, const int32_t *global_flow, int warp_filter_size,
-                          float *const out_planes[3], void *cuda_stream);
+/* The whole reconstruction in ONE kernel; out_planes in the layout of the references. */
+int ccd_reconstruct_frame(CcdContext *ctx, const CcdInterFrame *frame, float *const out_planes[3], void *cuda_stream);
 
 /* Output packing on the device (io/format/yuv.py:150-162, ppm.py:160-203, png.py:44-62): finished
  * planes (values on the k / (2^b - 1) grid) -> integer samples round(x * (2^b - 1)), uint8 when
@@ -254,19 +250,19 @@ typedef struct CcdDistJob {
 /* All jobs in ONE kernel launch; synchronous.  Returns CCD_OK or the first failing job's status. */
 int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cuda_stream);
 
-/* Statistics of a P/B frame's prediction (training/test.py:169-199), from the arguments of
- * ccd_reconstruct_frame (checked by the same rules): the prediction pred (beta * p0 + (1 - beta) * p1 for B),
- * alpha and beta, with the fp32 operations of the reconstruction.  d_src (optional): the frame's source samples
- * in the layout of ccd_frame_distortion (src_layout 1 for frame types other than yuv420 only); orig = ks / M
- * with 4:2:0 chroma read at >> 1, dummy = ((0 + r0) + r1) / n_refs.  Maps (each optional): d_alpha, d_beta
- * float32 [H][W], d_pred float32 [3][H][W].  sums (out): sum of alpha, sum of beta (0 for P), and with a source
- * the sums of fp32((pred - orig)^2) and fp32((dummy - orig)^2) over the 3 H W samples (else 0): f64 partials
- * per CTA added in tile order, the same on every run.  One launch; synchronous. */
-int ccd_inter_stats(CcdContext *ctx, const float *d_residue, int n_res_ch, const float *d_motion, int n_mot_ch,
-                    const float *const ref0_planes[3], const float *const ref1_planes[3], int frame_data_type,
-                    int bitdepth, int h, int w, int is_b, const int32_t *global_flow, int warp_filter_size,
-                    const void *d_src, int src_layout, float *d_alpha, float *d_beta, float *d_pred,
-                    double sums[4], void *cuda_stream);
+/* Statistics of a P/B frame's prediction (training/test.py:169-199), with the fp32 operations of the reconstruction
+ * (bitdepth >= 1: the source scale): pred (beta * p0 + (1 - beta) * p1 for B), alpha, beta.  d_src (optional): source
+ * samples as for ccd_frame_distortion (src_layout 1 not for yuv420); orig = ks / M, 4:2:0 chroma read at >> 1,
+ * dummy = ((0 + r0) + r1) / n_refs.  Optional maps: d_alpha, d_beta [H][W], d_pred [3][H][W].  sums (out): sum of
+ * alpha, of beta (0 for P) and, with a source (else 0), of fp32((pred - orig)^2) and fp32((dummy - orig)^2) over the
+ * 3 H W samples: f64 partials per CTA added in tile order, the same on every run.  One launch; synchronous. */
+typedef struct CcdInterStats {
+    const void *d_src;
+    int32_t src_layout;
+    float *d_alpha, *d_beta, *d_pred;
+    double sums[4];
+} CcdInterStats;
+int ccd_inter_stats(CcdContext *ctx, const CcdInterFrame *frame, CcdInterStats *stats, void *cuda_stream);
 
 /* Device-side evaluation of the quantised-Laplace left cumulative for testing the f64
  * exp() agreement with the host (SURVEY Appendix C.3): for sc in [sc_lo, sc_hi) and every

@@ -709,6 +709,40 @@ def test_corrupt_streams_fail_cleanly_on_the_device(ctx, seed_stream):
     assert torch.equal(ctx.decode_coolchic(d, nnb, lb), good)  # the context is still healthy
 
 
+def test_context_stays_healthy_after_a_failed_inter_stats(ctx, oracle, kodim14):
+    """A P/B call that fails (inter_stats of a 4:2:0 frame given an interleaved source layout) leaves the context as
+    every failing entry point does: a decode and a P/B reconstruction on it afterwards still match the oracle."""
+    import torch
+
+    from coolchic_b200 import _native
+    from coolchic_b200.io import FrameData
+
+    rng = np.random.default_rng(5)
+    h, w = 46, 72
+    residue = rng.normal(0, 0.3, size=(5, h, w)).astype(np.float32)
+    motion = rng.normal(0, 2.5, size=(4, h, w)).astype(np.float32)
+    refs = [{"y": (rng.integers(0, 256, size=(h, w)) / 255).astype(np.float32),
+             "u": (rng.integers(0, 256, size=(h // 2, w // 2)) / 255).astype(np.float32),
+             "v": (rng.integers(0, 256, size=(h // 2, w // 2)) / 255).astype(np.float32)} for _ in range(2)]
+    fds = [FrameData(8, "yuv420", {k: torch.from_numpy(v[None, None]).cuda() for k, v in r.items()}) for r in refs]
+    args = (torch.from_numpy(residue[None]).cuda(), torch.from_numpy(motion[None]).cuda(), fds, True, "yuv420", 8,
+            [2, -3, -1, 4], 8)
+    src = torch.zeros((h * w * 3 // 2,), dtype=torch.uint8, device="cuda")
+    with pytest.raises(_native.CcdError) as e:
+        ctx.inter_stats(*args, source=src, layout="hwc")
+    assert e.value.code == -1  # CCD_ERR_ARG
+    d = kodim14["desc"]
+    out = ctx.decode_coolchic(d, kodim14["nn_bytes"], kodim14["lat_bytes"])
+    assert np.array_equal(out[0].cpu().numpy(), oracle.synthesize(d, oracle.decode_nn(d, kodim14["nn_bytes"]),
+                                                                    kodim14["latents"]))
+    up = lambda p: np.repeat(np.repeat(p, 2, axis=0), 2, axis=1)  # noqa: E731
+    r444 = [np.stack([r["y"], up(r["u"]), up(r["v"])]) for r in refs]
+    want = oracle.finish_frame(oracle.inter_predict(residue, motion, r444[0], r444[1], [2, -3, -1, 4], 8), 8, "yuv420")
+    got = ctx.reconstruct_frame(*args)
+    for k in "yuv":
+        assert np.array_equal(got[k][0, 0].cpu().numpy(), want[k]), k
+
+
 def test_integration_stub_b_runs_against_the_reference_header(ctx, kodim14):
     """INTEGRATION.md, stub B, executed as documented: the code block is taken from the file, pointed at the in-tree
     library, and driven with a header object that answers every query the stub makes with what the REFERENCE's own

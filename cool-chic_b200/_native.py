@@ -30,6 +30,7 @@ EXPORTS = [
     "ccd_encode_latents", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
     "ccd_latent_rate", "ccd_frame_distortion", "ccd_inter_stats",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
+    "ccd_debug_entropy_plan",
 ]
 
 
@@ -184,6 +185,8 @@ def load_library():
         L.ccd_debug_set_producer_mask.argtypes = [vp, ctypes.c_uint32]
         L.ccd_last_timing.restype = ci
         L.ccd_last_timing.argtypes = [vp, vp]
+        L.ccd_debug_entropy_plan.restype = ci
+        L.ccd_debug_entropy_plan.argtypes = [pd, vp, vp]
         if L.ccd_sizeof_desc() != ctypes.sizeof(CcdCoolChicDesc):
             raise RuntimeError("CcdCoolChicDesc layout mismatch between Python and libccdec.so")
         _lib = L
@@ -207,6 +210,16 @@ def decode_nn(desc: CcdCoolChicDesc, nn_bytes: bytes) -> np.ndarray:
     if got < 0:
         _check(int(got))
     return out
+
+
+def entropy_plan(desc: CcdCoolChicDesc, nn_ints: np.ndarray):
+    """Host-side shared-memory plan of the entropy kernel for one Cool-chic: (window-ring slots, row-ring rows,
+    bytes).  Raises CcdError (CCD_ERR_UNSUPPORTED) when the stream does not fit, as decoding it would."""
+    nn = np.ascontiguousarray(nn_ints, dtype=np.int64)
+    out = np.zeros(3, dtype=np.int64)
+    _check(load_library().ccd_debug_entropy_plan(ctypes.byref(desc), nn.ctypes.data_as(ctypes.c_void_p),
+                                                  out.ctypes.data_as(ctypes.c_void_p)))
+    return int(out[0]), int(out[1]), int(out[2])
 
 
 def latent_layout(desc: CcdCoolChicDesc):

@@ -493,6 +493,27 @@ int guarded(CcdContext *ctx, void *cuda_stream, F &&body) {
 
 inline size_t al(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
+// Shared memory of the entropy kernel for one stream (DESIGN §4.1): sets S.ring and S.rows, returns the bytes.  The
+// row ring holds every row the wavefront still reads (row y - 4 runs 40 columns ahead of row y), so its size follows
+// from the width alone.  The window ring takes 2 slots per symbol of the longest diagonal + 64, up to 1024, and is
+// halved, down to 64 slots, while the whole does not fit: the producers wait for free slots, so a smaller ring only
+// lets fewer symbols run ahead of the coder.  More than CCD_SMEM_MAX bytes: not even a 64-slot ring fits.
+size_t plan_entropy_smem(EntStream &S, int n_max, int rows_need) {
+    S.rows = next_pow2(rows_need);
+    S.ring = std::min(1024, std::max(64, next_pow2(2 * n_max + 64)));
+    size_t smem = ccd_entropy_smem_bytes(S.ring, S.rows, S.arm_blob_bytes, S.ifce_blob_max);
+    while (smem > CCD_SMEM_MAX && S.ring > 64) {
+        S.ring /= 2;
+        smem = ccd_entropy_smem_bytes(S.ring, S.rows, S.arm_blob_bytes, S.ifce_blob_max);
+    }
+    return smem;
+}
+int entropy_smem_ok(size_t smem) {
+    if (smem <= CCD_SMEM_MAX) return CCD_OK;
+    return fail(CCD_ERR_UNSUPPORTED, "the entropy stage needs %zu bytes of shared memory, %d are available", smem,
+                CCD_SMEM_MAX);
+}
+
 // Host preparation of one job: NN decode, ARM/IFCE packing, stream descriptor.
 int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
     const CcdCoolChicDesc *d = P.d;
@@ -611,11 +632,7 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
         rows_need = std::max(rows_need, G.raster ? 8 : (G.w - 1) / CCD_MASK_STRIDE + 6);
     }
     S.ifce_blob_max = ifce_max;
-    S.ring = std::min(1024, std::max(64, next_pow2(2 * n_max + 64)));  // 148 B of shared memory per slot
-    S.rows = next_pow2(rows_need);
-    P.smem = ccd_entropy_smem_bytes(S.ring, S.rows, S.arm_blob_bytes, S.ifce_blob_max);
-    if (P.smem > 227 * 1024)
-        return fail(CCD_ERR_UNSUPPORTED, "stream needs %zu bytes of shared memory (grid too wide)", P.smem);
+    P.smem = plan_entropy_smem(S, n_max, rows_need);
 
     // ---- synthesis weights, dequantised (neuralnet.py:185-190: float32(int) * q_step)
     const float qs_w = ldexpf(1.0f, d->qshift[6]), qs_b = ldexpf(1.0f, d->qshift[7]);
@@ -1190,11 +1207,12 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         const bool own_lat = !jobs[i].d_latents;
         P[(size_t)i].pad_lat = own_lat && mode == 0;
         int rc = prepare_job(P[(size_t)i], nn_ints ? nn_ints[i] : nullptr);
+        PreparedJob &J = P[(size_t)i];
+        if (!rc) rc = entropy_smem_ok(J.smem);
         if (rc) {
             jobs[i].status = rc;
             return rc;
         }
-        PreparedJob &J = P[(size_t)i];
         if (mode == 0 && (!jobs[i].latent_bytes && jobs[i].latent_nbytes))
             return fail(CCD_ERR_ARG, "job %d: null latent bytes", i);
         const size_t nwords = mode == 0 ? jobs[i].latent_nbytes / 4 : 0;
@@ -1285,7 +1303,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         const PreparedJob &J0 = P[(size_t)order[(size_t)t]];
         // more streams than SMs: 8-warp CTAs, two per SM (registers: 2 x 256 x 128; shared memory permitting)
         const bool narrow = mode == 0 && (u - t) > ctx->n_sm &&
-                            2 * (smem + 1024) <= (size_t)227 * 1024;
+                            2 * (smem + 1024) <= (size_t)CCD_SMEM_MAX;
         EntLaunchCfg cfg{J0.d->n_ctx, J0.d->flag_ifce ? J0.d->n_ifce_out : 0, J0.fast, smem,
                          narrow ? CCD_ENT_THREADS_NARROW : CCD_ENT_THREADS};
         // group 0 on the caller's stream, the next ones on auxiliary streams forked after the upload
@@ -1448,7 +1466,7 @@ static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaS
         }
     }
     if (tiles.size() > (size_t)INT32_MAX) return fail(CCD_ERR_UNSUPPORTED, "too many rate tiles");
-    if (smem > 227 * 1024) return fail(CCD_ERR_UNSUPPORTED, "rate pass needs %zu bytes of shared memory", smem);
+    if (smem > CCD_SMEM_MAX) return fail(CCD_ERR_UNSUPPORTED, "rate pass needs %zu bytes of shared memory", smem);
     const size_t off_jobs = up;
     up += al(sizeof(RateJobDev) * (size_t)n_jobs);
     const size_t off_tiles = up;
@@ -1726,6 +1744,17 @@ int ccd_debug_laplace_domain(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *ou
 }
 
 uint64_t ccd_debug_launch_count(void) { return g_ccd_launches; }
+
+int ccd_debug_entropy_plan(const CcdCoolChicDesc *desc, const int64_t *nn_ints, int64_t out[3]) {
+    if (!desc || !nn_ints || !out) return fail(CCD_ERR_ARG, "null pointer");
+    PreparedJob P;
+    P.d = desc;
+    if (int rc = prepare_job(P, nn_ints)) return rc;
+    out[0] = P.es.ring;
+    out[1] = P.es.rows;
+    out[2] = (int64_t)P.smem;
+    return entropy_smem_ok(P.smem);
+}
 
 int ccd_debug_set_producer_mask(CcdContext *ctx, uint32_t mask) {
     if (!ctx || (mask & 0x3fffu) == 0) return fail(CCD_ERR_ARG, "bad producer mask");

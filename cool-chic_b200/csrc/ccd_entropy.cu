@@ -564,9 +564,10 @@ __device__ __forceinline__ void produce_chunk(const SLoc &S, const SmemLayout &s
     if (valid && member == 0) {
         const uint32_t out_off = (uint32_t)(g->lat_off + (long long)y * w + x);
         const uint32_t row_idx = (((uint32_t)y & row_mask) << 6) | ((uint32_t)x & (CCD_ROW_COLS - 1));
-        // meta: x = output offset, y = row-ring index | (s_lo + 128) << 16, z = mu_idx | sc_idx << 16, w = tag
+        // meta: x = output offset, y = row-ring byte index (bits 0-23: the 2048 rows x 64 columns of a 16383-wide
+        // grid need 17) | (s_lo + 128) << 24 (s_lo + 128 is 50 .. 178), z = mu_idx | sc_idx << 16, w = tag
         const uint32_t ma = sm.meta + slot * 16u;
-        sts_v2(ma, make_uint2(out_off, row_idx | ((uint32_t)(s_lo + 128) << 16)));
+        sts_v2(ma, make_uint2(out_off, row_idx | ((uint32_t)(s_lo + 128) << 24)));
         sts_u32(ma + 8u, (uint32_t)mu_idx | ((uint32_t)sc_idx << 16));
         sts_rel_u32(ma + 12u, ord + 1u);  // the tag: everything this quad / thread stored for the symbol is visible before it
     }
@@ -1138,7 +1139,7 @@ __device__ __forceinline__ void helper_grid(const SLoc &S, const SmemLayout &sm,
                 const uint32_t ra = sm.res + slot * 4u;
                 const uint32_t w = lds_u32(ra);
                 const uint4 m = lds_v4(sm.meta + slot * 16u);
-                const int base = (int)(m.y >> 16) - 128;  // s_lo
+                const int base = (int)(m.y >> 24) - 128;  // s_lo
                 int sym = base + CCD_WIN_HALF;
                 if ((w & 0xfffffe00u) == res_tag(jj)) {
                     const uint32_t v = w & 0x1ffu;
@@ -1157,7 +1158,7 @@ __device__ __forceinline__ void helper_grid(const SLoc &S, const SmemLayout &sm,
                         sts_u32(ra2, 0u);  // (the last reader of the round's word)
                     }
                 }
-                sts_u8(sm.rows + (m.y & 0xffffu), sym);
+                sts_u8(sm.rows + (m.y & 0xffffffu), sym);
                 S.latents[m.x] = (int8_t)sym;
             }
             __syncwarp();
@@ -1184,7 +1185,7 @@ __device__ __noinline__ void encode_grid(const SLoc &S, const SmemLayout &sm, co
         const uint32_t L0 = lds_u32(sm.win + slot * (CCD_WIN * 4) + (uint32_t)lane * 4u);
         const uint32_t L1 = __shfl_down_sync(0xffffffffu, L0, 1);  // lane 31 keeps L0: empty interval
         const int mu_idx = (int)(m.z & 0xffffu), sc_idx = (int)(m.z >> 16);
-        const int s_lo = (int)(m.y >> 16) - 128;
+        const int s_lo = (int)(m.y >> 24) - 128;
         uint32_t l0, l1;
         int src = -1, sym;
         if constexpr (MODE == 2) {
@@ -1218,7 +1219,7 @@ __device__ __noinline__ void encode_grid(const SLoc &S, const SmemLayout &sm, co
         }
         encoder_emit(S, c, l0, l1, lane);
         if (lane == 0) {
-            sts_u8(sm.rows + (m.y & 0xffffu), sym);
+            sts_u8(sm.rows + (m.y & 0xffffffu), sym);
             S.latents[m.x] = (int8_t)sym;
             sts_rel_u32(sm.ctrl, j + 1u);
         }

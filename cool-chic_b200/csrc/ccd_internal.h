@@ -22,6 +22,7 @@
 #define CCD_MAX_DIM 72               // n_ctx (<=40) + n_ifce_out (<=31)
 #define CCD_N_SCALE 2561
 #define CCD_MASK_STRIDE 10           // wavefront stride = ARM mask size 9 + 1 (latent.py:63,72)
+#define CCD_SMEM_MAX (227 * 1024)    // dynamic shared memory one CTA may use on sm_90
 
 // One latent grid, in DECODE order (index 0 = coarsest = first decoded).
 struct EntGrid {

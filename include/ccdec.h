@@ -286,6 +286,12 @@ int ccd_debug_set_producer_mask(CcdContext *ctx, uint32_t mask);
  * csrc/ccd_entropy.cu). */
 int ccd_debug_last_status(const CcdContext *ctx, int32_t st[16]);
 
+/* Shared-memory plan of the entropy kernel for one Cool-chic, computed on the host (no device needed) from its
+ * descriptor and network integers (ccd_nn_count of them): out[0] window-ring slots, out[1] row-ring rows, out[2]
+ * bytes of dynamic shared memory.  The out values are written even when the stream cannot be decoded, which is
+ * then reported with CCD_ERR_UNSUPPORTED, as decoding would report it. */
+int ccd_debug_entropy_plan(const CcdCoolChicDesc *desc, const int64_t *nn_ints, int64_t out[3]);
+
 /* Timing of the last ccd_decode_many call on this context, measured with CUDA events on the
  * launching stream: ms[0] entropy stage, ms[1] upsampling+synthesis, ms[2] host prep + H2D;
  * ms[3] = bytes uploaded host->device by that call (as a float). */

@@ -193,10 +193,15 @@ def load_library():
         return _lib
 
 
-def _check(rc: int) -> None:
+def _check(rc: int, jobs=None) -> None:
+    """Raises CcdError for a failing status; given the call's job array (one whose jobs have a bad_index), the error
+    carries ``bad_index``, one per job."""
     if rc != CCD_OK:
         msg = load_library().ccd_last_error(None)
-        raise CcdError(rc, msg.decode() if msg else "")
+        err = CcdError(rc, msg.decode() if msg else "")
+        if jobs is not None:
+            err.bad_index = [int(j.bad_index) for j in jobs]
+        raise err
 
 
 def decode_nn(desc: CcdCoolChicDesc, nn_bytes: bytes) -> np.ndarray:
@@ -514,12 +519,7 @@ class Context:
             jobs[i].d_mu_sc = r["mu_sc"].data_ptr() if want_mu_sc else None
             jobs[i].d_spatial = r["spatial"].data_ptr() if want_spatial else None
             res.append(r)
-        rc = self._lib.ccd_latent_rate(self._h, jobs, n, self._stream())
-        if rc != CCD_OK:
-            msg = self._lib.ccd_last_error(None)
-            err = CcdError(rc, msg.decode() if msg else "")
-            err.bad_index = [int(jobs[i].bad_index) for i in range(n)]
-            raise err
+        _check(self._lib.ccd_latent_rate(self._h, jobs, n, self._stream()), jobs)
         for i in range(n):
             res[i]["grid_bits"] = [float(jobs[i].grid_bits[g]) for g in range(descs[i].n_grids)]
         return res
@@ -553,12 +553,7 @@ class Context:
             jobs[i].src_layout = SOURCE_LAYOUTS[lay]
             jobs[i].d_map = r["map"].data_ptr() if want_maps else None
             res.append(r)
-        rc = self._lib.ccd_frame_distortion(self._h, jobs, n, self._stream())
-        if rc != CCD_OK:
-            msg = self._lib.ccd_last_error(None)
-            err = CcdError(rc, msg.decode() if msg else "")
-            err.bad_index = [int(jobs[i].bad_index) for i in range(n)]
-            raise err
+        _check(self._lib.ccd_frame_distortion(self._h, jobs, n, self._stream()), jobs)
         for i in range(n):
             res[i]["sse"] = [int(jobs[i].sse[c]) for c in range(3)]
             res[i]["max_abs"] = [int(jobs[i].max_abs[c]) for c in range(3)]

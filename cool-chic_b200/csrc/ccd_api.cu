@@ -394,7 +394,7 @@ struct PreparedJob {
     int tail_cinp = 0, tail_C = 0;
     size_t off_tailP = 0, off_tailQ = 0, off_tailRaw = 0;  // inside the batched path's scratch
     // device offsets inside the upload arena
-    size_t off_words = 0, off_blob = 0, off_status = 0, off_syn = 0, off_lat = 0;
+    size_t off_words = 0, off_blob = 0, off_syn = 0, off_lat = 0;
     std::vector<float> syn_f;  // dequantised synthesis weights, packed
     size_t syn_off_ot_w = 0, syn_off_ot_b = 0, syn_off_st_w = 0, syn_off_st_b = 0;
     size_t syn_off_w[CCD_MAX_SYN], syn_off_b[CCD_MAX_SYN];
@@ -450,24 +450,71 @@ int ensure_dev(DeviceBuf &b, size_t bytes) {
     return CCD_OK;
 }
 
-int ensure_pin(CcdContext *c, size_t bytes) {
-    if (bytes <= c->h_pin_cap) return CCD_OK;
-    if (c->h_pin) CUDA_TRY(cudaFreeHost(c->h_pin));
-    c->h_pin = nullptr;
-    c->h_pin_cap = 0;
-    size_t want = bytes + bytes / 4 + (1 << 16);
-    CUDA_TRY(cudaMallocHost(&c->h_pin, want));
-    c->h_pin_cap = want;
+inline size_t al(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
+
+// The staging of one job call: inputs, then one results region, at the same offsets in the pinned buffer (h) and the
+// upload arena (dv).  One copy takes the inputs and the initial result values up, one brings the results back.
+struct Arena {
+    size_t end = 0;
+    unsigned char *h = nullptr, *dv = nullptr;
+    size_t take(size_t bytes, size_t align = 256) {
+        const size_t at = al(end, align);
+        end = at + bytes;
+        return at;
+    }
+};
+
+// Reserves the pinned staging buffer and the upload arena for everything A has laid out
+int stage(CcdContext *c, Arena &A) {
+    if (A.end > c->h_pin_cap) {
+        if (c->h_pin) CUDA_TRY(cudaFreeHost(c->h_pin));
+        c->h_pin = nullptr;
+        c->h_pin_cap = 0;
+        const size_t want = A.end + A.end / 4 + (1 << 16);
+        CUDA_TRY(cudaMallocHost(&c->h_pin, want));
+        c->h_pin_cap = want;
+    }
+    if (int rc = ensure_dev(c->upload, A.end)) return rc;
+    A.h = c->h_pin;
+    A.dv = c->upload.p;
     return CCD_OK;
 }
 
-// n bytes of pinned staging (h) and of the upload arena (dv)
-int stage(CcdContext *c, size_t n, unsigned char *&h, unsigned char *&dv) {
-    int rc;
-    if ((rc = ensure_pin(c, n)) || (rc = ensure_dev(c->upload, n))) return rc;
-    h = c->h_pin;
-    dv = c->upload.p;
+// Copies the results region [off, A.end) back to the pinned buffer and waits for the call to finish
+int download(const Arena &A, size_t off, cudaStream_t st, const char *what) {
+    CUDA_TRY(cudaMemcpyAsync(A.h + off, A.dv + off, A.end - off, cudaMemcpyDeviceToHost, st));
+    const cudaError_t se = cudaStreamSynchronize(st);
+    if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "%s execution failed: %s", what, cudaGetErrorString(se));
     return CCD_OK;
+}
+
+// A job's status from its result words: a decode job's is word [0] of its entropy status words.  A job with a bad_index
+// gets the smallest bad index the kernel found, ~0 (bad_index -1) when there is none; any other one is CCD_ERR_ARG.
+int job_status(CcdJob &, const int32_t (&words)[16]) { return words[0]; }
+template <class Job> int job_status(Job &J, const unsigned long long &bad) {
+    J.bad_index = (int64_t)bad;
+    return bad == ~0ull ? CCD_OK : CCD_ERR_ARG;
+}
+
+// The per-job results of a job call from its downloaded result words (result[i]: job i's).  Sets each failing job's
+// status; returns CCD_OK, or the first failing job's status with the message say(i) gives it through fail().
+template <class Job, class Word, class Say>
+int report(Job *jobs, int n_jobs, const Word *result, Say &&say) {
+    int first = CCD_OK;
+    for (int i = 0; i < n_jobs; i++) {
+        const int s = job_status(jobs[i], result[i]);
+        if (s == CCD_OK) continue;
+        jobs[i].status = s;
+        if (!first) first = say(i);
+    }
+    return first;
+}
+
+// f64 partials added in order, part[0], part[stride], ..., part[(n - 1) * stride]: the same sum on every run
+double ordered_sum(const double *part, size_t n, size_t stride = 1) {
+    double s = 0.0;
+    for (size_t t = 0; t < n; t++) s += part[t * stride];
+    return s;
 }
 
 // The body of every entry point that takes a context: body(stream) runs on the context's device, and a failing call
@@ -491,7 +538,15 @@ int guarded(CcdContext *ctx, void *cuda_stream, F &&body) {
     return rc;
 }
 
-inline size_t al(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
+// A call on a job array: checks the list, sets every job's status to CCD_OK, runs body(stream) through guarded()
+template <class Job, class F>
+int job_call(CcdContext *ctx, Job *jobs, int n_jobs, void *cuda_stream, F &&body) {
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
+        for (int i = 0; i < n_jobs; i++) jobs[i].status = CCD_OK;
+        return n_jobs == 0 ? CCD_OK : body(st);
+    });
+}
 
 // Shared memory of the entropy kernel for one stream (DESIGN §4.1): sets S.ring and S.rows, returns the bytes.  The
 // row ring holds every row the wavefront still reads (row y - 4 runs 40 columns ahead of row y), so its size follows
@@ -1191,19 +1246,17 @@ int64_t ccd_decode_nn(const CcdCoolChicDesc *desc, const uint8_t *nn_bytes, size
 static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int64_t *const *nn_ints, bool tail,
                             int mode, uint64_t seed, uint32_t *const *d_out_words, int64_t out_cap,
                             int32_t (*statuses)[16], cudaStream_t st) {
-    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
-    if (n_jobs == 0) return CCD_OK;
     if (tail)
         for (int i = 0; i < n_jobs; i++)
             if (!jobs[i].d_out) return fail(CCD_ERR_ARG, "job %d: null output pointer", i);
     CUDA_TRY(cudaEventRecord(ctx->ev[0], st));
 
     std::vector<PreparedJob> P((size_t)n_jobs);
-    size_t up = 0, scratch_lat = 0;
+    Arena A;
+    size_t scratch_lat = 0;
     for (int i = 0; i < n_jobs; i++) {
         P[(size_t)i].job = &jobs[i];
         P[(size_t)i].d = jobs[i].desc;
-        jobs[i].status = CCD_OK;
         const bool own_lat = !jobs[i].d_latents;
         P[(size_t)i].pad_lat = own_lat && mode == 0;
         int rc = prepare_job(P[(size_t)i], nn_ints ? nn_ints[i] : nullptr);
@@ -1216,14 +1269,9 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         if (mode == 0 && (!jobs[i].latent_bytes && jobs[i].latent_nbytes))
             return fail(CCD_ERR_ARG, "job %d: null latent bytes", i);
         const size_t nwords = mode == 0 ? jobs[i].latent_nbytes / 4 : 0;
-        J.off_words = up;
-        up += al(nwords * 4 + 16);
-        J.off_blob = up;
-        up += al(J.blob.size());
-        J.off_status = up;
-        up += al(64);
-        J.off_syn = up;
-        up += al(J.syn_f.size() * 4);
+        J.off_words = A.take(nwords * 4 + 16);
+        J.off_blob = A.take(J.blob.size());
+        J.off_syn = A.take(J.syn_f.size() * 4);
         if (tail && jobs[i].finish_bitdepth != 0) {
             if (jobs[i].finish_bitdepth < 1 || jobs[i].finish_bitdepth > 16 || jobs[i].finish_type < 0 || jobs[i].finish_type > 3)
                 return fail(CCD_ERR_ARG, "job %d: bad frame tail request (bitdepth %d, type %d)", i, jobs[i].finish_bitdepth, jobs[i].finish_type);
@@ -1237,15 +1285,13 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     TailPlan T;
     if (tail) plan_tail(P, jobs, T);
     // device-resident job arrays of the float tail (filled below, uploaded with everything else)
-    T.off_syn = up;
-    up += al(T.order.size() * ccd_tail_job_bytes());
-    T.off_lvl = up;
-    up += al(T.lvl_jobs.size() * ccd_tail_level_job_bytes());
-    const size_t off_streams = up;
-    up += al(sizeof(EntStream) * (size_t)n_jobs);
-    unsigned char *h, *dv;
+    T.off_syn = A.take(T.order.size() * ccd_tail_job_bytes());
+    T.off_lvl = A.take(T.lvl_jobs.size() * ccd_tail_level_job_bytes());
+    const size_t off_streams = A.take(sizeof(EntStream) * (size_t)n_jobs);
+    const size_t off_status = A.take(sizeof(int32_t[16]) * (size_t)n_jobs);  // results: zeroed status words per job
     int rc;
-    if ((rc = stage(ctx, up, h, dv))) return rc;
+    if ((rc = stage(ctx, A))) return rc;
+    unsigned char *h = A.h, *dv = A.dv;
     if ((rc = ensure_dev(ctx->scratch, scratch_lat + al(T.scratch_syn) + T.scratch_tail + T.scratch_fin + 4096))) return rc;
     unsigned char *d_scr_syn = ctx->scratch.p + scratch_lat;
     unsigned char *d_scr_tail = d_scr_syn + al(T.scratch_syn);
@@ -1267,7 +1313,6 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         memset(h + J.off_words, 0, al(nbytes4 + 16));
         if (nbytes4) memcpy(h + J.off_words, jobs[i].latent_bytes, nbytes4);
         memcpy(h + J.off_blob, J.blob.data(), J.blob.size());
-        memset(h + J.off_status, 0, 64);
         if (!J.syn_f.empty()) memcpy(h + J.off_syn, J.syn_f.data(), J.syn_f.size() * 4);
         int8_t *lat = jobs[i].d_latents;
         if (!lat) lat = reinterpret_cast<int8_t *>(ctx->scratch.p + J.off_lat);
@@ -1280,16 +1325,17 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         S.n_words = (int64_t)(nbytes4 / 4);
         S.latents = lat;
         S.blob = dv + J.off_blob;
-        S.status = reinterpret_cast<int32_t *>(dv + J.off_status);
+        S.status = reinterpret_cast<int32_t *>(dv + off_status) + 16 * (size_t)i;
         S.out_words = d_out_words ? d_out_words[i] : nullptr;
         S.out_cap = d_out_words ? out_cap : 0;
     }
     for (int t = 0; t < n_jobs; t++)
         memcpy(h + off_streams + sizeof(EntStream) * (size_t)t, &P[(size_t)order[(size_t)t]].es, sizeof(EntStream));
+    memset(h + off_status, 0, A.end - off_status);
 
     if (tail) fill_tail(T, P, jobs, d_lat, h, dv, d_scr_tail);
-    CUDA_TRY(cudaMemcpyAsync(dv, h, up, cudaMemcpyHostToDevice, st));
-    ctx->last_upload_bytes = up;
+    CUDA_TRY(cudaMemcpyAsync(dv, h, A.end, cudaMemcpyHostToDevice, st));
+    ctx->last_upload_bytes = A.end;
     CUDA_TRY(cudaEventRecord(ctx->ev[1], st));
 
     int t = 0, g = 0;
@@ -1346,31 +1392,22 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         }
     }
     CUDA_TRY(cudaEventRecord(ctx->ev[3], st));
-    // statuses back
-    for (int i = 0; i < n_jobs; i++)
-        CUDA_TRY(cudaMemcpyAsync(h + P[(size_t)i].off_status, dv + P[(size_t)i].off_status, 64, cudaMemcpyDeviceToHost, st));
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "kernel execution failed: %s", cudaGetErrorString(se));
+    if ((rc = download(A, off_status, st, "kernel"))) return rc;
     cudaEventElapsedTime(&ctx->last_ms[2], ctx->ev[0], ctx->ev[1]);
     cudaEventElapsedTime(&ctx->last_ms[0], ctx->ev[1], ctx->ev[2]);
     cudaEventElapsedTime(&ctx->last_ms[1], ctx->ev[2], ctx->ev[3]);
-    int first = CCD_OK;
-    for (int i = 0; i < n_jobs; i++) {
-        const int32_t *s = reinterpret_cast<const int32_t *>(h + P[(size_t)i].off_status);
-        if (statuses) memcpy(statuses[i], s, 64);
-        memcpy(ctx->last_status, s, 64);
-        if (s[0] != 0) {
-            jobs[i].status = s[0];
-            if (!first) first = fail(s[0], "job %d: corrupt latent payload (range decoder desynchronised)", i);
-        }
-    }
-    return first;
+    const auto *words = reinterpret_cast<const int32_t(*)[16]>(h + off_status);
+    if (statuses) memcpy(statuses, words, sizeof(int32_t[16]) * (size_t)n_jobs);
+    memcpy(ctx->last_status, words[n_jobs - 1], sizeof(int32_t[16]));
+    return report(jobs, n_jobs, words, [&](int i) {
+        return fail(jobs[i].status, "job %d: corrupt latent payload (range decoder desynchronised)", i);
+    });
 }
 
 static int decode_impl(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int64_t *const *nn_ints, bool tail, int mode,
                        uint64_t seed, uint32_t *const *d_out_words, int64_t out_cap, int32_t (*statuses)[16],
                        void *cuda_stream) {
-    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int {
         return decode_impl_body(ctx, jobs, n_jobs, nn_ints, tail, mode, seed, d_out_words, out_cap, statuses, st);
     });
 }
@@ -1411,31 +1448,23 @@ int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
 }
 
 static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaStream_t st) {
-    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
-    if (n_jobs == 0) return CCD_OK;
     std::vector<PreparedJob> P((size_t)n_jobs);
     std::vector<RateTile> tiles;
     // tiles of job i, decode-order grid gi: [tile_at[i][gi], tile_at[i][gi + 1])
     std::vector<std::vector<size_t>> tile_at((size_t)n_jobs);
-    std::vector<size_t> off_blob((size_t)n_jobs), off_es((size_t)n_jobs), off_bad((size_t)n_jobs);
     std::vector<RateSpatialDev> sp;
     int64_t max_pixels = 0;
-    size_t up = 0, smem = 0;
+    Arena A;
+    size_t smem = 0;
     for (int i = 0; i < n_jobs; i++) {
         CcdRateJob &R = jobs[i];
-        R.status = CCD_OK;
         R.bad_index = -1;
         if (!R.desc || !R.nn_ints || !R.d_latents || !R.d_bits) return R.status = fail(CCD_ERR_ARG, "job %d: null pointer", i);
         PreparedJob &J = P[(size_t)i];
         J.d = R.desc;
         int rc = prepare_job(J, R.nn_ints);  // the decoder's build_arm / pack_arm / pack_ifce and fast-path choice
         if (rc) return R.status = rc;
-        off_blob[(size_t)i] = up;
-        up += al(J.blob.size());
-        off_es[(size_t)i] = up;
-        up += al(sizeof(EntStream));
-        off_bad[(size_t)i] = up;
-        up += al(8);
+        J.off_blob = A.take(J.blob.size());
         smem = std::max(smem, ccd_rate_smem_bytes(J.es.arm_blob_bytes, J.es.ifce_blob_max));
         const CcdCoolChicDesc *d = J.d;
         tile_at[(size_t)i].push_back(tiles.size());
@@ -1467,83 +1496,62 @@ static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaS
     }
     if (tiles.size() > (size_t)INT32_MAX) return fail(CCD_ERR_UNSUPPORTED, "too many rate tiles");
     if (smem > CCD_SMEM_MAX) return fail(CCD_ERR_UNSUPPORTED, "rate pass needs %zu bytes of shared memory", smem);
-    const size_t off_jobs = up;
-    up += al(sizeof(RateJobDev) * (size_t)n_jobs);
-    const size_t off_tiles = up;
-    up += al(sizeof(RateTile) * tiles.size());
-    const size_t off_sp = up;
-    up += al(sizeof(RateSpatialDev) * sp.size());
-    const size_t off_part = up;
-    up += al(sizeof(double) * tiles.size());
-    unsigned char *h, *dv;
-    if (int rc = stage(ctx, up, h, dv)) return rc;
+    const size_t off_es = A.take(sizeof(EntStream) * (size_t)n_jobs);
+    const size_t off_jobs = A.take(sizeof(RateJobDev) * (size_t)n_jobs);
+    const size_t off_tiles = A.take(sizeof(RateTile) * tiles.size());
+    const size_t off_sp = A.take(sizeof(RateSpatialDev) * sp.size());
+    // results: the bad words (~0 before the launch), then the partials, which are not uploaded
+    const size_t off_bad = A.take(sizeof(unsigned long long) * (size_t)n_jobs);
+    const size_t off_part = A.take(sizeof(double) * tiles.size());
+    if (int rc = stage(ctx, A)) return rc;
+    memset(A.h + off_bad, 0xff, sizeof(unsigned long long) * (size_t)n_jobs);
     for (int i = 0; i < n_jobs; i++) {
         PreparedJob &J = P[(size_t)i];
-        memcpy(h + off_blob[(size_t)i], J.blob.data(), J.blob.size());
+        memcpy(A.h + J.off_blob, J.blob.data(), J.blob.size());
         J.es.latents = const_cast<int8_t *>(jobs[i].d_latents);
-        J.es.blob = dv + off_blob[(size_t)i];
-        memcpy(h + off_es[(size_t)i], &J.es, sizeof(EntStream));
-        memset(h + off_bad[(size_t)i], 0xff, 8);
+        J.es.blob = A.dv + J.off_blob;
+        memcpy(A.h + off_es + sizeof(EntStream) * (size_t)i, &J.es, sizeof(EntStream));
         RateJobDev D;
-        D.es = reinterpret_cast<const EntStream *>(dv + off_es[(size_t)i]);
+        D.es = reinterpret_cast<const EntStream *>(A.dv + off_es) + i;
         D.bits = jobs[i].d_bits;
         D.freq = jobs[i].d_freq;
         D.mu_sc = jobs[i].d_mu_sc;
-        D.bad = reinterpret_cast<unsigned long long *>(dv + off_bad[(size_t)i]);
+        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
         D.kind = ccd_rate_kind(J.d->n_ctx, J.es.cf, J.fast);
-        memcpy(h + off_jobs + sizeof(RateJobDev) * (size_t)i, &D, sizeof(D));
+        memcpy(A.h + off_jobs + sizeof(RateJobDev) * (size_t)i, &D, sizeof(D));
     }
-    memcpy(h + off_tiles, tiles.data(), sizeof(RateTile) * tiles.size());
-    if (!sp.empty()) memcpy(h + off_sp, sp.data(), sizeof(RateSpatialDev) * sp.size());
-    CUDA_TRY(cudaMemcpyAsync(dv, h, off_part, cudaMemcpyHostToDevice, st));
-    double *d_part = reinterpret_cast<double *>(dv + off_part);
-    int e = ccd_rate_launch(reinterpret_cast<const RateTile *>(dv + off_tiles), (int)tiles.size(),
-                            reinterpret_cast<const RateJobDev *>(dv + off_jobs), smem, ctx->d_cdf, ctx->d_scale, d_part, st);
+    memcpy(A.h + off_tiles, tiles.data(), sizeof(RateTile) * tiles.size());
+    if (!sp.empty()) memcpy(A.h + off_sp, sp.data(), sizeof(RateSpatialDev) * sp.size());
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
+    int e = ccd_rate_launch(reinterpret_cast<const RateTile *>(A.dv + off_tiles), (int)tiles.size(),
+                            reinterpret_cast<const RateJobDev *>(A.dv + off_jobs), smem, ctx->d_cdf, ctx->d_scale,
+                            reinterpret_cast<double *>(A.dv + off_part), st);
     if (e != 0) return fail(CCD_ERR_CUDA, "rate kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     if (!sp.empty()) {
-        e = ccd_rate_spatial_launch(reinterpret_cast<const RateSpatialDev *>(dv + off_sp), (int)sp.size(), max_pixels, st);
+        e = ccd_rate_spatial_launch(reinterpret_cast<const RateSpatialDev *>(A.dv + off_sp), (int)sp.size(), max_pixels, st);
         if (e != 0) return fail(CCD_ERR_CUDA, "spatial rate launch failed: %s", cudaGetErrorString((cudaError_t)e));
     }
-    CUDA_TRY(cudaMemcpyAsync(h + off_part, d_part, sizeof(double) * tiles.size(), cudaMemcpyDeviceToHost, st));
-    for (int i = 0; i < n_jobs; i++) CUDA_TRY(cudaMemcpyAsync(h + off_bad[(size_t)i], dv + off_bad[(size_t)i], 8, cudaMemcpyDeviceToHost, st));
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "rate kernel execution failed: %s", cudaGetErrorString(se));
-    const double *part = reinterpret_cast<const double *>(h + off_part);
-    int first = CCD_OK;
+    if (int rc = download(A, off_bad, st, "rate kernel")) return rc;
+    const double *part = reinterpret_cast<const double *>(A.h + off_part);
     for (int i = 0; i < n_jobs; i++) {
-        CcdRateJob &R = jobs[i];
+        const std::vector<size_t> &at = tile_at[(size_t)i];  // a grid's sum: its tiles in order
         const int n_grids = P[(size_t)i].d->n_grids;
-        for (int g = 0; g < CCD_MAX_GRIDS; g++) R.grid_bits[g] = 0.0;
-        for (int gi = 0; gi < n_grids; gi++) {
-            double s = 0.0;  // tiles in order: a fixed-order sum
-            for (size_t t = tile_at[(size_t)i][(size_t)gi]; t < tile_at[(size_t)i][(size_t)gi + 1]; t++) s += part[t];
-            R.grid_bits[n_grids - 1 - gi] = s;
-        }
-        unsigned long long bad;
-        memcpy(&bad, h + off_bad[(size_t)i], 8);
-        if (bad != ~0ull) {
-            R.bad_index = (int64_t)bad;
-            R.status = CCD_ERR_ARG;
-            if (!first) first = fail(CCD_ERR_ARG, "job %d: latent %lld is outside [-64, 63]", i, (long long)bad);
-        }
+        for (int g = 0; g < CCD_MAX_GRIDS; g++) jobs[i].grid_bits[g] = 0.0;
+        for (int gi = 0; gi < n_grids; gi++) jobs[i].grid_bits[n_grids - 1 - gi] = ordered_sum(part + at[gi], at[gi + 1] - at[gi]);
     }
-    return first;
+    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {
+        return fail(CCD_ERR_ARG, "job %d: latent %lld is outside [-64, 63]", i, (long long)jobs[i].bad_index);
+    });
 }
 
 int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_stream) {
-    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int { return latent_rate_body(ctx, jobs, n_jobs, st); });
+    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return latent_rate_body(ctx, jobs, n_jobs, st); });
 }
 
 static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, cudaStream_t st) {
-    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(CCD_ERR_ARG, "bad job list");
-    if (n_jobs == 0) return CCD_OK;
-    // pinned / device staging: the job array, then per job sse[3] (u64), bad (u64), max_abs[3] (u32)
-    const size_t off_res = al(sizeof(DistJobDev) * (size_t)n_jobs), res_bytes = 48;
-    const size_t up = off_res + res_bytes * (size_t)n_jobs;
     int64_t max_pixels = 1;
     for (int i = 0; i < n_jobs; i++) {
         CcdDistJob &J = jobs[i];
-        J.status = CCD_OK;
         J.bad_index = -1;
         if (!J.d_planes[0] || !J.d_planes[1] || !J.d_planes[2] || !J.d_src || J.h < 1 || J.w < 1)
             return J.status = fail(CCD_ERR_ARG, "job %d: bad argument", i);
@@ -1556,13 +1564,15 @@ static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, 
         max_pixels = std::max(max_pixels, (int64_t)J.h * J.w);
     }
     if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
-    unsigned char *h, *dv;
-    if (int rc = stage(ctx, up, h, dv)) return rc;
-    memset(h + off_res, 0, res_bytes * (size_t)n_jobs);
+    // the job array, then the results: sse[n][3] and max_abs[n][3] zeroed, bad[n] ~0
+    Arena A;
+    const size_t n = (size_t)n_jobs, off_jobs = A.take(sizeof(DistJobDev) * n), off_sse = A.take(24 * n);
+    const size_t off_bad = A.take(8 * n, 8), off_max = A.take(12 * n, 4);
+    if (int rc = stage(ctx, A)) return rc;
+    memset(A.h + off_sse, 0, A.end - off_sse);
+    memset(A.h + off_bad, 0xff, 8 * n);
     for (int i = 0; i < n_jobs; i++) {
         const CcdDistJob &J = jobs[i];
-        unsigned char *res = dv + off_res + res_bytes * (size_t)i;
-        memset(h + off_res + res_bytes * (size_t)i + 24, 0xff, 8);
         DistJobDev D;
         for (int c = 0; c < 3; c++) D.p[c] = J.d_planes[c];
         D.src = J.d_src;
@@ -1575,36 +1585,27 @@ static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, 
         D.M = (float)M;
         D.M2 = (float)(M * M);
         D.wide = J.bitdepth > 8;
-        D.sse = reinterpret_cast<unsigned long long *>(res);
-        D.bad = reinterpret_cast<unsigned long long *>(res + 24);
-        D.max_abs = reinterpret_cast<unsigned int *>(res + 32);
-        memcpy(h + sizeof(DistJobDev) * (size_t)i, &D, sizeof(D));
+        D.sse = reinterpret_cast<unsigned long long *>(A.dv + off_sse) + 3 * i;
+        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
+        D.max_abs = reinterpret_cast<unsigned int *>(A.dv + off_max) + 3 * i;
+        memcpy(A.h + off_jobs + sizeof(DistJobDev) * (size_t)i, &D, sizeof(D));
     }
-    CUDA_TRY(cudaMemcpyAsync(dv, h, up, cudaMemcpyHostToDevice, st));
-    int e = ccd_dist_launch(reinterpret_cast<const DistJobDev *>(dv), n_jobs, max_pixels, ctx->n_sm, st);
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, A.end, cudaMemcpyHostToDevice, st));
+    int e = ccd_dist_launch(reinterpret_cast<const DistJobDev *>(A.dv + off_jobs), n_jobs, max_pixels, ctx->n_sm, st);
     if (e != 0) return fail(CCD_ERR_CUDA, "frame distortion launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    CUDA_TRY(cudaMemcpyAsync(h + off_res, dv + off_res, res_bytes * (size_t)n_jobs, cudaMemcpyDeviceToHost, st));
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "frame distortion execution failed: %s", cudaGetErrorString(se));
-    int first = CCD_OK;
+    if (int rc = download(A, off_sse, st, "frame distortion")) return rc;
     for (int i = 0; i < n_jobs; i++) {
-        CcdDistJob &J = jobs[i];
-        const unsigned char *res = h + off_res + res_bytes * (size_t)i;
-        unsigned long long bad;
-        memcpy(J.sse, res, 24);
-        memcpy(&bad, res + 24, 8);
-        memcpy(J.max_abs, res + 32, 12);
-        if (bad != ~0ull) {
-            J.bad_index = (int64_t)bad;
-            J.status = CCD_ERR_ARG;
-            if (!first) first = fail(CCD_ERR_ARG, "job %d: decoded sample %lld is off the k / (2^%d - 1) grid", i, (long long)bad, J.bitdepth);
-        }
+        memcpy(jobs[i].sse, A.h + off_sse + 24 * (size_t)i, 24);
+        memcpy(jobs[i].max_abs, A.h + off_max + 12 * (size_t)i, 12);
     }
-    return first;
+    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {
+        return fail(CCD_ERR_ARG, "job %d: decoded sample %lld is off the k / (2^%d - 1) grid", i,
+                    (long long)jobs[i].bad_index, jobs[i].bitdepth);
+    });
 }
 
 int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cuda_stream) {
-    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int { return frame_distortion_body(ctx, jobs, n_jobs, st); });
+    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return frame_distortion_body(ctx, jobs, n_jobs, st); });
 }
 
 int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitdepth, int data_type, float *d_out_a,
@@ -1682,9 +1683,9 @@ int ccd_inter_stats(CcdContext *ctx, const CcdInterFrame *frame, CcdInterStats *
         if (layout < 0 || layout > 1 || (layout == 1 && frame->frame_data_type == 1))
             return fail(CCD_ERR_ARG, "bad source layout %d for frame_data_type %d", layout, frame->frame_data_type);
         const int64_t n_ctas = ccd_inter_stats_ctas(L.h, L.w);
-        const size_t bytes = sizeof(double) * 4 * (size_t)n_ctas;
-        unsigned char *h, *dv;
-        if (int rc = stage(ctx, bytes, h, dv)) return rc;
+        Arena A;  // results only: the partials, which need no initial value (nothing is uploaded)
+        const size_t off_part = A.take(sizeof(double) * 4 * (size_t)n_ctas);
+        if (int rc = stage(ctx, A)) return rc;
         InterStatsOut o{};
         o.src = stats->d_src;
         o.src_hwc = layout;
@@ -1693,15 +1694,11 @@ int ccd_inter_stats(CcdContext *ctx, const CcdInterFrame *frame, CcdInterStats *
         o.alpha = stats->d_alpha;
         o.beta = stats->d_beta;
         o.pred = stats->d_pred;
-        o.part = reinterpret_cast<double *>(dv);
+        o.part = reinterpret_cast<double *>(A.dv + off_part);
         if (int rc = inter_launched(ccd_inter_stats_launch(L, o, st), L.filter_size)) return rc;
-        CUDA_TRY(cudaMemcpyAsync(h, dv, bytes, cudaMemcpyDeviceToHost, st));
-        cudaError_t se = cudaStreamSynchronize(st);
-        if (se != cudaSuccess) return fail(CCD_ERR_CUDA, "inter_stats execution failed: %s", cudaGetErrorString(se));
-        const double *part = reinterpret_cast<const double *>(h);
-        for (int k = 0; k < 4; k++) stats->sums[k] = 0.0;
-        for (int64_t b = 0; b < n_ctas; b++)  // tiles in order: a fixed-order sum
-            for (int k = 0; k < 4; k++) stats->sums[k] += part[4 * b + k];
+        if (int rc = download(A, off_part, st, "inter_stats")) return rc;
+        const double *part = reinterpret_cast<const double *>(A.h + off_part);
+        for (int k = 0; k < 4; k++) stats->sums[k] = ordered_sum(part + k, (size_t)n_ctas, 4);  // CTAs in order
         return CCD_OK;
     });
 }

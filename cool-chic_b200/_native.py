@@ -28,7 +28,7 @@ EXPORTS = [
     "ccd_version", "ccd_sizeof_desc", "ccd_last_error", "ccd_create", "ccd_destroy", "ccd_nn_count",
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
     "ccd_encode_latents", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
-    "ccd_latent_rate", "ccd_frame_distortion", "ccd_inter_stats",
+    "ccd_latent_rate", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
     "ccd_debug_entropy_plan",
 ]
@@ -78,6 +78,23 @@ class CcdDistJob(ctypes.Structure):
         ("d_map", ctypes.c_void_p),
         ("sse", ctypes.c_uint64 * 3),
         ("max_abs", ctypes.c_uint32 * 3),
+        ("bad_index", ctypes.c_int64),
+        ("status", ctypes.c_int32),
+    ]
+
+
+class CcdSsimJob(ctypes.Structure):
+    _fields_ = [
+        ("d_planes", ctypes.c_void_p * 3),
+        ("d_src", ctypes.c_void_p),
+        ("h", ctypes.c_int32),
+        ("w", ctypes.c_int32),
+        ("chroma_shift", ctypes.c_int32),
+        ("bitdepth", ctypes.c_int32),
+        ("src_layout", ctypes.c_int32),
+        ("d_map", ctypes.c_void_p * 3),
+        ("cs", (ctypes.c_double * 5) * 3),
+        ("ssim", (ctypes.c_double * 5) * 3),
         ("bad_index", ctypes.c_int64),
         ("status", ctypes.c_int32),
     ]
@@ -173,6 +190,8 @@ def load_library():
         L.ccd_latent_rate.argtypes = [vp, ctypes.POINTER(CcdRateJob), ci, vp]
         L.ccd_frame_distortion.restype = ci
         L.ccd_frame_distortion.argtypes = [vp, ctypes.POINTER(CcdDistJob), ci, vp]
+        L.ccd_frame_ssim.restype = ci
+        L.ccd_frame_ssim.argtypes = [vp, ctypes.POINTER(CcdSsimJob), ci, vp]
         L.ccd_inter_stats.restype = ci
         L.ccd_inter_stats.argtypes = [vp, ctypes.POINTER(CcdInterFrame), ctypes.POINTER(CcdInterStats), vp]
         L.ccd_debug_laplace_domain.restype = ci
@@ -524,16 +543,12 @@ class Context:
             res[i]["grid_bits"] = [float(jobs[i].grid_bits[g]) for g in range(descs[i].n_grids)]
         return res
 
-    def frame_distortion(self, frames, sources: Sequence[torch.Tensor], layouts: Sequence[str],
-                         want_maps: bool = False) -> List[dict]:
-        """Distortion of finished frames against their source samples (``ccd_frame_distortion``), one launch for all.
-        ``frames[i]``: a FrameData on this device; ``sources[i]``: its source samples on this device as read from the
-        file (uint8, or int16 holding the uint16 samples), in layout ``layouts[i]`` ("planar" or "hwc").  Per frame a
-        dict with ``sse`` and ``max_abs`` (three ints, one per plane) and on request ``map`` ([H, W] float32 CUDA,
-        fp32(sum_c d_c^2) / fp32(M^2)).  An off-grid decoded sample raises CcdError with ``bad_index`` per frame."""
+    def _frame_jobs(self, job_type, frames, sources, layouts):
+        """The job array of a call that compares finished frames with their source samples (frame_distortion,
+        frame_ssim), the tensors it points into, and each frame's planes."""
         n = len(frames)
-        jobs = (CcdDistJob * n)()
-        keep, res = [], []
+        jobs = (job_type * n)()
+        keep, planes = [], []
         for i, (fd, src, lay) in enumerate(zip(frames, sources, layouts)):
             ts, cs = _planes(fd.data, fd.frame_data_type)
             h, w = ts[0].shape[-2:]
@@ -542,21 +557,57 @@ class Context:
             if src.numel() != h * w + 2 * (h >> cs) * (w >> cs):
                 raise ValueError(f"sources[{i}] holds {src.numel()} samples, a {h}x{w} {fd.frame_data_type} frame has "
                                  f"{h * w + 2 * (h >> cs) * (w >> cs)}")
-            r = {}
-            if want_maps:
-                r["map"] = torch.empty((h, w), dtype=torch.float32, device=self.torch_device)
             keep += [ts, src]
+            planes.append(ts)
             for c in range(3):
                 jobs[i].d_planes[c] = ts[c].data_ptr()
             jobs[i].d_src = src.data_ptr()
             jobs[i].h, jobs[i].w, jobs[i].chroma_shift, jobs[i].bitdepth = h, w, cs, int(fd.bitdepth)
             jobs[i].src_layout = SOURCE_LAYOUTS[lay]
-            jobs[i].d_map = r["map"].data_ptr() if want_maps else None
+        return jobs, keep, planes
+
+    def frame_distortion(self, frames, sources: Sequence[torch.Tensor], layouts: Sequence[str],
+                         want_maps: bool = False) -> List[dict]:
+        """Distortion of finished frames against their source samples (``ccd_frame_distortion``), one launch for all.
+        ``frames[i]``: a FrameData on this device; ``sources[i]``: its source samples on this device as read from the
+        file (uint8, or int16 holding the uint16 samples), in layout ``layouts[i]`` ("planar" or "hwc").  Per frame a
+        dict with ``sse`` and ``max_abs`` (three ints, one per plane) and on request ``map`` ([H, W] float32 CUDA,
+        fp32(sum_c d_c^2) / fp32(M^2)).  An off-grid decoded sample raises CcdError with ``bad_index`` per frame."""
+        n = len(frames)
+        jobs, keep, planes = self._frame_jobs(CcdDistJob, frames, sources, layouts)
+        res = []
+        for i in range(n):
+            r = {}
+            if want_maps:
+                r["map"] = torch.empty(tuple(planes[i][0].shape[-2:]), dtype=torch.float32, device=self.torch_device)
+                jobs[i].d_map = r["map"].data_ptr()
             res.append(r)
         _check(self._lib.ccd_frame_distortion(self._h, jobs, n, self._stream()), jobs)
         for i in range(n):
             res[i]["sse"] = [int(jobs[i].sse[c]) for c in range(3)]
             res[i]["max_abs"] = [int(jobs[i].max_abs[c]) for c in range(3)]
+        return res
+
+    def frame_ssim(self, frames, sources: Sequence[torch.Tensor], layouts: Sequence[str],
+                   want_maps: bool = False) -> List[dict]:
+        """MS-SSIM statistics of finished frames against their source samples (``ccd_frame_ssim``), five launches for
+        all (one per scale).  Arguments as for frame_distortion; every plane needs both sides >= 176.  Per frame a dict
+        with ``cs`` and ``ssim``: per plane, the five per-scale means of cs and of l * cs (f64, the same on every run),
+        and on request ``maps``: per plane the scale-0 SSIM map ([h_c - 10, w_c - 10] float32 CUDA)."""
+        n = len(frames)
+        jobs, keep, planes = self._frame_jobs(CcdSsimJob, frames, sources, layouts)
+        res = []
+        for i in range(n):
+            r = {}
+            if want_maps:
+                r["maps"] = [torch.empty((max(t.shape[-2] - 10, 0), max(t.shape[-1] - 10, 0)), dtype=torch.float32,
+                                         device=self.torch_device) for t in planes[i]]
+                jobs[i].d_map[:] = [m.data_ptr() for m in r["maps"]]
+            res.append(r)
+        _check(self._lib.ccd_frame_ssim(self._h, jobs, n, self._stream()), jobs)
+        for i in range(n):
+            res[i]["cs"] = [list(jobs[i].cs[c]) for c in range(3)]
+            res[i]["ssim"] = [list(jobs[i].ssim[c]) for c in range(3)]
         return res
 
     def inter_stats(self, residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow, warp_filter_size,

@@ -11,6 +11,10 @@ Decoding goes through ``decode_video_bytes``; the prediction statistics are take
 residue and motion just before that frame is reconstructed (``ccd_inter_stats``), and one ``ccd_frame_distortion``
 call then covers every frame.  The source frames are read and uploaded in one pinned host-to-device copy, as the
 integers stored in the file.
+
+On request, MS-SSIM (Wang, Simoncelli and Bovik 2003; DESIGN §4.6) from the same integers: one ``ccd_frame_ssim`` call
+for every frame whose planes all have both sides of at least 176 samples (five scales of at least 11), formed per plane
+on the host from the per-scale means, and per frame the pixel-weighted mean over the planes.  Smaller frames get None.
 """
 import math
 from dataclasses import dataclass, field
@@ -36,6 +40,26 @@ def pred_to_db(sse: float, n: int) -> float:
     return -10 * math.log10(sse / n + 1e-10)
 
 
+MS_SSIM_WEIGHTS = (0.0448, 0.2856, 0.3001, 0.2363, 0.1333)
+MS_SSIM_MIN_SIDE = 176  # 11 samples at the fifth scale
+
+
+def ms_ssim_from_scales(cs: List[float], ssim: List[float]) -> float:
+    """MS-SSIM of one plane from its five per-scale means of cs and of l * cs: prod_{j<4} max(cs_j, 0)^w_j *
+    max(ssim_4, 0)^w_4."""
+    w = MS_SSIM_WEIGHTS
+    v = 1.0
+    for j in range(4):
+        v *= max(cs[j], 0.0) ** w[j]
+    return v * max(ssim[4], 0.0) ** w[4]
+
+
+def ms_ssim_applies(img_size, frame_data_type: str) -> bool:
+    """Whether every plane of an (h, w) frame has both sides >= 176 (4:2:0 chroma: (h / 2, w / 2))."""
+    cs = 1 if frame_data_type == "yuv420" else 0
+    return min(img_size) >> cs >= MS_SSIM_MIN_SIDE
+
+
 @dataclass
 class FrameQuality:
     """Quality of one decoded frame.  Planes are y / u / v, or r / g / b for rgb frames."""
@@ -56,6 +80,8 @@ class FrameQuality:
     alpha_map: Optional[torch.Tensor] = None   # [H, W] (P / B)
     beta_map: Optional[torch.Tensor] = None    # [H, W] (P / B)
     pred_map: Optional[torch.Tensor] = None    # [3, H, W] (P / B)
+    ms_ssim_planes: Optional[List[float]] = None        # per plane; None: not asked for, or a plane below 176
+    ssim_maps: Optional[List[torch.Tensor]] = None      # per plane, [h_c - 10, w_c - 10] scale-0 SSIM map
     plane_mse: List[float] = field(init=False)
 
     def __post_init__(self):
@@ -81,6 +107,21 @@ class FrameQuality:
     psnr_u_db = property(lambda self: dist_to_db(self.plane_mse[1]))
     psnr_v_db = property(lambda self: dist_to_db(self.plane_mse[2]))
 
+    @property
+    def ms_ssim(self) -> Optional[float]:
+        """Pixel-weighted mean of the planes' MS-SSIM (the rule of training/loss.py:121-155)."""
+        if self.ms_ssim_planes is None:
+            return None
+        return sum(n * m for n, m in zip(self.n_samples, self.ms_ssim_planes)) / sum(self.n_samples)
+
+    @property
+    def ms_ssim_db(self) -> Optional[float]:
+        return None if self.ms_ssim_planes is None else dist_to_db(1.0 - self.ms_ssim)
+
+    ms_ssim_y = property(lambda self: None if self.ms_ssim_planes is None else self.ms_ssim_planes[0])
+    ms_ssim_u = property(lambda self: None if self.ms_ssim_planes is None else self.ms_ssim_planes[1])
+    ms_ssim_v = property(lambda self: None if self.ms_ssim_planes is None else self.ms_ssim_planes[2])
+
 
 def _frame_layout(buf, max_decoding_order: int):
     """Per frame in coding order: (frame header, display index, n_bytes, (h, w)), without decoding anything."""
@@ -101,9 +142,10 @@ def _frame_layout(buf, max_decoding_order: int):
 
 @torch.no_grad()
 def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int = 0, max_decoding_order: int = -1,
-                  device: int = 0, want_maps: bool = False) -> Dict[str, FrameQuality]:
+                  device: int = 0, want_maps: bool = False, ms_ssim: bool = False) -> Dict[str, FrameQuality]:
     """Quality of every frame of an image / video bitstream against its source file (.yuv / .png / .ppm):
-    ``{str(display_idx): FrameQuality}`` in display order.  A source whose format, bitdepth or size differs from the
+    ``{str(display_idx): FrameQuality}`` in display order.  ``ms_ssim`` adds MS-SSIM for every frame whose planes
+    all have both sides >= 176 (``ms_ssim_planes`` stays None for the others), with the SSIM maps if ``want_maps``.  A source whose format, bitdepth or size differs from the
     decoded frames, or that has too few frames, raises ValueError before anything runs on the device."""
     frames = _frame_layout(memoryview(bytes(bitstream_bytes)), max_decoding_order)
     by_display = {}
@@ -156,6 +198,13 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
     order = sorted(by_display)
     dist = ctx.frame_distortion([decoded[str(d)] for d in order], [sources[d] for d in order],
                                 [by_display[d][3].layout for d in order], want_maps=want_maps)
+    ssim = {}
+    if ms_ssim:
+        big = [d for d in order if ms_ssim_applies(by_display[d][3].img_size, by_display[d][3].frame_data_type)]
+        if big:
+            res = ctx.frame_ssim([decoded[str(d)] for d in big], [sources[d] for d in big],
+                                 [by_display[d][3].layout for d in big], want_maps=want_maps)
+            ssim = dict(zip(big, res))
     out = {}
     for d, r in zip(order, dist):
         _, fh, n_bytes, s = by_display[d]
@@ -172,5 +221,8 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
             q.pred_psnr_db = pred_to_db(st["sums"][2], 3 * h * w)
             q.dummy_pred_psnr_db = pred_to_db(st["sums"][3], 3 * h * w)
             q.alpha_map, q.beta_map, q.pred_map = st.get("alpha"), st.get("beta"), st.get("pred")
+        if d in ssim:
+            q.ms_ssim_planes = [ms_ssim_from_scales(c, s_) for c, s_ in zip(ssim[d]["cs"], ssim[d]["ssim"])]
+            q.ssim_maps = ssim[d].get("maps")
         out[str(d)] = q
     return out

@@ -407,7 +407,7 @@ struct CcdContext {
     float *d_scale = nullptr;
     uint32_t *d_cdf = nullptr;
     DeviceBuf upload;   // words / blobs / stream structs / statuses / synthesis weights
-    DeviceBuf scratch;  // synthesis intermediates, latents when the caller does not want them
+    DeviceBuf scratch;  // synthesis intermediates, latents when the caller does not want them, MS-SSIM pyramid levels
     unsigned char *h_pin = nullptr;
     size_t h_pin_cap = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1548,20 +1548,33 @@ int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_st
     return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return latent_rate_body(ctx, jobs, n_jobs, st); });
 }
 
+// The checks of a job that compares a finished frame with its source samples (CcdDistJob, CcdSsimJob)
+extern "C++" template <class Job>
+int check_frame_job(Job &J, int i) {
+    J.bad_index = -1;
+    if (!J.d_planes[0] || !J.d_planes[1] || !J.d_planes[2] || !J.d_src || J.h < 1 || J.w < 1)
+        return J.status = fail(CCD_ERR_ARG, "job %d: bad argument", i);
+    if (J.bitdepth < 1 || J.bitdepth > 16) return J.status = fail(CCD_ERR_ARG, "job %d: bad bitdepth %d", i, J.bitdepth);
+    if (J.chroma_shift < 0 || J.chroma_shift > 1 || J.src_layout < 0 || J.src_layout > 1 || (J.src_layout && J.chroma_shift))
+        return J.status = fail(CCD_ERR_ARG, "job %d: bad layout", i);
+    if (J.chroma_shift && ((J.h | J.w) & 1))
+        return J.status = fail(CCD_ERR_ARG, "job %d: 4:2:0 needs even frame sizes, got %dx%d", i, J.h, J.w);
+    if ((int64_t)J.h * J.w > (int64_t)INT32_MAX / 3) return J.status = fail(CCD_ERR_UNSUPPORTED, "job %d: frame too large", i);
+    return CCD_OK;
+}
+
+// The message of a job whose decoded frame has a sample off the k / M grid (report(), after the kernel)
+extern "C++" template <class Job>
+int off_grid_error(const Job &J, int i) {
+    return fail(CCD_ERR_ARG, "job %d: decoded sample %lld is off the k / (2^%d - 1) grid", i, (long long)J.bad_index,
+                J.bitdepth);
+}
+
 static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, cudaStream_t st) {
     int64_t max_pixels = 1;
     for (int i = 0; i < n_jobs; i++) {
-        CcdDistJob &J = jobs[i];
-        J.bad_index = -1;
-        if (!J.d_planes[0] || !J.d_planes[1] || !J.d_planes[2] || !J.d_src || J.h < 1 || J.w < 1)
-            return J.status = fail(CCD_ERR_ARG, "job %d: bad argument", i);
-        if (J.bitdepth < 1 || J.bitdepth > 16) return J.status = fail(CCD_ERR_ARG, "job %d: bad bitdepth %d", i, J.bitdepth);
-        if (J.chroma_shift < 0 || J.chroma_shift > 1 || J.src_layout < 0 || J.src_layout > 1 || (J.src_layout && J.chroma_shift))
-            return J.status = fail(CCD_ERR_ARG, "job %d: bad layout", i);
-        if (J.chroma_shift && ((J.h | J.w) & 1))
-            return J.status = fail(CCD_ERR_ARG, "job %d: 4:2:0 needs even frame sizes, got %dx%d", i, J.h, J.w);
-        if ((int64_t)J.h * J.w > (int64_t)INT32_MAX / 3) return J.status = fail(CCD_ERR_UNSUPPORTED, "job %d: frame too large", i);
-        max_pixels = std::max(max_pixels, (int64_t)J.h * J.w);
+        if (int rc = check_frame_job(jobs[i], i)) return rc;
+        max_pixels = std::max(max_pixels, (int64_t)jobs[i].h * jobs[i].w);
     }
     if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
     // the job array, then the results: sse[n][3] and max_abs[n][3] zeroed, bad[n] ~0
@@ -1598,14 +1611,103 @@ static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, 
         memcpy(jobs[i].sse, A.h + off_sse + 24 * (size_t)i, 24);
         memcpy(jobs[i].max_abs, A.h + off_max + 12 * (size_t)i, 12);
     }
-    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {
-        return fail(CCD_ERR_ARG, "job %d: decoded sample %lld is off the k / (2^%d - 1) grid", i,
-                    (long long)jobs[i].bad_index, jobs[i].bitdepth);
-    });
+    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) { return off_grid_error(jobs[i], i); });
 }
 
 int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cuda_stream) {
     return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return frame_distortion_body(ctx, jobs, n_jobs, st); });
+}
+
+static int frame_ssim_body(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, cudaStream_t st) {
+    constexpr int S = CCD_SSIM_SCALES;
+    const size_t n = (size_t)n_jobs;
+    auto side = [&](int i, int c, int j, bool width) {  // plane c of job i at scale j
+        const CcdSsimJob &J = jobs[i];
+        return ((width ? J.w : J.h) >> (c ? J.chroma_shift : 0)) >> j;
+    };
+    auto tiles = [&](int i, int c, int j) { return ccd_ssim_tiles(side(i, c, j, false), side(i, c, j, true)); };
+    // the job's partials at scale j start at part_at[i * S + j] (pairs, planes in order); the pyramid levels 1..4 of
+    // every plane of every job, one after the other, in the context's scratch
+    std::vector<size_t> part_at(n * S);
+    size_t n_part = 0, pyr_bytes = 0;
+    int max_tiles[S] = {0, 0, 0, 0, 0};
+    for (int i = 0; i < n_jobs; i++) {
+        if (int rc = check_frame_job(jobs[i], i)) return rc;
+        for (int c = 0; c < 3; c++)
+            if (std::min(side(i, c, 0, false), side(i, c, 0, true)) < 176)
+                return jobs[i].status = fail(CCD_ERR_ARG, "job %d: plane %d is %dx%d, MS-SSIM needs both sides >= 176", i, c,
+                                             side(i, c, 0, true), side(i, c, 0, false));
+        for (int j = 0; j < S; j++) {
+            part_at[(size_t)i * S + j] = n_part;
+            const int t = tiles(i, 0, j) + tiles(i, 1, j) + tiles(i, 2, j);
+            max_tiles[j] = std::max(max_tiles[j], t);
+            n_part += (size_t)t;
+            for (int c = 0; j > 0 && c < 3; c++) pyr_bytes += al(sizeof(uint2) * (size_t)side(i, c, j, false) * side(i, c, j, true));
+        }
+    }
+    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
+    // the job array, then the results: bad[n] ~0, then the partials, which are not uploaded
+    Arena A;
+    const size_t off_jobs = A.take(sizeof(SsimJobDev) * n), off_bad = A.take(8 * n, 8);
+    const size_t off_part = A.take(2 * sizeof(double) * n_part, 8);
+    if (int rc = stage(ctx, A)) return rc;
+    if (int rc = ensure_dev(ctx->scratch, pyr_bytes)) return rc;
+    memset(A.h + off_bad, 0xff, 8 * n);
+    double *d_part = reinterpret_cast<double *>(A.dv + off_part);
+    unsigned char *pyr = ctx->scratch.p;
+    for (int i = 0; i < n_jobs; i++) {
+        const CcdSsimJob &J = jobs[i];
+        SsimJobDev D;
+        memset(&D, 0, sizeof(D));
+        for (int c = 0; c < 3; c++) {
+            D.p[c] = J.d_planes[c];
+            D.map[c] = J.d_map[c];
+        }
+        for (int j = 0; j < S; j++) {
+            D.part[j] = d_part + 2 * part_at[(size_t)i * S + j];
+            for (int c = 0; j > 0 && c < 3; c++) {
+                D.lvl[c][j] = reinterpret_cast<uint2 *>(pyr);
+                pyr += al(sizeof(uint2) * (size_t)side(i, c, j, false) * side(i, c, j, true));
+            }
+        }
+        D.src = J.d_src;
+        D.h = J.h;
+        D.w = J.w;
+        D.cs = J.chroma_shift;
+        D.hwc = J.src_layout;
+        D.wide = J.bitdepth > 8;
+        const double M = (double)((1 << J.bitdepth) - 1);
+        D.M = (float)M;
+        D.C1 = (0.01 * M) * (0.01 * M);
+        D.C2 = (0.03 * M) * (0.03 * M);
+        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
+        memcpy(A.h + off_jobs + sizeof(SsimJobDev) * (size_t)i, &D, sizeof(D));
+    }
+    double g[11], gs = 0.0;  // the Gaussian window, sigma 1.5, normalised to sum 1
+    for (int k = 0; k < 11; k++) gs += (g[k] = std::exp(-(double)((k - 5) * (k - 5)) / (2.0 * 1.5 * 1.5)));
+    for (int k = 0; k < 11; k++) g[k] /= gs;
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
+    int e = ccd_ssim_launch(reinterpret_cast<const SsimJobDev *>(A.dv + off_jobs), n_jobs, max_tiles, g, st);
+    if (e != 0) return fail(CCD_ERR_CUDA, "MS-SSIM launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    if (int rc = download(A, off_bad, st, "MS-SSIM")) return rc;
+    const double *part = reinterpret_cast<const double *>(A.h + off_part);
+    for (int i = 0; i < n_jobs; i++) {
+        for (int j = 0; j < S; j++) {
+            const double *p = part + 2 * part_at[(size_t)i * S + j];  // the planes' tiles in order
+            for (int c = 0; c < 3; c++) {
+                const size_t t = (size_t)tiles(i, c, j);
+                const double n_pos = (double)(side(i, c, j, false) - CCD_SSIM_HALO) * (side(i, c, j, true) - CCD_SSIM_HALO);
+                jobs[i].cs[c][j] = ordered_sum(p, t, 2) / n_pos;
+                jobs[i].ssim[c][j] = ordered_sum(p + 1, t, 2) / n_pos;
+                p += 2 * t;
+            }
+        }
+    }
+    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) { return off_grid_error(jobs[i], i); });
+}
+
+int ccd_frame_ssim(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, void *cuda_stream) {
+    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return frame_ssim_body(ctx, jobs, n_jobs, st); });
 }
 
 int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitdepth, int data_type, float *d_out_a,

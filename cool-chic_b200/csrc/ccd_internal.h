@@ -218,6 +218,43 @@ struct DistJobDev {
 };
 int ccd_dist_launch(const DistJobDev *d_jobs, int n_jobs, int64_t max_pixels, int n_sm, cudaStream_t st);
 
+// A decoded sample read back to its integer kd = rint(v * M) (k_frame_dist, k_frame_ssim)
+struct DecodedSample {
+    float v, vm, kd;  // the decoded value, fp32(v * M), rint(v * M)
+};
+static __device__ __forceinline__ DecodedSample read_decoded(const float *p, unsigned j, float M) {
+    const float v = __ldg(p + j), vm = __fmul_rn(v, M);
+    return DecodedSample{v, vm, rintf(vm)};
+}
+// A decoded sample off the k / M grid: outside [0, 1] or more than 1/16 away.  A macro, not a function: written into
+// the condition of its if, it compiles to the same branches as k_frame_dist had before it was shared.
+#define CCD_OFF_GRID(D) (!((D).v >= 0.0f && (D).v <= 1.0f) || fabsf(__fsub_rn((D).vm, (D).kd)) > 0.0625f)
+
+// MS-SSIM (DESIGN §4.6): one k_frame_ssim launch per scale for every plane of every job of a call, blockIdx.y = job,
+// blockIdx.x = tile over the job's planes (plane 0's tiles, then plane 1's, then plane 2's, each row-major).  A tile owns
+// CCD_SSIM_T x CCD_SSIM_T samples of its plane's level (even origin) and reads a CCD_SSIM_HALO halo below and right.
+#define CCD_SSIM_T 32
+#define CCD_SSIM_HALO 10
+#define CCD_SSIM_SCALES 5
+struct SsimJobDev {
+    const float *p[3];          // finished planes (FrameData layout), read at scale 0
+    const void *src;            // source samples as for DistJobDev
+    float *map[3];              // optional scale-0 SSIM maps, [h_c - 10][w_c - 10]
+    uint2 *lvl[3][CCD_SSIM_SCALES];  // pyramid levels 1..4 per plane: (decoded, source) 2 x 2 sums of the level above
+    double *part[CCD_SSIM_SCALES];   // per scale: (sum cs, sum l cs) of each of the job's tiles, in tile order
+    int32_t h, w, cs, hwc, wide;
+    float M;
+    double C1, C2;              // (0.01 M)^2, (0.03 M)^2
+    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
+};
+// tiles of one plane of h x w samples at some level
+static __host__ __device__ __forceinline__ int ccd_ssim_tiles(int h, int w) {
+    return ((h + CCD_SSIM_T - 1) / CCD_SSIM_T) * ((w + CCD_SSIM_T - 1) / CCD_SSIM_T);
+}
+// five launches; max_tiles[j]: the most tiles of one job at scale j; g: the 11 Gaussian taps
+int ccd_ssim_launch(const SsimJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_SSIM_SCALES], const double g[11],
+                    cudaStream_t st);
+
 // P/B reconstruction (ccd_inter.cu); returns -1 for an unsupported filter size
 struct InterLaunch {
     const float *residue, *motion;  // [4|5][h][w], [2|4][h][w]

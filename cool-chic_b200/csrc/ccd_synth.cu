@@ -1526,6 +1526,10 @@ int ccd_pack_flat(const float *d_in, size_t n, int bitdepth, int sample_bytes, v
 // [H][W][3], never widened on the host).  A thread owns pixels of the luma grid; with 4:2:0 chroma only the thread of
 // the even (x, y) counts the chroma sample, the others read it only for the error map.  Sums are integers: exact, and
 // the same whatever the order of the atomics.
+static __device__ __forceinline__ int source_sample(const void *src, bool wide, size_t k) {
+    return wide ? (int)__ldg(static_cast<const uint16_t *>(src) + k) : (int)__ldg(static_cast<const uint8_t *>(src) + k);
+}
+
 __global__ void __launch_bounds__(256) k_frame_dist(const DistJobDev *__restrict__ jobs) {
     const DistJobDev &J = jobs[blockIdx.y];
     const unsigned w = (unsigned)J.w, cs = (unsigned)J.cs, n0 = (unsigned)J.h * w;
@@ -1544,17 +1548,16 @@ __global__ void __launch_bounds__(256) k_frame_dist(const DistJobDev *__restrict
             const unsigned j = c == 0 ? i : (y >> cs) * wc + (x >> cs);
             const unsigned pidx = c == 0 ? i : n0 + (unsigned)(c - 1) * n1 + j;  // planar (FrameData) sample index
             const size_t k = J.hwc ? (size_t)i * 3 + c : (size_t)pidx;
-            const float v = __ldg(J.p[c] + j);
-            const float vm = __fmul_rn(v, M), kd = rintf(vm);
-            const int ks = J.wide ? (int)__ldg(static_cast<const uint16_t *>(J.src) + k)
-                                  : (int)__ldg(static_cast<const uint8_t *>(J.src) + k);
+            const DecodedSample D = read_decoded(J.p[c], j, M);
+            const float kd = D.kd;
+            const int ks = source_sample(J.src, J.wide, k);
             const unsigned a = (unsigned)abs((int)kd - ks);
             const unsigned long long d2 = (unsigned long long)a * a;
             e += d2;
             if (c == 0 || own) {
                 s[c] += d2;
                 mx[c] = max(mx[c], a);
-                if (!(v >= 0.0f && v <= 1.0f) || fabsf(__fsub_rn(vm, kd)) > 0.0625f) bad = min(bad, (unsigned long long)pidx);
+                if (CCD_OFF_GRID(D)) bad = min(bad, (unsigned long long)pidx);
             }
         }
         if (want_map) J.map[i] = __fdiv_rn(__ull2float_rn(e), J.M2);
@@ -1582,6 +1585,181 @@ int ccd_dist_launch(const DistJobDev *d_jobs, int n_jobs, int64_t max_pixels, in
     k_frame_dist<<<dim3((unsigned)per_job, (unsigned)n_jobs, 1), 256, 0, st>>>(d_jobs);
     g_ccd_launches++;
     return (int)cudaGetLastError();
+}
+
+// ---- MS-SSIM against the source (DESIGN §4.6), one scale per launch.  x = the decoded image, y = the source, both as
+// the integer sums S_j of the 4^j samples a level-j sample covers: below 65535 * 256 < 2^24, so staged exactly in fp32
+// (68 KB of shared memory: three CTAs per SM); every moment is formed in f64 on S_j and scaled by 4^-j or 16^-j
+// afterwards, which is exact.  Per tile: stage (T + 10)^2 samples of both images, write the next level's T/2 x T/2
+// samples, filter the five moments horizontally then vertically (11 taps, valid positions only), and add cs and
+// l * cs of the tile's valid positions in a fixed order into one f64 partial each.
+namespace {
+constexpr int kSsimIn = CCD_SSIM_T + CCD_SSIM_HALO;  // staged rows and columns
+constexpr int kSsimK = 4;                            // consecutive outputs per thread in either pass
+constexpr int kSsimWarps = 8;
+constexpr size_t kSsimSmem = sizeof(float) * 2 * kSsimIn * kSsimIn + sizeof(double) * (5 * kSsimIn * CCD_SSIM_T + 2 * kSsimWarps);
+static_assert(CCD_SSIM_T == 32 && CCD_SSIM_T / kSsimK == kSsimWarps, "vertical pass: lane = column, warp = K rows");
+static_assert((CCD_SSIM_T / 2) * (CCD_SSIM_T / 2) == 32 * kSsimWarps, "one next-level sample per thread");
+struct SsimArgs {
+    double g[11];
+    int scale;
+};
+}  // namespace
+
+__global__ void __launch_bounds__(32 * kSsimWarps, 3) k_frame_ssim(const SsimJobDev *__restrict__ jobs, const SsimArgs a) {
+    constexpr int T = CCD_SSIM_T, K = kSsimK;
+    extern __shared__ double ssim_sm[];
+    double *sh = ssim_sm;                                 // [5][kSsimIn][T]: the horizontal pass
+    float *sx = reinterpret_cast<float *>(sh + 5 * kSsimIn * T), *sy = sx + kSsimIn * kSsimIn;  // [kSsimIn][kSsimIn]
+    double *sred = reinterpret_cast<double *>(sy + kSsimIn * kSsimIn);  // [warps][2]
+    const SsimJobDev &J = jobs[blockIdx.y];
+    const int j = a.scale, tid = (int)threadIdx.x;
+    int c = 0, t = (int)blockIdx.x, h = 0, w = 0;
+    for (;; c++) {  // the plane and tile of this CTA
+        if (c == 3) return;
+        h = (c ? J.h >> J.cs : J.h) >> j;
+        w = (c ? J.w >> J.cs : J.w) >> j;
+        const int n = ccd_ssim_tiles(h, w);
+        if (t < n) break;
+        t -= n;
+    }
+    const int tw = (w + T - 1) / T, y0 = t / tw * T, x0 = t % tw * T;
+
+    unsigned long long bad = ~0ull;
+    const unsigned n0 = (unsigned)J.h * J.w, n1 = (unsigned)(J.h >> J.cs) * (unsigned)(J.w >> J.cs);
+    for (int i = tid; i < kSsimIn * kSsimIn; i += 32 * kSsimWarps) {
+        const int r = i / kSsimIn, q = i - r * kSsimIn, y = y0 + r, x = x0 + q;
+        float vx = 0.0f, vy = 0.0f;  // integers below 2^24: exact
+        if (y < h && x < w) {
+            const unsigned s = (unsigned)y * (unsigned)w + (unsigned)x;
+            if (j == 0) {
+                const DecodedSample D = read_decoded(J.p[c], s, J.M);
+                const unsigned pidx = c == 0 ? s : n0 + (unsigned)(c - 1) * n1 + s;  // as k_frame_dist reports it
+                vx = D.kd;
+                vy = source_sample(J.src, J.wide, J.hwc ? (size_t)s * 3 + c : (size_t)pidx);
+                if (r < T && q < T && CCD_OFF_GRID(D)) bad = min(bad, (unsigned long long)pidx);
+            } else {
+                const uint2 v = J.lvl[c][j][s];
+                vx = (float)v.x;
+                vy = (float)v.y;
+            }
+        }
+        sx[i] = vx;
+        sy[i] = vy;
+    }
+    if (j == 0) {
+        for (int o = 16; o > 0; o >>= 1) bad = min(bad, __shfl_down_sync(0xffffffffu, bad, o));
+        if ((tid & 31) == 0 && bad != ~0ull) atomicMin(J.bad, bad);
+    }
+    __syncthreads();
+
+    if (j + 1 < CCD_SSIM_SCALES) {  // the next level: floor sizes, an odd last row or column is dropped
+        const int r = tid / (T / 2), q = tid % (T / 2), Y = (y0 >> 1) + r, X = (x0 >> 1) + q;
+        if (Y < (h >> 1) && X < (w >> 1)) {
+            const int k = 2 * r * kSsimIn + 2 * q;
+            J.lvl[c][j + 1][(size_t)Y * (w >> 1) + X] =
+                make_uint2((unsigned)(sx[k] + sx[k + 1] + sx[k + kSsimIn] + sx[k + kSsimIn + 1]),
+                           (unsigned)(sy[k] + sy[k + 1] + sy[k + kSsimIn] + sy[k + kSsimIn + 1]));
+        }
+    }
+
+    // horizontal pass: x, y, x^2, y^2, x y (the f64 products are exact: S_j < 2^24) over 11 columns
+    for (int task = tid; task < kSsimIn * (T / K); task += 32 * kSsimWarps) {
+        const int r = task / (T / K), q0 = task % (T / K) * K;
+        const float *rx = sx + r * kSsimIn + q0, *ry = sy + r * kSsimIn + q0;
+        double m[5][K];
+#pragma unroll
+        for (int k = 0; k < K; k++)
+#pragma unroll
+            for (int e = 0; e < 5; e++) m[e][k] = 0.0;
+#pragma unroll
+        for (int i = 0; i < K + 10; i++) {
+            const double x = rx[i], y = ry[i], v[5] = {x, y, x * x, y * y, x * y};
+#pragma unroll
+            for (int k = 0; k < K; k++) {
+                if (i - k < 0 || i - k > 10) continue;
+#pragma unroll
+                for (int e = 0; e < 5; e++) m[e][k] = fma(a.g[i - k], v[e], m[e][k]);
+            }
+        }
+#pragma unroll
+        for (int e = 0; e < 5; e++)
+#pragma unroll
+            for (int k = 0; k < K; k++) sh[(e * kSsimIn + r) * T + q0 + k] = m[e][k];
+    }
+    __syncthreads();
+
+    // vertical pass: lane = column, warp = K consecutive output rows
+    double s_cs = 0.0, s_ssim = 0.0;
+    {
+        const int q = tid & 31, r0 = (tid >> 5) * K;
+        double m[5][K];
+#pragma unroll
+        for (int k = 0; k < K; k++)
+#pragma unroll
+            for (int e = 0; e < 5; e++) m[e][k] = 0.0;
+#pragma unroll
+        for (int i = 0; i < K + 10; i++) {
+#pragma unroll
+            for (int e = 0; e < 5; e++) {
+                const double v = sh[(e * kSsimIn + r0 + i) * T + q];
+#pragma unroll
+                for (int k = 0; k < K; k++)
+                    if (i - k >= 0 && i - k <= 10) m[e][k] = fma(a.g[i - k], v, m[e][k]);
+            }
+        }
+        const double s1 = ldexp(1.0, -2 * j), s2 = __dmul_rn(s1, s1);
+        const int x = x0 + q, wo = w - CCD_SSIM_HALO, ho = h - CCD_SSIM_HALO;
+#pragma unroll
+        for (int k = 0; k < K; k++) {
+            const int y = y0 + r0 + k;
+            if (x >= wo || y >= ho) continue;
+            // no contraction: identical images give cs = l = 1 exactly
+            const double mx = __dmul_rn(m[0][k], s1), my = __dmul_rn(m[1][k], s1);
+            const double mxx = __dmul_rn(mx, mx), myy = __dmul_rn(my, my), mxy = __dmul_rn(mx, my);
+            const double vx = __dsub_rn(__dmul_rn(m[2][k], s2), mxx), vy = __dsub_rn(__dmul_rn(m[3][k], s2), myy);
+            const double cxy = __dsub_rn(__dmul_rn(m[4][k], s2), mxy);
+            const double cs = __ddiv_rn(__dadd_rn(__dmul_rn(2.0, cxy), J.C2), __dadd_rn(__dadd_rn(vx, vy), J.C2));
+            const double l = __ddiv_rn(__dadd_rn(__dmul_rn(2.0, mxy), J.C1), __dadd_rn(__dadd_rn(mxx, myy), J.C1));
+            const double ls = __dmul_rn(l, cs);
+            s_cs = __dadd_rn(s_cs, cs);
+            s_ssim = __dadd_rn(s_ssim, ls);
+            if (j == 0 && J.map[c]) J.map[c][(size_t)y * wo + x] = __double2float_rn(ls);
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) {  // lane butterfly, then the warps in order
+        s_cs += __shfl_xor_sync(0xffffffffu, s_cs, o);
+        s_ssim += __shfl_xor_sync(0xffffffffu, s_ssim, o);
+    }
+    if ((tid & 31) == 0) {
+        sred[2 * (tid >> 5)] = s_cs;
+        sred[2 * (tid >> 5) + 1] = s_ssim;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        double pc = 0.0, ps = 0.0;
+        for (int wi = 0; wi < kSsimWarps; wi++) {
+            pc += sred[2 * wi];
+            ps += sred[2 * wi + 1];
+        }
+        J.part[j][2 * blockIdx.x] = pc;
+        J.part[j][2 * blockIdx.x + 1] = ps;
+    }
+}
+
+int ccd_ssim_launch(const SsimJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_SSIM_SCALES], const double g[11],
+                    cudaStream_t st) {
+    cudaError_t e = cudaFuncSetAttribute(k_frame_ssim, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSsimSmem);
+    if (e != cudaSuccess) return (int)e;
+    SsimArgs a;
+    memcpy(a.g, g, sizeof(a.g));
+    for (int j = 0; j < CCD_SSIM_SCALES; j++) {  // scale j + 1 reads the level scale j wrote: stream order
+        a.scale = j;
+        k_frame_ssim<<<dim3((unsigned)max_tiles[j], (unsigned)n_jobs, 1), 32 * kSsimWarps, kSsimSmem, st>>>(d_jobs, a);
+        g_ccd_launches++;
+        if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
+    }
+    return 0;
 }
 
 int ccd_finish(const float *d_in, int h, int w, int bitdepth, int data_type, float *a, float *b, float *c,

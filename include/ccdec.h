@@ -250,6 +250,28 @@ typedef struct CcdDistJob {
 /* All jobs in ONE kernel launch; synchronous.  Returns CCD_OK or the first failing job's status. */
 int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cuda_stream);
 
+/* MS-SSIM of finished frames against their source (Wang, Simoncelli and Bovik 2003; DESIGN §4.6), from the same
+ * integers as ccd_frame_distortion: kd = rint(x * M) against ks, data range M, C1 = (0.01 M)^2, C2 = (0.03 M)^2.
+ * Inputs as for CcdDistJob.  Each plane at its own resolution: scale 0 is the plane, scale j + 1 the 2 x 2 average
+ * of scale j (floor sizes); an 11-tap Gaussian window (sigma 1.5), "valid" filtering.  Every plane needs both
+ * sides >= 176 (five scales of at least 11 samples), else CCD_ERR_ARG.
+ * d_map[c] (optional): float32 [h_c - 10][w_c - 10], the scale-0 SSIM map (l * cs) of plane c.
+ * Outputs: cs[c][j] = mean of cs, ssim[c][j] = mean of l * cs over plane c at scale j (f64 partials per tile added
+ * in tile order: the same on every run).  An off-grid decoded value is reported as by ccd_frame_distortion. */
+typedef struct CcdSsimJob {
+    const float *d_planes[3];
+    const void *d_src;
+    int32_t h, w, chroma_shift, bitdepth, src_layout;
+    float *d_map[3];
+    double cs[3][5];
+    double ssim[3][5];
+    int64_t bad_index;
+    int32_t status;
+} CcdSsimJob;
+
+/* All jobs in five kernel launches, one per scale; synchronous.  Returns CCD_OK or the first failing job's status. */
+int ccd_frame_ssim(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, void *cuda_stream);
+
 /* Statistics of a P/B frame's prediction (training/test.py:169-199), with the fp32 operations of the reconstruction
  * (bitdepth >= 1: the source scale): pred (beta * p0 + (1 - beta) * p1 for B), alpha, beta.  d_src (optional): source
  * samples as for ccd_frame_distortion (src_layout 1 not for yuv420); orig = ks / M, 4:2:0 chroma read at >> 1,

@@ -27,7 +27,7 @@ ERROR_NAMES = {
 EXPORTS = [
     "ccd_version", "ccd_sizeof_desc", "ccd_last_error", "ccd_create", "ccd_destroy", "ccd_nn_count",
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
-    "ccd_encode_latents", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
+    "ccd_encode_latents", "ccd_synthesize_many", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
     "ccd_latent_rate", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
     "ccd_debug_entropy_plan",
@@ -48,6 +48,21 @@ class CcdJob(ctypes.Structure):
         ("finish_type", ctypes.c_int32),
         ("d_out_u", ctypes.c_void_p),
         ("d_out_v", ctypes.c_void_p),
+    ]
+
+
+class CcdSynthJob(ctypes.Structure):
+    _fields_ = [
+        ("desc", ctypes.POINTER(CcdCoolChicDesc)),
+        ("nn_ints", ctypes.c_void_p),
+        ("d_latents", ctypes.c_void_p),
+        ("zero_grids", ctypes.c_uint32),
+        ("d_out", ctypes.c_void_p),
+        ("finish_bitdepth", ctypes.c_int32),
+        ("finish_type", ctypes.c_int32),
+        ("d_out_u", ctypes.c_void_p),
+        ("d_out_v", ctypes.c_void_p),
+        ("status", ctypes.c_int32),
     ]
 
 
@@ -178,6 +193,8 @@ def load_library():
         L.ccd_decode_latents.argtypes = [vp, pd, vp, ctypes.c_char_p, sz, vp, vp]
         L.ccd_encode_latents.restype = ci
         L.ccd_encode_latents.argtypes = [vp, pd, vp, ci, ctypes.c_uint64, vp, vp, i64, vp, vp, vp]
+        L.ccd_synthesize_many.restype = ci
+        L.ccd_synthesize_many.argtypes = [vp, ctypes.POINTER(CcdSynthJob), ci, vp]
         L.ccd_finish_frame.restype = ci
         L.ccd_finish_frame.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp]
         L.ccd_reconstruct_frame.restype = ci
@@ -292,27 +309,41 @@ class Context:
         y / u / v dictionary for yuv420)."""
         n = len(descs)
         jobs = (CcdJob * n)()
-        outs, lats = [], []
-        # all outputs are slices of ONE buffer, frame after frame, plane after plane: a batch of finished planar frames
-        # is then already in output order (pack_frames: one launch, one copy to the host for the whole batch)
-        sizes = []
+        lats = []
+        outs = self._job_outputs(jobs, descs, finish)
         for i in range(n):
             d = descs[i]
-            fin = finish[i] if finish is not None else None
-            if fin is not None and fin[1] == "yuv420":
-                sizes.append(d.img_h * d.img_w + 2 * (d.img_h // 2) * (d.img_w // 2))
-            else:
-                sizes.append(d.n_out_channels * d.img_h * d.img_w)
-        slab = torch.empty((sum(sizes),), dtype=torch.float32, device=self.torch_device)
-        off = 0
-        for i in range(n):
-            d = descs[i]
-            fin = finish[i] if finish is not None else None
             jobs[i].desc = ctypes.pointer(d)
             jobs[i].nn_bytes = nn_bytes[i]
             jobs[i].nn_nbytes = len(nn_bytes[i])
             jobs[i].latent_bytes = latent_bytes[i]
             jobs[i].latent_nbytes = len(latent_bytes[i])
+            if want_latents:
+                lat = torch.empty((d.n_symbols(),), dtype=torch.int8, device=self.torch_device)
+                lats.append(lat)
+                jobs[i].d_latents = lat.data_ptr()
+            else:
+                jobs[i].d_latents = None
+        rc = self._lib.ccd_decode_many(self._h, jobs, n, self._stream())
+        _check(rc)
+        return outs, (lats if want_latents else None)
+
+    def _job_outputs(self, jobs, descs, finish):
+        """The outputs of a job array whose jobs take CcdJob's output fields (d_out, d_out_u, d_out_v, finish_bitdepth,
+        finish_type): per job a raw [1, C, H, W] tensor, or with ``finish[i]`` the finished frame in FrameData layout.
+        All outputs are slices of ONE buffer, frame after frame, plane after plane: a batch of finished planar frames is
+        then already in output order (pack_frames: one launch, one copy to the host for the whole batch)."""
+        n = len(descs)
+        fins = [finish[i] if finish is not None else None for i in range(n)]
+        sizes = []
+        for d, fin in zip(descs, fins):
+            if fin is not None and fin[1] == "yuv420":
+                sizes.append(d.img_h * d.img_w + 2 * (d.img_h // 2) * (d.img_w // 2))
+            else:
+                sizes.append(d.n_out_channels * d.img_h * d.img_w)
+        slab = torch.empty((sum(sizes),), dtype=torch.float32, device=self.torch_device)
+        outs, off = [], 0
+        for i, (d, fin) in enumerate(zip(descs, fins)):
             if fin is not None and fin[1] == "yuv420":
                 h, w = d.img_h, d.img_w
                 ny, nc = h * w, (h // 2) * (w // 2)
@@ -330,15 +361,30 @@ class Context:
                 jobs[i].finish_bitdepth = int(fin[0])
                 jobs[i].finish_type = _frame_type_code(fin[1])
             outs.append(out)
-            if want_latents:
-                lat = torch.empty((d.n_symbols(),), dtype=torch.int8, device=self.torch_device)
-                lats.append(lat)
-                jobs[i].d_latents = lat.data_ptr()
-            else:
-                jobs[i].d_latents = None
-        rc = self._lib.ccd_decode_many(self._h, jobs, n, self._stream())
-        _check(rc)
-        return outs, (lats if want_latents else None)
+        return outs
+
+    def synthesize(self, descs: Sequence[CcdCoolChicDesc], nn_ints: Sequence[np.ndarray],
+                   latents: Sequence[torch.Tensor], zero_grids: Sequence[int], finish=None):
+        """The float tail of decode_many on given latents (``ccd_synthesize_many``): ``latents[i]`` is an int8 CUDA
+        tensor in decode order (what ``decode_many(want_latents=True)`` returns), read only; bit g of ``zero_grids[i]``
+        reads grid g (0 = finest, a synthesis grid) as all zeros.  Outputs as decode_many's, ``finish`` included."""
+        n = len(descs)
+        jobs = (CcdSynthJob * n)()
+        outs = self._job_outputs(jobs, descs, finish)
+        keep = []
+        for i in range(n):
+            d = descs[i]
+            nn = np.ascontiguousarray(nn_ints[i], dtype=np.int64)
+            lat = latents[i]
+            if not (lat.is_cuda and lat.dtype == torch.int8 and lat.is_contiguous() and lat.numel() == d.n_symbols()):
+                raise ValueError(f"latents[{i}] must be a contiguous int8 CUDA tensor of {d.n_symbols()} symbols")
+            keep += [nn, lat]
+            jobs[i].desc = ctypes.pointer(d)
+            jobs[i].nn_ints = nn.ctypes.data
+            jobs[i].d_latents = lat.data_ptr()
+            jobs[i].zero_grids = int(zero_grids[i])
+        _check(self._lib.ccd_synthesize_many(self._h, jobs, n, self._stream()))
+        return outs
 
     def decode_coolchic(self, desc, nn_bytes: bytes, latent_bytes: bytes, want_latents: bool = False):
         outs, lats = self.decode_many([desc], [nn_bytes], [latent_bytes], want_latents)

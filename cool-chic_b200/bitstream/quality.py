@@ -140,14 +140,9 @@ def _frame_layout(buf, max_decoding_order: int):
     return out
 
 
-@torch.no_grad()
-def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int = 0, max_decoding_order: int = -1,
-                  device: int = 0, want_maps: bool = False, ms_ssim: bool = False) -> Dict[str, FrameQuality]:
-    """Quality of every frame of an image / video bitstream against its source file (.yuv / .png / .ppm):
-    ``{str(display_idx): FrameQuality}`` in display order.  ``ms_ssim`` adds MS-SSIM for every frame whose planes
-    all have both sides >= 176 (``ms_ssim_planes`` stays None for the others), with the SSIM maps if ``want_maps``.  A source whose format, bitdepth or size differs from the
-    decoded frames, or that has too few frames, raises ValueError before anything runs on the device."""
-    frames = _frame_layout(memoryview(bytes(bitstream_bytes)), max_decoding_order)
+def _read_sources(frames, original_path: str, frame_offset: int):
+    """``{display_idx: (coding_idx, frame header, n_bytes, source samples)}`` for the frames of _frame_layout.  A source
+    whose format, bitdepth or size differs from the decoded frame, or that has too few frames, raises ValueError."""
     by_display = {}
     for coding_idx, (fh, disp, n_bytes, size) in enumerate(frames):
         fmt, b = fh.get_value("frame_data_type"), fh.get_value("bitdepth")
@@ -159,9 +154,12 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
             raise ValueError(f"source frame {frame_offset + disp} of {original_path} is {s.img_size[1]}x{s.img_size[0]} "
                              f"{s.frame_data_type} {s.bitdepth}-bit, decoded frame {disp} is {size[1]}x{size[0]} {fmt} {b}-bit")
         by_display[disp] = (coding_idx, fh, n_bytes, s)
+    return by_display
 
-    # every source frame in one pinned buffer, one host-to-device copy
-    ctx = _native.get_context(device)
+
+def _upload_sources(ctx, by_display):
+    """Every source frame of _read_sources in one pinned buffer, one host-to-device copy: ``{display_idx: samples}``
+    on the device (uint8, or int16 holding the uint16 samples)."""
     offs, total = {}, 0
     for disp, (_, _, _, s) in by_display.items():
         offs[disp] = total
@@ -175,6 +173,20 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
     for disp, (_, _, _, s) in by_display.items():
         raw = dev_all[offs[disp]:offs[disp] + s.samples.nbytes]
         sources[disp] = raw if s.samples.itemsize == 1 else raw.view(torch.int16)
+    return sources
+
+
+@torch.no_grad()
+def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int = 0, max_decoding_order: int = -1,
+                  device: int = 0, want_maps: bool = False, ms_ssim: bool = False) -> Dict[str, FrameQuality]:
+    """Quality of every frame of an image / video bitstream against its source file (.yuv / .png / .ppm):
+    ``{str(display_idx): FrameQuality}`` in display order.  ``ms_ssim`` adds MS-SSIM for every frame whose planes
+    all have both sides >= 176 (``ms_ssim_planes`` stays None for the others), with the SSIM maps if ``want_maps``.  A source whose format, bitdepth or size differs from the
+    decoded frames, or that has too few frames, raises ValueError before anything runs on the device."""
+    frames = _frame_layout(memoryview(bytes(bitstream_bytes)), max_decoding_order)
+    by_display = _read_sources(frames, original_path, frame_offset)
+    ctx = _native.get_context(device)
+    sources = _upload_sources(ctx, by_display)
 
     display_of = {coding_idx: disp for disp, (coding_idx, _, _, _) in by_display.items()}
     stats = {}

@@ -141,6 +141,12 @@ def _rates(headers: List[CoolChicHeader], nn_bytes: List[bytes], lat_bytes: List
     lat_bytes = [bytes(lb[:h.get_value("n_bytes_latent")]) for h, lb in zip(headers, lat_bytes)]
     _, lats = ctx.decode_many(descs, nn_bytes, lat_bytes, want_latents=True)
     nns = [_native.decode_nn(d, nb) for d, nb in zip(descs, nn_bytes)]
+    return _rates_of_latents(ctx, headers, descs, nns, lats)
+
+
+def _rates_of_latents(ctx, headers: List[CoolChicHeader], descs: List[CcdCoolChicDesc], nns: List[np.ndarray],
+                      lats: List[torch.Tensor]) -> List[CoolChicRate]:
+    """The rates of Cool-chics whose latents are already decoded: one ccd_latent_rate call."""
     res = ctx.latent_rate(descs, nns, lats, want_mu_sc=True, want_spatial=True)
     table = torch.from_numpy(scale_table()).to(ctx.torch_device)
     out = []

@@ -389,6 +389,7 @@ struct PreparedJob {
     int64_t lat_bytes = 0;  // bytes of the latent buffer in that layout
     int nl = 0, gl[CCD_MAX_GRIDS];  // latent grids (not hyper), finest first
     bool resized = false;   // the finest latent grid is smaller than the image: the output is computed at its size
+    const int8_t *lat[CCD_MAX_GRIDS];  // the device latents the float tail reads for each grid
     // float tail (plan_tail)
     bool tail = false;      // goes through the batched path
     int tail_cinp = 0, tail_C = 0;
@@ -408,6 +409,7 @@ struct CcdContext {
     uint32_t *d_cdf = nullptr;
     DeviceBuf upload;   // words / blobs / stream structs / statuses / synthesis weights
     DeviceBuf scratch;  // synthesis intermediates, latents when the caller does not want them, MS-SSIM pyramid levels
+    DeviceBuf zeros;    // all zero: the latents of the grids a synthesis job masks
     unsigned char *h_pin = nullptr;
     size_t h_pin_cap = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -491,6 +493,7 @@ int download(const Arena &A, size_t off, cudaStream_t st, const char *what) {
 // A job's status from its result words: a decode job's is word [0] of its entropy status words.  A job with a bad_index
 // gets the smallest bad index the kernel found, ~0 (bad_index -1) when there is none; any other one is CCD_ERR_ARG.
 int job_status(CcdJob &, const int32_t (&words)[16]) { return words[0]; }
+int job_status(CcdSynthJob &, const int32_t &word) { return word; }
 template <class Job> int job_status(Job &J, const unsigned long long &bad) {
     J.bad_index = (int64_t)bad;
     return bad == ~0ull ? CCD_OK : CCD_ERR_ARG;
@@ -569,8 +572,8 @@ int entropy_smem_ok(size_t smem) {
                 CCD_SMEM_MAX);
 }
 
-// Host preparation of one job: NN decode, ARM/IFCE packing, stream descriptor.
-int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
+// Host preparation of the float tail of one job: NN integers, latent layout, dequantised synthesis weights.
+int prepare_synthesis(PreparedJob &P, const int64_t *nn_ints_opt) {
     const CcdCoolChicDesc *d = P.d;
     int rc = nn_layout(d, &P.L);
     if (rc) return rc;
@@ -598,6 +601,39 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
         if (!d->grid_is_hyper[g]) P.gl[P.nl++] = g;
     P.resized = P.nl > 0 && (d->grid_h[P.gl[0]] != d->img_h || d->grid_w[P.gl[0]] != d->img_w);
     if (off >= ((int64_t)1 << 31)) return fail(CCD_ERR_UNSUPPORTED, "more than 2^31 latent symbols");
+    // ---- synthesis weights, dequantised (neuralnet.py:185-190: float32(int) * q_step)
+    const float qs_w = ldexpf(1.0f, d->qshift[6]), qs_b = ldexpf(1.0f, d->qshift[7]);
+    std::vector<float> &F = P.syn_f;
+    F.clear();
+    auto push = [&](int64_t off0, int64_t n, float qs) {
+        size_t at = F.size();
+        for (int64_t i = 0; i < n; i++) F.push_back((float)nn[off0 + i] * qs);
+        while (F.size() % 4) F.push_back(0.0f);
+        return at;
+    };
+    const int C = L.syn_c;
+    P.syn_off_ot_w = push(L.syn_ot_w, (int64_t)C * C, qs_w);
+    P.syn_off_ot_b = push(L.syn_ot_b, C, qs_b);
+    if (d->syn_stab) {
+        P.syn_off_st_w = push(L.syn_st_w, (int64_t)C * L.syn_stab_in, qs_w);
+        P.syn_off_st_b = push(L.syn_st_b, C, qs_b);
+    }
+    int in_ft = d->syn_in;
+    for (int l = 0; l < d->n_syn_layers; l++) {
+        P.syn_off_w[l] = push(L.syn_w[l], (int64_t)d->syn_out[l] * in_ft * d->syn_k[l] * d->syn_k[l], qs_w);
+        P.syn_off_b[l] = push(L.syn_b[l], d->syn_out[l], qs_b);
+        if (d->syn_res[l] && d->syn_out[l] != in_ft) return fail(CCD_ERR_ARG, "residual layer %d changes width", l);
+        in_ft = d->syn_out[l];
+    }
+    return CCD_OK;
+}
+
+// Host preparation of one job: prepare_synthesis, then the entropy stage's ARM / IFCE packing and stream descriptor.
+int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
+    if (int rc = prepare_synthesis(P, nn_ints_opt)) return rc;
+    const CcdCoolChicDesc *d = P.d;
+    const NNLayout &L = P.L;
+    const int64_t *nn = P.nn.data();
     // ---- ARM + IFCE integers
     const int dim = L.dim;
     std::vector<const int64_t *> qw, qb;
@@ -689,30 +725,6 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt) {
     S.ifce_blob_max = ifce_max;
     P.smem = plan_entropy_smem(S, n_max, rows_need);
 
-    // ---- synthesis weights, dequantised (neuralnet.py:185-190: float32(int) * q_step)
-    const float qs_w = ldexpf(1.0f, d->qshift[6]), qs_b = ldexpf(1.0f, d->qshift[7]);
-    std::vector<float> &F = P.syn_f;
-    F.clear();
-    auto push = [&](int64_t off0, int64_t n, float qs) {
-        size_t at = F.size();
-        for (int64_t i = 0; i < n; i++) F.push_back((float)nn[off0 + i] * qs);
-        while (F.size() % 4) F.push_back(0.0f);
-        return at;
-    };
-    const int C = L.syn_c;
-    P.syn_off_ot_w = push(L.syn_ot_w, (int64_t)C * C, qs_w);
-    P.syn_off_ot_b = push(L.syn_ot_b, C, qs_b);
-    if (d->syn_stab) {
-        P.syn_off_st_w = push(L.syn_st_w, (int64_t)C * L.syn_stab_in, qs_w);
-        P.syn_off_st_b = push(L.syn_st_b, C, qs_b);
-    }
-    int in_ft = d->syn_in;
-    for (int l = 0; l < d->n_syn_layers; l++) {
-        P.syn_off_w[l] = push(L.syn_w[l], (int64_t)d->syn_out[l] * in_ft * d->syn_k[l] * d->syn_k[l], qs_w);
-        P.syn_off_b[l] = push(L.syn_b[l], d->syn_out[l], qs_b);
-        if (d->syn_res[l] && d->syn_out[l] != in_ft) return fail(CCD_ERR_ARG, "residual layer %d changes width", l);
-        in_ft = d->syn_out[l];
-    }
     return CCD_OK;
 }
 
@@ -817,8 +829,8 @@ int resize_output(const CcdCoolChicDesc *d, const float *src, int C, int h0, int
 }
 
 // Upsampling cascade + synthesis + final resize for one job on the per-stream path (all kernels on `st`).
-int run_synthesis(const PreparedJob &P, const int8_t *d_lat, const float *d_synw, float *d_out, unsigned char *scratch,
-                  size_t scratch_bytes, cudaStream_t st) {
+int run_synthesis(const PreparedJob &P, const float *d_synw, float *d_out, unsigned char *scratch, size_t scratch_bytes,
+                  cudaStream_t st) {
     const CcdCoolChicDesc *d = P.d;
     const int cr = d->common_randomness != 0;
     const int nl = P.nl;
@@ -841,7 +853,7 @@ int run_synthesis(const PreparedJob &P, const int8_t *d_lat, const float *d_synw
     int gc = gl[nl - 1];
     int ch = d->grid_h[gc], cw = d->grid_w[gc], cc = 1;
     int rc;
-    if ((rc = ccd_ups_first(d_lat + P.lat_off_by_grid[gc], ch, cw, cur, st))) return fail(CCD_ERR_CUDA, "ups_first launch");
+    if ((rc = ccd_ups_first(P.lat[gc], ch, cw, cur, st))) return fail(CCD_ERR_CUDA, "ups_first launch");
     for (int idx = 0; idx < nl - 1; idx++) {
         const int gt = gl[nl - 2 - idx];
         const int th = d->grid_h[gt], tw = d->grid_w[gt];
@@ -849,10 +861,10 @@ int run_synthesis(const PreparedJob &P, const int8_t *d_lat, const float *d_synw
         float full_t[16], full_c[16];
         level_taps(P, idx, full_t, full_c);
         if (d->ups_k == 8 && d->ups_pre_k == 7) {
-            if ((rc = ccd_ups_level(d_lat + P.lat_off_by_grid[gt], th, tw, cur, cc, ch, cw, full_t, full_c, nxt, st)))
+            if ((rc = ccd_ups_level(P.lat[gt], th, tw, cur, cc, ch, cw, full_t, full_c, nxt, st)))
                 return fail(CCD_ERR_CUDA, "ups_level launch");
         } else {
-            if ((rc = ccd_ups_pre(d_lat + P.lat_off_by_grid[gt], th, tw, full_c, d->ups_pre_k, nxt, st)))
+            if ((rc = ccd_ups_pre(P.lat[gt], th, tw, full_c, d->ups_pre_k, nxt, st)))
                 return fail(CCD_ERR_CUDA, "ups_pre launch");
             if ((rc = ccd_ups_convt(cur, cc, ch, cw, full_t, d->ups_k, nxt + (size_t)th * tw, th, tw, st)))
                 return fail(CCD_ERR_CUDA, "ups_convt launch");
@@ -937,6 +949,17 @@ int run_synthesis(const PreparedJob &P, const int8_t *d_lat, const float *d_synw
 
 size_t synthesis_scratch_bytes(const CcdCoolChicDesc *d) { return syn_scratch_plan(d).total + 4096; }
 
+// The checks of a job's frame-tail request (job i of its call)
+int check_finish(const CcdJob &job, const PreparedJob &J, int i) {
+    if (job.finish_bitdepth == 0) return CCD_OK;
+    if (job.finish_bitdepth < 1 || job.finish_bitdepth > 16 || job.finish_type < 0 || job.finish_type > 3)
+        return fail(CCD_ERR_ARG, "job %d: bad frame tail request (bitdepth %d, type %d)", i, job.finish_bitdepth, job.finish_type);
+    if (J.L.syn_c != 3) return fail(CCD_ERR_ARG, "job %d: the frame tail needs a 3-channel output, found %d", i, J.L.syn_c);
+    if (job.finish_type == 1 && (!job.d_out_u || !job.d_out_v))
+        return fail(CCD_ERR_ARG, "job %d: yuv420 frame tail needs u and v outputs", i);
+    return CCD_OK;
+}
+
 // decode_frame's frame tail (decode.py:191-206) of a job that asks for it, from its raw output at the image size: the
 // finished frame goes to the job's outputs.  (k_tail_syn finishes the full-size outputs it writes itself.)
 int finish_job(const CcdJob &job, const float *raw, cudaStream_t st) {
@@ -1007,9 +1030,12 @@ struct TailPlan {
     size_t scratch_syn = 0, scratch_tail = 0;   // per-stream path (reused job after job), batched path
     size_t scratch_fin = 0;                     // raw output for finish_job (jobs finished one after the other)
     size_t off_syn = 0, off_lvl = 0;            // job arrays in the upload arena
+    unsigned char *d_scr_syn = nullptr, *d_scr_tail = nullptr;  // the scratch of both paths (reserve_tail_scratch)
+    float *d_fin = nullptr;
 };
 
-void plan_tail(std::vector<PreparedJob> &P, const CcdJob *jobs, TailPlan &T) {
+// Plans the float tail of the prepared jobs and lays out its job arrays in the call's arena A
+void plan_tail(std::vector<PreparedJob> &P, const CcdJob *jobs, TailPlan &T, Arena &A) {
     for (int i = 0; i < (int)P.size(); i++) {
         PreparedJob &J = P[(size_t)i];
         J.tail = tail_eligible(J);
@@ -1061,17 +1087,28 @@ void plan_tail(std::vector<PreparedJob> &P, const CcdJob *jobs, TailPlan &T) {
         G.max_w = std::max(G.max_w, d->grid_w[J.gl[0]]);
         G.max_h = std::max(G.max_h, d->grid_h[J.gl[0]]);
     }
+    T.off_syn = A.take(T.order.size() * ccd_tail_job_bytes());
+    T.off_lvl = A.take(T.lvl_jobs.size() * ccd_tail_level_job_bytes());
 }
 
-// Fills the batched path's job arrays at h (host side of the upload arena dv); d_scr_tail: its scratch.
-void fill_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJob *jobs, const std::vector<int8_t *> &d_lat,
-               unsigned char *h, const unsigned char *dv, unsigned char *d_scr_tail) {
+// Reserves the context's scratch: `before` bytes for the caller, then the float tail's (T.d_scr_syn, d_scr_tail, d_fin)
+int reserve_tail_scratch(CcdContext *ctx, size_t before, TailPlan &T) {
+    if (int rc = ensure_dev(ctx->scratch, before + al(T.scratch_syn) + T.scratch_tail + T.scratch_fin + 4096)) return rc;
+    T.d_scr_syn = ctx->scratch.p + before;
+    T.d_scr_tail = T.d_scr_syn + al(T.scratch_syn);
+    T.d_fin = reinterpret_cast<float *>(T.d_scr_tail + T.scratch_tail);
+    return CCD_OK;
+}
+
+// Fills the batched path's job arrays at h (host side of the upload arena dv); every grid is read at J.lat.
+void fill_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJob *jobs, unsigned char *h,
+               const unsigned char *dv) {
     const size_t lb = ccd_tail_level_job_bytes(), jb = ccd_tail_job_bytes();
+    unsigned char *d_scr_tail = T.d_scr_tail;
     for (size_t k = 0; k < T.lvl_jobs.size(); k++) {
         const int i = T.lvl_jobs[k].first, idx = T.lvl_jobs[k].second;
         const PreparedJob &J = P[(size_t)i];
         const CcdCoolChicDesc *d = J.d;
-        const int8_t *lat = d_lat[(size_t)i];
         const int gt = J.gl[J.nl - 2 - idx], gc = J.gl[J.nl - 1 - idx];
         // level idx writes P when (nl - 3 - idx) is even (the last one, idx = nl - 3, always writes P); level 0 reads
         // the coarsest int8 grid itself
@@ -1080,8 +1117,8 @@ void fill_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJo
         const float *in = reinterpret_cast<const float *>(d_scr_tail + (to_p ? J.off_tailQ : J.off_tailP));
         float full_t[16], full_c[16];
         level_taps(J, idx, full_t, full_c);
-        ccd_tail_fill_level(h + T.off_lvl + k * lb, lat + J.lat_off_by_grid[gt], idx == 0 ? nullptr : in,
-                            idx == 0 ? lat + J.lat_off_by_grid[gc] : nullptr, out, idx + 1, d->grid_h[gc], d->grid_w[gc],
+        ccd_tail_fill_level(h + T.off_lvl + k * lb, J.lat[gt], idx == 0 ? nullptr : in, idx == 0 ? J.lat[gc] : nullptr,
+                            out, idx + 1, d->grid_h[gc], d->grid_w[gc],
                             d->grid_h[gt], d->grid_w[gt], full_t, full_c);
     }
     for (size_t t = 0; t < T.order.size(); t++) {
@@ -1092,8 +1129,8 @@ void fill_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJo
         const SynNet N = syn_net(J, reinterpret_cast<const float *>(dv + J.off_syn));
         CcdTailSynDesc S;
         memset(&S, 0, sizeof(S));
-        S.lat = d_lat[(size_t)i] + J.lat_off_by_grid[g0];
-        if (nl == 2) S.stk8 = d_lat[(size_t)i] + J.lat_off_by_grid[g1];
+        S.lat = J.lat[g0];
+        if (nl == 2) S.stk8 = J.lat[g1];
         else S.stk = reinterpret_cast<const float *>(d_scr_tail + J.off_tailP);
         S.h = d->grid_h[g0]; S.w = d->grid_w[g0]; S.ch = d->grid_h[g1]; S.cw = d->grid_w[g1]; S.cin = nl;
         S.layers = N.layers; S.n_layers = d->n_syn_layers; S.stab = d->syn_stab ? &N.stab : nullptr;
@@ -1123,8 +1160,10 @@ void fill_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJo
 // the final resize of the outputs computed at a smaller size than the image (motion fields, reduced-resolution I
 // frames), followed by the frame tail of those that ask for it.
 int launch_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJob *jobs, const unsigned char *dv,
-                const unsigned char *d_scr_tail, float *d_fin, cudaStream_t st) {
+                cudaStream_t st) {
     const size_t lb = ccd_tail_level_job_bytes(), jb = ccd_tail_job_bytes();
+    const unsigned char *d_scr_tail = T.d_scr_tail;
+    float *d_fin = T.d_fin;
     for (const TailPlan::LevelLaunch &LL : T.levels)
         if (ccd_tail_launch_level(dv + T.off_lvl + LL.first * lb, LL.count, LL.planes, LL.max_tw, LL.max_th, st))
             return fail(CCD_ERR_CUDA, "cascade level launch failed");
@@ -1144,6 +1183,37 @@ int launch_tail(const TailPlan &T, const std::vector<PreparedJob> &P, const CcdJ
         if (rc) return rc;
     }
     return CCD_OK;
+}
+
+// The float tail of a call (DESIGN §4.2) once its job arrays are on the device at dv: the batched path's launches,
+// then every other job, one after the other, through the per-stream path.  A failing job gets its status.
+int run_tail(const TailPlan &T, const std::vector<PreparedJob> &P, CcdJob *jobs, const unsigned char *dv, cudaStream_t st) {
+    if (int rc = launch_tail(T, P, jobs, dv, st)) return rc;
+    for (int i = 0; i < (int)P.size(); i++) {
+        const PreparedJob &J = P[(size_t)i];
+        if (J.tail) continue;
+        float *out = jobs[i].finish_bitdepth != 0 ? T.d_fin : jobs[i].d_out;
+        int rc = run_synthesis(J, reinterpret_cast<const float *>(dv + J.off_syn), out, T.d_scr_syn, T.scratch_syn, st);
+        if (!rc) rc = finish_job(jobs[i], out, st);
+        if (rc) {
+            jobs[i].status = rc;
+            return rc;
+        }
+    }
+    return CCD_OK;
+}
+
+// A zeroed device region of at least `bytes` in the context.  A region whose clear could not be queued is given back,
+// so that no later call takes it for zeros.
+int ensure_zeros(CcdContext *ctx, size_t bytes, cudaStream_t st) {
+    if (bytes <= ctx->zeros.cap) return CCD_OK;
+    if (int rc = ensure_dev(ctx->zeros, bytes)) return rc;
+    const cudaError_t e = cudaMemsetAsync(ctx->zeros.p, 0, ctx->zeros.cap, st);
+    if (e == cudaSuccess) return CCD_OK;
+    cudaFree(ctx->zeros.p);
+    ctx->zeros.p = nullptr;
+    ctx->zeros.cap = 0;
+    return fail(CCD_ERR_CUDA, "clearing the zero region failed: %s", cudaGetErrorString(e));
 }
 
 }  // namespace
@@ -1206,6 +1276,7 @@ void ccd_destroy(CcdContext *c) {
     if (c->d_cdf) cudaFree(c->d_cdf);
     if (c->upload.p) cudaFree(c->upload.p);
     if (c->scratch.p) cudaFree(c->scratch.p);
+    if (c->zeros.p) cudaFree(c->zeros.p);
     if (c->h_pin) cudaFreeHost(c->h_pin);
     for (int i = 0; i < 4; i++)
         if (c->ev[i]) cudaEventDestroy(c->ev[i]);
@@ -1272,30 +1343,19 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         J.off_words = A.take(nwords * 4 + 16);
         J.off_blob = A.take(J.blob.size());
         J.off_syn = A.take(J.syn_f.size() * 4);
-        if (tail && jobs[i].finish_bitdepth != 0) {
-            if (jobs[i].finish_bitdepth < 1 || jobs[i].finish_bitdepth > 16 || jobs[i].finish_type < 0 || jobs[i].finish_type > 3)
-                return fail(CCD_ERR_ARG, "job %d: bad frame tail request (bitdepth %d, type %d)", i, jobs[i].finish_bitdepth, jobs[i].finish_type);
-            if (J.L.syn_c != 3) return fail(CCD_ERR_ARG, "job %d: the frame tail needs a 3-channel output, found %d", i, J.L.syn_c);
-            if (jobs[i].finish_type == 1 && (!jobs[i].d_out_u || !jobs[i].d_out_v))
-                return fail(CCD_ERR_ARG, "job %d: yuv420 frame tail needs u and v outputs", i);
-        }
+        if (tail && (rc = check_finish(jobs[i], J, i))) return rc;
         J.off_lat = scratch_lat;
         if (own_lat) scratch_lat += al((size_t)J.lat_bytes);
     }
+    // the float tail's device-resident job arrays (filled below, uploaded with everything else)
     TailPlan T;
-    if (tail) plan_tail(P, jobs, T);
-    // device-resident job arrays of the float tail (filled below, uploaded with everything else)
-    T.off_syn = A.take(T.order.size() * ccd_tail_job_bytes());
-    T.off_lvl = A.take(T.lvl_jobs.size() * ccd_tail_level_job_bytes());
+    if (tail) plan_tail(P, jobs, T, A);
     const size_t off_streams = A.take(sizeof(EntStream) * (size_t)n_jobs);
     const size_t off_status = A.take(sizeof(int32_t[16]) * (size_t)n_jobs);  // results: zeroed status words per job
     int rc;
     if ((rc = stage(ctx, A))) return rc;
     unsigned char *h = A.h, *dv = A.dv;
-    if ((rc = ensure_dev(ctx->scratch, scratch_lat + al(T.scratch_syn) + T.scratch_tail + T.scratch_fin + 4096))) return rc;
-    unsigned char *d_scr_syn = ctx->scratch.p + scratch_lat;
-    unsigned char *d_scr_tail = d_scr_syn + al(T.scratch_syn);
-    float *d_fin = reinterpret_cast<float *>(d_scr_tail + T.scratch_tail);
+    if ((rc = reserve_tail_scratch(ctx, scratch_lat, T))) return rc;
 
     // group jobs by kernel configuration so that each group is one launch
     std::vector<int> order((size_t)n_jobs);
@@ -1306,7 +1366,6 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
     };
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return key(a) < key(b); });
 
-    std::vector<int8_t *> d_lat((size_t)n_jobs);
     for (int i = 0; i < n_jobs; i++) {
         PreparedJob &J = P[(size_t)i];
         const size_t nbytes4 = mode == 0 ? jobs[i].latent_nbytes / 4 * 4 : 0;
@@ -1316,7 +1375,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         if (!J.syn_f.empty()) memcpy(h + J.off_syn, J.syn_f.data(), J.syn_f.size() * 4);
         int8_t *lat = jobs[i].d_latents;
         if (!lat) lat = reinterpret_cast<int8_t *>(ctx->scratch.p + J.off_lat);
-        d_lat[(size_t)i] = lat;
+        for (int g = 0; g < J.d->n_grids; g++) J.lat[g] = lat + J.lat_off_by_grid[g];
         EntStream &S = J.es;
         S.mode = mode;
         S.prod_mask = ctx->prod_mask;
@@ -1333,7 +1392,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         memcpy(h + off_streams + sizeof(EntStream) * (size_t)t, &P[(size_t)order[(size_t)t]].es, sizeof(EntStream));
     memset(h + off_status, 0, A.end - off_status);
 
-    if (tail) fill_tail(T, P, jobs, d_lat, h, dv, d_scr_tail);
+    if (tail) fill_tail(T, P, jobs, h, dv);
     CUDA_TRY(cudaMemcpyAsync(dv, h, A.end, cudaMemcpyHostToDevice, st));
     ctx->last_upload_bytes = A.end;
     CUDA_TRY(cudaEventRecord(ctx->ev[1], st));
@@ -1375,22 +1434,7 @@ static int decode_impl_body(CcdContext *ctx, CcdJob *jobs, int n_jobs, const int
         g++;
     }
     CUDA_TRY(cudaEventRecord(ctx->ev[2], st));
-    if (tail) {
-        if ((rc = launch_tail(T, P, jobs, dv, d_scr_tail, d_fin, st))) return rc;
-        // everything else: one job after the other through the per-stream path
-        for (int i = 0; i < n_jobs; i++) {
-            const PreparedJob &J = P[(size_t)i];
-            if (J.tail) continue;
-            float *out = jobs[i].finish_bitdepth != 0 ? d_fin : jobs[i].d_out;
-            rc = run_synthesis(J, d_lat[(size_t)i], reinterpret_cast<const float *>(dv + J.off_syn), out, d_scr_syn,
-                               T.scratch_syn, st);
-            if (!rc) rc = finish_job(jobs[i], out, st);
-            if (rc) {
-                jobs[i].status = rc;
-                return rc;
-            }
-        }
-    }
+    if (tail && (rc = run_tail(T, P, jobs, dv, st))) return rc;
     CUDA_TRY(cudaEventRecord(ctx->ev[3], st));
     if ((rc = download(A, off_status, st, "kernel"))) return rc;
     cudaEventElapsedTime(&ctx->last_ms[2], ctx->ev[0], ctx->ev[1]);
@@ -1445,6 +1489,67 @@ int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
     if (slow_out) *slow_out = stt[0][2];
     if (stt[0][3] > out_cap_words) return fail(CCD_ERR_ARG, "output buffer too small (%d words needed)", stt[0][3]);
     return CCD_OK;
+}
+
+// The float tail of every job on the caller's latents: decode's plan, arrays and launches, no entropy stage.  A grid
+// the job masks is read from the context's zeroed region instead of its latents.
+static int synthesize_body(CcdContext *ctx, CcdSynthJob *jobs, int n_jobs, cudaStream_t st) {
+    std::vector<PreparedJob> P((size_t)n_jobs);
+    std::vector<CcdJob> tj((size_t)n_jobs);  // each job's outputs and frame-tail request, as the float tail takes them
+    Arena A;
+    size_t max_grid = 16;
+    for (int i = 0; i < n_jobs; i++) {
+        CcdSynthJob &S = jobs[i];
+        if (!S.desc || !S.nn_ints) return S.status = fail(CCD_ERR_ARG, "job %d: null descriptor or network integers", i);
+        if (!S.d_latents || !S.d_out) return S.status = fail(CCD_ERR_ARG, "job %d: null latents or output pointer", i);
+        tj[(size_t)i] = CcdJob{S.desc, nullptr, 0, nullptr, 0, S.d_out, nullptr, CCD_OK, S.finish_bitdepth, S.finish_type,
+                               S.d_out_u, S.d_out_v};
+        PreparedJob &J = P[(size_t)i];
+        J.job = &tj[(size_t)i];
+        J.d = S.desc;
+        if (int rc = prepare_synthesis(J, S.nn_ints)) return S.status = rc;
+        const CcdCoolChicDesc *d = J.d;
+        for (int g = 0; g < 32; g++) {
+            if (!((S.zero_grids >> g) & 1u)) continue;
+            if (g >= d->n_grids)
+                return S.status = fail(CCD_ERR_ARG, "job %d: zero_grids bit %d, the stream has %d grids", i, g, d->n_grids);
+            if (d->grid_is_hyper[g])
+                return S.status = fail(CCD_ERR_ARG, "job %d: zero_grids bit %d is a hyperlatent grid, which no synthesis reads", i, g);
+        }
+        if (int rc = check_finish(tj[(size_t)i], J, i)) return S.status = rc;
+        J.off_syn = A.take(J.syn_f.size() * 4);
+        for (int g = 0; g < d->n_grids; g++) max_grid = std::max(max_grid, (size_t)d->grid_h[g] * d->grid_w[g]);
+    }
+    TailPlan T;
+    plan_tail(P, tj.data(), T, A);
+    // results: one status word per job, zero on the way up.  No float-tail kernel reports a per-job fault, so the download
+    // is the call's synchronisation and the report every job call makes.
+    const size_t off_status = A.take(sizeof(int32_t) * (size_t)n_jobs);
+    if (int rc = stage(ctx, A)) return rc;
+    if (int rc = reserve_tail_scratch(ctx, 0, T)) return rc;
+    if (int rc = ensure_zeros(ctx, max_grid, st)) return rc;
+    for (int i = 0; i < n_jobs; i++) {
+        PreparedJob &J = P[(size_t)i];
+        if (!J.syn_f.empty()) memcpy(A.h + J.off_syn, J.syn_f.data(), J.syn_f.size() * 4);
+        for (int g = 0; g < J.d->n_grids; g++)
+            J.lat[g] = ((jobs[i].zero_grids >> g) & 1u) ? reinterpret_cast<const int8_t *>(ctx->zeros.p)
+                                                        : jobs[i].d_latents + J.lat_off_by_grid[g];
+    }
+    memset(A.h + off_status, 0, A.end - off_status);
+    fill_tail(T, P, tj.data(), A.h, A.dv);
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, A.end, cudaMemcpyHostToDevice, st));
+    if (int rc = run_tail(T, P, tj.data(), A.dv, st)) {
+        for (int i = 0; i < n_jobs; i++)
+            if (tj[(size_t)i].status != CCD_OK) jobs[i].status = tj[(size_t)i].status;
+        return rc;
+    }
+    if (int rc = download(A, off_status, st, "synthesis")) return rc;
+    return report(jobs, n_jobs, reinterpret_cast<const int32_t *>(A.h + off_status),
+                  [&](int i) { return fail(jobs[i].status, "job %d: synthesis failed", i); });
+}
+
+int ccd_synthesize_many(CcdContext *ctx, CcdSynthJob *jobs, int n_jobs, void *cuda_stream) {
+    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return synthesize_body(ctx, jobs, n_jobs, st); });
 }
 
 static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaStream_t st) {

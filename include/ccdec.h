@@ -152,6 +152,28 @@ int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
                        uint64_t seed, int8_t *d_latents, uint32_t *d_out_words, int64_t out_cap_words,
                        int64_t *n_words_out, int32_t *slow_path_count_out, void *cuda_stream);
 
+/* The float tail of ccd_decode_many (upsampling cascade, synthesis, final resize and the optional frame tail) on
+ * latents the caller supplies: d_out (and d_out_u, d_out_v with finish_bitdepth / finish_type, as in CcdJob) receives
+ * exactly what ccd_decode_many writes for a stream whose decoded latents are d_latents, except that every grid g with
+ * bit g of zero_grids set (g = 0: the finest) is read as all zeros.  nn_ints: the host NN integers (ccd_decode_nn).
+ * d_latents: int8 in decode order, as CcdJob.d_latents receives them; read only.  A mask bit at or above n_grids, or
+ * on a hyperlatent grid (those only feed the entropy model), makes the job CCD_ERR_ARG. */
+typedef struct CcdSynthJob {
+    const CcdCoolChicDesc *desc;
+    const int64_t *nn_ints;
+    const int8_t *d_latents;
+    uint32_t zero_grids;
+    float *d_out;
+    int32_t finish_bitdepth, finish_type;
+    float *d_out_u, *d_out_v;
+    int32_t status;
+} CcdSynthJob;
+
+/* All jobs share the batched launches, one per cascade level and one per synthesis group, as in a decode; jobs outside
+ * the batched path make their own launches.  No entropy launch.  One host->device and one device->host copy;
+ * synchronous.  Returns CCD_OK or the first failing job's status. */
+int ccd_synthesize_many(CcdContext *ctx, CcdSynthJob *jobs, int n_jobs, void *cuda_stream);
+
 /* Rate analysis of decoded latents: the information content of every latent symbol under the model the
  * range coder used -- the ARM + IFCE evaluated exactly as decoding does, (mu_idx, sc_idx) clamped like
  * latent.py:165 / rangecoder.py:89-91, freq = left(s+1) - left(s) of constriction's leaky quantised Laplace

@@ -30,7 +30,7 @@ EXPORTS = [
     "ccd_encode_latents", "ccd_synthesize_many", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
     "ccd_latent_rate", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
-    "ccd_debug_entropy_plan",
+    "ccd_debug_entropy_plan", "ccd_debug_cdf_table",
 ]
 
 
@@ -226,6 +226,8 @@ def load_library():
         L.ccd_inter_stats.argtypes = [vp, ctypes.POINTER(CcdInterFrame), ctypes.POINTER(CcdInterStats), vp]
         L.ccd_debug_laplace_domain.restype = ci
         L.ccd_debug_laplace_domain.argtypes = [vp, ci, ci, vp, vp]
+        L.ccd_debug_cdf_table.restype = ci
+        L.ccd_debug_cdf_table.argtypes = [vp, ci, ci, vp]
         L.ccd_debug_last_status.restype = ci
         L.ccd_debug_last_status.argtypes = [vp, vp]
         L.ccd_debug_launch_count.restype = ctypes.c_uint64
@@ -453,7 +455,9 @@ class Context:
         else:
             lat = latents.to(self.torch_device, torch.int8).contiguous().clone()
             mode, seed = 1, 0
-        cap = n // 2 + 1024
+        # a symbol costs at most 24 - log2(1 - 2^-8) < 24.0057 bits (freq >= 1 of 2^24, scale truncation at R >= 2^32);
+        # 3 words for the initial state, the seal and rounding
+        cap = -(-n * 240057 // 320000) + 3
         words = torch.zeros((cap,), dtype=torch.int32, device=self.torch_device)
         n_words = ctypes.c_int64(0)
         slow = ctypes.c_int32(0)
@@ -733,6 +737,10 @@ class Context:
     def launch_count(self) -> int:
         return int(self._lib.ccd_debug_launch_count())
 
+    def set_producer_mask(self, mask: int) -> None:
+        """Which of warps 0..13 of an entropy CTA produce windows (ccd_debug_set_producer_mask; default 0x3777)."""
+        _check(self._lib.ccd_debug_set_producer_mask(self._h, mask))
+
     def last_status(self):
         st = (ctypes.c_int32 * 16)()
         _check(self._lib.ccd_debug_last_status(self._h, st))
@@ -745,6 +753,12 @@ class Context:
         _check(self._lib.ccd_debug_laplace_domain(self._h, sc_lo, sc_hi, lo.ctypes.data_as(ctypes.c_void_p),
                                                   hi.ctypes.data_as(ctypes.c_void_p)))
         return lo, hi
+
+    def cdf_table(self, sc_lo: int, sc_hi: int) -> np.ndarray:
+        """The context's cumulative table for the scales [sc_lo, sc_hi): uint32 [sc_hi - sc_lo, 256, 32]."""
+        out = np.zeros((sc_hi - sc_lo, 256, 32), dtype=np.uint32)
+        _check(self._lib.ccd_debug_cdf_table(self._h, sc_lo, sc_hi, out.ctypes.data_as(ctypes.c_void_p)))
+        return out
 
 
 def _planes(data, frame_data_type: str):

@@ -1542,6 +1542,22 @@ int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
                        int8_t *d_latents, uint32_t *d_out_words, int64_t out_cap_words, int64_t *n_words_out,
                        int32_t *slow_out, void *cuda_stream) {
     if (!d_latents || !nn_ints || !d_out_words || (mode != 1 && mode != 2)) return fail(CCD_ERR_ARG, "bad argument");
+    if (mode == 1) {
+        // the model has no interval outside [-64, 63] (left(s) = left(s + 1) there: the range would drop to 0 and the
+        // payload decode to something else), so such a latent is refused before the coder sees it
+        const int rc = guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+            const int64_t n = ccd_latent_count(desc, nullptr);
+            if (n < 0) return (int)n;
+            std::vector<int8_t> h((size_t)n);
+            CUDA_TRY(cudaMemcpyAsync(h.data(), d_latents, (size_t)n, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
+            for (int64_t i = 0; i < n; i++)
+                if (h[(size_t)i] < -64 || h[(size_t)i] > 63)
+                    return fail(CCD_ERR_ARG, "latent %lld is outside [-64, 63]", (long long)i);
+            return CCD_OK;
+        });
+        if (rc) return rc;
+    }
     CcdJob j{desc, nullptr, 0, nullptr, 0, nullptr, d_latents, 0, 0, 0, nullptr, nullptr};
     const int64_t *nn[1] = {nn_ints};
     uint32_t *ow[1] = {d_out_words};
@@ -2006,6 +2022,16 @@ int ccd_debug_laplace_domain(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *ou
         if (ccd_laplace_domain(ctx->d_scale, sc_lo, sc_hi, lo, hi, st)) return fail(CCD_ERR_CUDA, "launch failed");
         CUDA_TRY(cudaMemcpy(out_lo, lo, n * 4, cudaMemcpyDeviceToHost));
         CUDA_TRY(cudaMemcpy(out_hi, hi, n * 4, cudaMemcpyDeviceToHost));
+        return CCD_OK;
+    });
+}
+
+int ccd_debug_cdf_table(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *out) {
+    return guarded(ctx, nullptr, [&](cudaStream_t) -> int {
+        if (sc_lo < 0 || sc_hi > CCD_N_SCALE || sc_lo >= sc_hi || !out) return fail(CCD_ERR_ARG, "bad argument");
+        const size_t row = (size_t)256 * CCD_WIN;
+        CUDA_TRY(cudaMemcpy(out, ctx->d_cdf + (size_t)sc_lo * row, (size_t)(sc_hi - sc_lo) * row * 4,
+                            cudaMemcpyDeviceToHost));
         return CCD_OK;
     });
 }

@@ -238,13 +238,16 @@ class SeedStream:
 
 
 def make_coolchic(ctx, seed_stream: SeedStream, img_size, latent_resolution=(0, 6), hyperlatent_resolution=None,
-                  seed: int = 0, final_upsampling_type=None, overrides=None, latents: Optional[torch.Tensor] = None
-                  ) -> Tuple[bytes, CoolChicHeader, torch.Tensor]:
-    """One Cool-chic section (header + NN payload + latent payload) for an image of ``img_size``."""
+                  seed: int = 0, final_upsampling_type=None, overrides=None, latents: Optional[torch.Tensor] = None,
+                  nn: Optional[np.ndarray] = None) -> Tuple[bytes, CoolChicHeader, torch.Tensor]:
+    """One Cool-chic section (header + NN payload + latent payload) for an image of ``img_size``.  ``nn``: the
+    network integers to write (in bitstream order, for the header's architecture) instead of the sample's."""
     header = make_coolchic_header(seed_stream.header, img_size, latent_resolution, hyperlatent_resolution,
                                   final_upsampling_type, overrides)
     desc = desc_from_header(header)
-    nn = adapt_nn(seed_stream.desc, seed_stream.nn, desc)
+    if nn is None:
+        nn = adapt_nn(seed_stream.desc, seed_stream.nn, desc)
+    nn = np.asarray(nn, dtype=np.int64)
     _, counts = join_nn(desc, split_nn(desc, nn))
     nn_bytes, pad = encode_exp_golomb(nn.tolist(), counts)
     header.set_value("nn_n_bytes", len(nn_bytes))

@@ -165,7 +165,10 @@ int ccd_decode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64
  * d_latents (decode order);  mode 2: DRAW the latents from the stream's own ARM (seeded
  * splitmix64, one 24-bit quantile per symbol), store them in d_latents and encode them --
  * used to fabricate self-consistent synthetic streams (SURVEY 8d).  Output: little-endian
- * u32 words in d_out_words (device), count in *n_words_out. */
+ * u32 words in d_out_words (device), count in *n_words_out.  A symbol costs at most
+ * 24 - log2(1 - 2^-8) < 24.0057 bits, so out_cap_words = ceil(n * 24.0057 / 32) + 3 always
+ * suffices.  Mode 1 refuses a latent outside [-64, 63] with CCD_ERR_ARG, the message naming
+ * the smallest such decode-order index. */
 int ccd_encode_latents(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints, int mode,
                        uint64_t seed, int8_t *d_latents, uint32_t *d_out_words, int64_t out_cap_words,
                        int64_t *n_words_out, int32_t *slow_path_count_out, void *cuda_stream);
@@ -333,6 +336,12 @@ int ccd_inter_stats(CcdContext *ctx, const CcdInterFrame *frame, CcdInterStats *
  * out_hi[...]                = trunc(FW * (1 - 0.5*exp(-|d|/b))). */
 int ccd_debug_laplace_domain(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *out_lo,
                              uint32_t *out_hi);
+
+/* The context's cumulative table, as the entropy decoder and the rate pass read it: for sc in
+ * [sc_lo, sc_hi), f < 256, t < 32, writes to the host array
+ * out[((sc-sc_lo)*256+f)*32+t] = trunc(FW * cdf(n/256)), n = 256 t - f - 3584 (window entry t of a
+ * symbol whose mu_idx has (mu_idx + 128) & 255 = f). */
+int ccd_debug_cdf_table(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *out);
 
 /* Number of CUDA kernels this library has launched since it was loaded. */
 uint64_t ccd_debug_launch_count(void);

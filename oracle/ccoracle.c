@@ -774,6 +774,9 @@ static int64_t finish_encode(RcEnc *en, uint8_t *out, size_t cap) {
 int64_t cco_encode_latents(const CcoDesc *d, const int64_t *nn, const int8_t *latents, uint8_t *out,
                            size_t cap) {
     int64_t n = cco_latent_layout(d, NULL);
+    /* the model has no interval outside [-64, 63]: left(s) = left(s + 1) there, so R would drop to 0 */
+    for (int64_t i = 0; i < n; i++)
+        if (latents[i] < SYM_MIN || latents[i] > SYM_MAX) return CCO_ERR_ARG;
     int8_t *tmp = (int8_t *)malloc((size_t)n + 1);
     if (!tmp) return CCO_ERR_NOMEM;
     memcpy(tmp, latents, (size_t)n);

@@ -90,7 +90,8 @@ int cco_decode_latents(const CcoDesc *d, const int64_t *nn, const uint8_t *laten
                        size_t nbytes, int8_t *latents_out, int64_t *stats);
 
 /* Range ENcode given latents (the mode=="encode" branch of the same functions,
- * rangecoder.py:46-78).  Returns nbytes written or <0. */
+ * rangecoder.py:46-78).  Returns nbytes written or <0; CCO_ERR_ARG for a latent outside
+ * [-64, 63].  A symbol costs at most 24.0057 bits: cap >= 4 * (ceil(n * 24.0057 / 32) + 3). */
 int64_t cco_encode_latents(const CcoDesc *d, const int64_t *nn, const int8_t *latents,
                            uint8_t *out, size_t cap);
 

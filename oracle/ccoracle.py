@@ -121,12 +121,22 @@ def decode_latents(desc, nn: np.ndarray, latent_bytes: bytes):
     return out, stats
 
 
+def payload_cap_bytes(n_symbols: int) -> int:
+    """Largest payload of n symbols: freq >= 1 of 2^24 and the scale truncation (R >= 2^32) cost at most
+    24 - log2(1 - 2^-8) < 24.0057 bits per symbol; 3 words for the initial state, the seal and rounding."""
+    return 4 * (-(-n_symbols * 240057 // 320000) + 3)
+
+
 def encode_latents(desc, nn: np.ndarray, latents: np.ndarray) -> bytes:
     latents = np.ascontiguousarray(latents, dtype=np.int8)
     nn = np.ascontiguousarray(nn, dtype=np.int64)
-    out = np.zeros(latents.size * 2 + 64, dtype=np.uint8)
-    n = _chk(lib().cco_encode_latents(ctypes.byref(desc), _p(nn), _p(latents), _p(out), out.size),
-             "encode_latents")
+    out = np.zeros(payload_cap_bytes(latents.size), dtype=np.uint8)
+    rc = lib().cco_encode_latents(ctypes.byref(desc), _p(nn), _p(latents), _p(out), out.size)
+    if rc == -1:
+        bad = np.flatnonzero((latents < -64) | (latents > 63))
+        if bad.size:
+            raise OracleError(f"oracle encode_latents: latent {int(bad[0])} is outside [-64, 63] (code -1)")
+    n = _chk(rc, "encode_latents")
     return out[:n].tobytes()
 
 
@@ -134,7 +144,7 @@ def sample_latents(desc, nn: np.ndarray, seed: int):
     total, _ = latent_layout(desc)
     lat = np.zeros(total, dtype=np.int8)
     nn = np.ascontiguousarray(nn, dtype=np.int64)
-    out = np.zeros(total * 2 + 64, dtype=np.uint8)
+    out = np.zeros(payload_cap_bytes(total), dtype=np.uint8)
     n = _chk(lib().cco_sample_latents(ctypes.byref(desc), _p(nn), ctypes.c_uint64(seed), _p(lat), _p(out),
                                       out.size), "sample_latents")
     return lat, out[:n].tobytes()

@@ -2,7 +2,7 @@
 prediction statistics of P / B frames, with the reference encoder's column names.
 
     python cc_eval.py -i <bitstream.cool> --original <src.yuv|png|ppm> [--frame_offset N] [--ms_ssim] [--maps out.npz]
-                      [--grids] [--device N]
+                      [--grids] [--motion] [--device N]
 
 Display frame i is compared with source frame frame_offset + i.  ``--maps`` writes, per frame, the error map
 (sum over planes of the squared integer errors / (2^b - 1)^2, chroma at (y >> 1, x >> 1) for 4:2:0) and for P / B
@@ -12,6 +12,11 @@ every plane.  ``--grids`` appends, per frame and per Cool-chic, a table of its l
 the frame PSNR with the grid alone read as zeros and its change from the decoded frame's, and for the residue the PSNR
 with only the synthesis grids from the coarsest down to that one kept (DESIGN §4.7).  The grid analysis decodes the
 bitstream a second time, after the quality table.
+``--motion`` appends, for every P / B frame, a table of its variants (DESIGN §4.9): the frame with every motion
+channel zeroed (no_local_motion), with the global flow zeroed too (no_motion), predicted from one reference only (B:
+ref0_only, ref1_only), without the residue (no_residue) and without the prediction (no_prediction), each with its PSNR,
+per plane, and its change from the decoded frame's; then one line of flow statistics per reference.  With ``--maps``
+it also writes the total displacement of every reference, ``frame<k>_flow<r>`` ([2, H, W]).
 """
 import argparse
 
@@ -19,11 +24,13 @@ import numpy as np
 
 import coolchic_b200  # noqa: F401  (import alias of the cool-chic_b200/ package)
 from coolchic_b200.bitstream.grids import video_grid_analysis
+from coolchic_b200.bitstream.motion import variants_of
 from coolchic_b200.bitstream.quality import video_quality
 
 COLUMNS = ["frame_idx", "frame_type", "psnr_db", "psnr_y_db", "psnr_u_db", "psnr_v_db", "rate_bpp", "alpha_mean",
            "beta_mean", "pred_psnr_db", "dummy_pred_psnr_db"]
 MS_SSIM_COLUMNS = ["ms_ssim", "ms_ssim_db", "ms_ssim_y", "ms_ssim_u", "ms_ssim_v"]
+MOTION_COLUMNS = ["variant", "psnr_db", "psnr_y_db", "psnr_u_db", "psnr_v_db", "delta_db"]
 GRID_COLUMNS = ["grid", "size", "hyper", "bits", "bpp", "drop_psnr_db", "drop_delta_db", "coarse_psnr_db"]
 
 
@@ -39,12 +46,14 @@ if __name__ == "__main__":
     parser.add_argument("--maps", type=str, default=None, help="Write the error / alpha / beta / prediction maps here (.npz).")
     parser.add_argument("--ms_ssim", action="store_true", help="Also report MS-SSIM.")
     parser.add_argument("--grids", action="store_true", help="Also report what each latent grid costs and buys.")
+    parser.add_argument("--motion", action="store_true", help="Also report what the motion, each reference and the "
+                        "residue of every P / B frame buy.")
     parser.add_argument("--device", type=int, help="CUDA device ordinal.", default=0)
     args = parser.parse_args()
 
     with open(args.input, "rb") as f_in:
         frames = video_quality(f_in.read(), args.original, frame_offset=args.frame_offset, device=args.device,
-                               want_maps=args.maps is not None, ms_ssim=args.ms_ssim)
+                               want_maps=args.maps is not None, ms_ssim=args.ms_ssim, motion=args.motion)
     columns = COLUMNS + (MS_SSIM_COLUMNS if args.ms_ssim else [])
     print(" ".join(f"{c:<18}" for c in columns))
     for key, q in frames.items():
@@ -67,7 +76,23 @@ if __name__ == "__main__":
                     maps[f"frame{key}_{name}"] = t.cpu().numpy()
             for plane, t in zip("yuv", q.ssim_maps or []):
                 maps[f"frame{key}_ssim_{plane}"] = t.cpu().numpy()
+            for r, ref in enumerate(q.motion.refs if q.motion is not None else []):
+                maps[f"frame{key}_flow{r}"] = ref.flow_map.cpu().numpy()
         np.savez_compressed(args.maps, **maps)
+    if args.motion:
+        for key, q in frames.items():
+            m = q.motion
+            if m is None:
+                continue
+            print(f"motion frame {key} {q.frame_type} psnr_db {q.psnr_db:.6f}")
+            print(" ".join(f"{c:<18}" for c in MOTION_COLUMNS))
+            for v in variants_of(q.frame_type):
+                vals = [v] + [_fmt(x) for x in [m.psnr_db(v)] + m.plane_psnr_db(v) + [m.delta_db(v)]]
+                print(" ".join(f"{x:<18}" for x in vals))
+            for r, ref in enumerate(m.refs):
+                print(f"ref{r} global_flow {ref.global_flow[0]} {ref.global_flow[1]}  mean_flow {ref.mean_flow[0]:.6f} "
+                      f"{ref.mean_flow[1]:.6f}  mean_local {ref.mean_local:.6f}  max_local {ref.max_local:.6f}  "
+                      f"outside {ref.outside} ({100 * ref.outside_fraction:.2f} %)")
     if args.grids:
         with open(args.input, "rb") as f_in:
             grids = video_grid_analysis(f_in.read(), args.original, frame_offset=args.frame_offset, device=args.device)

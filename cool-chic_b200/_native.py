@@ -28,7 +28,7 @@ EXPORTS = [
     "ccd_version", "ccd_sizeof_desc", "ccd_last_error", "ccd_create", "ccd_destroy", "ccd_nn_count",
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
     "ccd_encode_latents", "ccd_synthesize_many", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
-    "ccd_latent_rate", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats",
+    "ccd_latent_rate", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats", "ccd_inter_analysis",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
     "ccd_debug_entropy_plan", "ccd_debug_cdf_table",
 ]
@@ -157,6 +157,23 @@ class CcdInterStats(ctypes.Structure):
     ]
 
 
+INTER_VARIANTS = 7  # CCD_INTER_VARIANTS
+
+
+class CcdInterAnalysis(ctypes.Structure):
+    _fields_ = [
+        ("d_src", ctypes.c_void_p),
+        ("src_layout", ctypes.c_int32),
+        ("d_flow", ctypes.c_void_p * 2),
+        ("sse", (ctypes.c_uint64 * 3) * INTER_VARIANTS),
+        ("flow_sum", (ctypes.c_double * 3) * 2),
+        ("flow_max", ctypes.c_double * 2),
+        ("outside", ctypes.c_uint64 * 2),
+        ("bad_index", ctypes.c_int64),
+        ("status", ctypes.c_int32),
+    ]
+
+
 SOURCE_LAYOUTS = {"planar": 0, "hwc": 1}
 
 
@@ -224,6 +241,8 @@ def load_library():
         L.ccd_frame_ssim.argtypes = [vp, ctypes.POINTER(CcdSsimJob), ci, vp]
         L.ccd_inter_stats.restype = ci
         L.ccd_inter_stats.argtypes = [vp, ctypes.POINTER(CcdInterFrame), ctypes.POINTER(CcdInterStats), vp]
+        L.ccd_inter_analysis.restype = ci
+        L.ccd_inter_analysis.argtypes = [vp, ctypes.POINTER(CcdInterFrame), ctypes.POINTER(CcdInterAnalysis), vp]
         L.ccd_debug_laplace_domain.restype = ci
         L.ccd_debug_laplace_domain.argtypes = [vp, ci, ci, vp, vp]
         L.ccd_debug_cdf_table.restype = ci
@@ -727,6 +746,37 @@ class Context:
         _check(self._lib.ccd_inter_stats(self._h, ctypes.byref(f), ctypes.byref(st), self._stream()))
         del keep
         out["sums"] = [float(s) for s in st.sums]
+        return out
+
+    def inter_analysis(self, residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow, warp_filter_size,
+                       source: torch.Tensor, layout: str = "planar", want_maps: bool = False) -> dict:
+        """Motion analysis of a P/B frame (``ccd_inter_analysis``, DESIGN §4.9), from the arguments of
+        reconstruct_frame and the frame's source samples (as for frame_distortion): one launch.  Returns ``sse``, per
+        variant (bitstream/motion.py VARIANTS order) the three per-plane sums of squared integer errors (None for the
+        beta variants of a P frame), and per reference ``refs``: a dict with ``sum`` (f64 sums of fx + gx, fy + gy and
+        |local|), ``max`` (max |local|) and ``outside`` (pixels sampled outside the reference), and on request
+        ``flow`` ([2, H, W] float32 CUDA, the total displacement)."""
+        f, keep, h, w = self._inter_frame(residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow,
+                                          warp_filter_size)
+        cs = 1 if frame_data_type == "yuv420" else 0
+        if not (source.is_cuda and source.is_contiguous() and source.dtype == (torch.uint8 if bitdepth <= 8 else torch.int16)
+                and source.numel() == h * w + 2 * (h >> cs) * (w >> cs)):
+            raise ValueError(f"source must hold the {h}x{w} {frame_data_type} frame's samples, contiguous on the device")
+        n_ref = 2 if is_b else 1
+        flows = [torch.empty((2, h, w), dtype=torch.float32, device=self.torch_device) for _ in range(n_ref)] if want_maps else []
+        an = CcdInterAnalysis(d_src=source.data_ptr(), src_layout=SOURCE_LAYOUTS[layout])
+        an.d_flow[:] = [t.data_ptr() for t in flows] + [None] * (2 - len(flows))
+        _check(self._lib.ccd_inter_analysis(self._h, ctypes.byref(f), ctypes.byref(an), self._stream()), [an])
+        del keep
+        sse = [[int(v) for v in an.sse[k]] for k in range(INTER_VARIANTS)]
+        if not is_b:
+            sse[3] = sse[4] = None
+        out = {"sse": sse, "refs": []}
+        for r in range(n_ref):
+            ref = {"sum": [float(v) for v in an.flow_sum[r]], "max": float(an.flow_max[r]), "outside": int(an.outside[r])}
+            if want_maps:
+                ref["flow"] = flows[r]
+            out["refs"].append(ref)
         return out
 
     def last_timing(self):

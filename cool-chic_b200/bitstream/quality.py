@@ -12,6 +12,9 @@ residue and motion just before that frame is reconstructed (``ccd_inter_stats``)
 call then covers every frame.  The source frames are read and uploaded in one pinned host-to-device copy, as the
 integers stored in the file.
 
+On request, the motion analysis of every P / B frame (``bitstream/motion.py``, DESIGN §4.9): one
+``ccd_inter_analysis`` launch next to ``ccd_inter_stats``, on the same inputs, so there is no second decode.
+
 On request, MS-SSIM (Wang, Simoncelli and Bovik 2003; DESIGN §4.6) from the same integers: one ``ccd_frame_ssim`` call
 for every frame whose planes all have both sides of at least 176 samples (five scales of at least 11), formed per plane
 on the host from the per-scale means, and per frame the pixel-weighted mean over the planes.  Smaller frames get None.
@@ -82,6 +85,7 @@ class FrameQuality:
     pred_map: Optional[torch.Tensor] = None    # [3, H, W] (P / B)
     ms_ssim_planes: Optional[List[float]] = None        # per plane; None: not asked for, or a plane below 176
     ssim_maps: Optional[List[torch.Tensor]] = None      # per plane, [h_c - 10, w_c - 10] scale-0 SSIM map
+    motion: Optional["MotionAnalysis"] = None  # noqa: F821  (bitstream/motion.py; P / B frames with motion=True)
     plane_mse: List[float] = field(init=False)
 
     def __post_init__(self):
@@ -178,10 +182,13 @@ def _upload_sources(ctx, by_display):
 
 @torch.no_grad()
 def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int = 0, max_decoding_order: int = -1,
-                  device: int = 0, want_maps: bool = False, ms_ssim: bool = False) -> Dict[str, FrameQuality]:
+                  device: int = 0, want_maps: bool = False, ms_ssim: bool = False,
+                  motion: bool = False) -> Dict[str, FrameQuality]:
     """Quality of every frame of an image / video bitstream against its source file (.yuv / .png / .ppm):
     ``{str(display_idx): FrameQuality}`` in display order.  ``ms_ssim`` adds MS-SSIM for every frame whose planes
-    all have both sides >= 176 (``ms_ssim_planes`` stays None for the others), with the SSIM maps if ``want_maps``.  A source whose format, bitdepth or size differs from the
+    all have both sides >= 176 (``ms_ssim_planes`` stays None for the others), with the SSIM maps if ``want_maps``.
+    ``motion`` fills ``FrameQuality.motion`` of every P / B frame (a MotionAnalysis, with the flow maps if
+    ``want_maps``); I frames keep None.  A source whose format, bitdepth or size differs from the
     decoded frames, or that has too few frames, raises ValueError before anything runs on the device."""
     frames = _frame_layout(memoryview(bytes(bitstream_bytes)), max_decoding_order)
     by_display = _read_sources(frames, original_path, frame_offset)
@@ -189,7 +196,9 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
     sources = _upload_sources(ctx, by_display)
 
     display_of = {coding_idx: disp for disp, (coding_idx, _, _, _) in by_display.items()}
-    stats = {}
+    from .motion import motion_analysis
+
+    stats, motions = {}, {}
     calls = [0]
 
     def reconstruct(frame_header, cc_out, reference_frames, dev):
@@ -203,6 +212,14 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
                 frame_header.get_value("bitdepth"), frame_header.get_value("global_flow"),
                 frame_header.get_value("warp_filter_size"), source=sources[disp], layout=by_display[disp][3].layout,
                 want_maps=want_maps)
+            if motion:
+                s = by_display[disp][3]
+                r = ctx.inter_analysis(
+                    cc_out["residue"], cc_out["motion"], refs, ftype == "B", s.frame_data_type, s.bitdepth,
+                    frame_header.get_value("global_flow"), frame_header.get_value("warp_filter_size"),
+                    source=sources[disp], layout=s.layout, want_maps=want_maps)
+                motions[disp] = motion_analysis(r, ftype, s.bitdepth, s.img_size, s.frame_data_type,
+                                                frame_header.get_value("global_flow"))
         return decode._reconstruct(frame_header, cc_out, reference_frames, dev)
 
     decoded = decode.decode_video_bytes(bitstream_bytes, max_decoding_order=max_decoding_order, device=device,
@@ -233,6 +250,7 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
             q.pred_psnr_db = pred_to_db(st["sums"][2], 3 * h * w)
             q.dummy_pred_psnr_db = pred_to_db(st["sums"][3], 3 * h * w)
             q.alpha_map, q.beta_map, q.pred_map = st.get("alpha"), st.get("beta"), st.get("pred")
+        q.motion = motions.get(d)
         if d in ssim:
             q.ms_ssim_planes = [ms_ssim_from_scales(c, s_) for c, s_ in zip(ssim[d]["cs"], ssim[d]["ssim"])]
             q.ssim_maps = ssim[d].get("maps")

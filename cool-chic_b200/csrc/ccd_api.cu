@@ -1989,6 +1989,53 @@ int ccd_inter_stats(CcdContext *ctx, const CcdInterFrame *frame, CcdInterStats *
     });
 }
 
+int ccd_inter_analysis(CcdContext *ctx, const CcdInterFrame *frame, CcdInterAnalysis *an, void *cuda_stream) {
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        InterLaunch L;
+        if (int rc = inter_launch_args(frame, L)) return rc;
+        if (!an || !an->d_src) return fail(CCD_ERR_ARG, "bad argument");
+        an->status = CCD_OK;
+        an->bad_index = -1;
+        if (frame->bitdepth < 1) return an->status = fail(CCD_ERR_ARG, "bad bitdepth %d", frame->bitdepth);
+        const int layout = an->src_layout;
+        if (layout < 0 || layout > 1 || (layout == 1 && frame->frame_data_type == 1))
+            return an->status = fail(CCD_ERR_ARG, "bad source layout %d for frame_data_type %d", layout, frame->frame_data_type);
+        const int64_t n_ctas = ccd_inter_stats_ctas(L.h, L.w);
+        // the results: sse, max bits and outside counts zeroed, the bad word ~0 (uploaded), then the partials (not)
+        Arena A;
+        const size_t off_sse = A.take(8 * 3 * CCD_INTER_VARIANTS, 8), off_max = A.take(16, 8), off_out = A.take(16, 8);
+        const size_t off_bad = A.take(8, 8), off_part = A.take(sizeof(double) * 6 * (size_t)n_ctas, 8);
+        if (int rc = stage(ctx, A)) return rc;
+        memset(A.h + off_sse, 0, off_bad - off_sse);
+        memset(A.h + off_bad, 0xff, 8);
+        CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
+        InterAnalysisOut o{};
+        o.src = an->d_src;
+        o.src_hwc = layout;
+        o.src_wide = frame->bitdepth > 8;
+        for (int r = 0; r < 2; r++) o.flow[r] = (r == 0 || L.is_b) ? an->d_flow[r] : nullptr;
+        o.sse = reinterpret_cast<unsigned long long *>(A.dv + off_sse);
+        o.max_bits = reinterpret_cast<unsigned long long *>(A.dv + off_max);
+        o.outside = reinterpret_cast<unsigned long long *>(A.dv + off_out);
+        o.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad);
+        o.part = reinterpret_cast<double *>(A.dv + off_part);
+        if (int rc = inter_launched(ccd_inter_analysis_launch(L, o, st), L.filter_size)) return an->status = rc;
+        if (int rc = download(A, 0, st, "inter_analysis")) return an->status = rc;
+        memcpy(an->sse, A.h + off_sse, sizeof(an->sse));
+        memcpy(an->outside, A.h + off_out, sizeof(an->outside));
+        const double *part = reinterpret_cast<const double *>(A.h + off_part);
+        for (int r = 0; r < 2; r++) {
+            uint64_t bits;
+            memcpy(&bits, A.h + off_max + 8 * r, 8);
+            memcpy(&an->flow_max[r], &bits, 8);
+            for (int k = 0; k < 3; k++) an->flow_sum[r][k] = ordered_sum(part + 3 * r + k, (size_t)n_ctas, 6);  // CTAs in order
+        }
+        return report(an, 1, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int) {
+            return fail(CCD_ERR_ARG, "non-finite flow at pixel %lld", (long long)an->bad_index);
+        });
+    });
+}
+
 int ccd_pack_frame(CcdContext *ctx, const float *const planes[3], int h, int w, int chroma_shift, int bitdepth,
                    int sample_bytes, int interleaved, void *d_out, void *cuda_stream) {
     return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {

@@ -307,6 +307,151 @@ __global__ void __launch_bounds__(128)
     if (t < 4) o.part[4 * ((size_t)blockIdx.y * gridDim.x + blockIdx.x) + t] = red[t][0];
 }
 
+// Motion analysis (DESIGN §4.9), in the 16 x 2 warp patches of k_inter_predict.  Each variant is the reconstruction of
+// k_inter_predict with one decoder input overridden (ccdec.h, CcdInterAnalysis), finished by the same frame tail and
+// compared with the source as k_frame_dist does: kd = rint(x * M) against ks, per-plane d^2 summed over the warp, one
+// integer atomic per warp.  The warp runs three times per reference (decoded flow, global shift only, no flow); the
+// alpha / beta / residue variants re-blend the decoded predictions.  Variants are formed one after the other, so only
+// one pair of predictions is live at a time.  Flow statistics per reference on the luma pixels: f64 sums in a
+// fixed-order CTA tree, max |local| as an integer atomicMax on its f64 bits (non-negative), an integer count outside.
+template <int N>
+__global__ void __launch_bounds__(128)
+    k_inter_analysis(const float *__restrict__ residue, const float *__restrict__ motion, RefPlanes ref0,
+                     RefPlanes ref1, int ref_cs, int h, int w, int is_b, int g0x, int g0y, int g1x, int g1y, float M,
+                     int out_420, InterAnalysisOut o) {
+    __shared__ double red[6][128];
+    const int t = threadIdx.x, lane = t & 31, wrp = t >> 5;
+    const int px = blockIdx.x * 32 + (wrp & 1) * 16 + (lane & 15);
+    const int py = blockIdx.y * 4 + (wrp >> 1) * 2 + (lane >> 4);
+    const bool inside = px < w && py < h;
+    const int x = px < w ? px : w - 1, y = py < h ? py : h - 1;  // every lane computes (shuffles below)
+    const size_t plane = (size_t)h * w, i = (size_t)y * w + x;
+    const int gx[2] = {g0x, g1x}, gy[2] = {g0y, g1y};
+
+    // ---- flow statistics of each reference
+    unsigned long long bad = ~0ull;
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+        double acc[3] = {0.0, 0.0, 0.0};
+        unsigned long long mbits = 0ull;
+        unsigned out = 0u;
+        if (inside && (r == 0 || is_b)) {
+            const float fx = motion[2 * r * plane + i], fy = motion[(2 * r + 1) * plane + i];
+            if (!(isfinite(fx) && isfinite(fy))) bad = (unsigned long long)i;
+            const double dx = (double)fx, dy = (double)fy;
+            acc[0] = __dadd_rn(dx, (double)gx[r]);
+            acc[1] = __dadd_rn(dy, (double)gy[r]);
+            acc[2] = __dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
+            mbits = (unsigned long long)__double_as_longlong(acc[2]);
+            const double sx = __dadd_rn(__dadd_rn((double)x, (double)gx[r]), dx);
+            const double sy = __dadd_rn(__dadd_rn((double)y, (double)gy[r]), dy);
+            out = (sx < 0.0 || sx > (double)(w - 1) || sy < 0.0 || sy > (double)(h - 1)) ? 1u : 0u;
+            if (o.flow[r]) {
+                o.flow[r][i] = __fadd_rn(fx, (float)gx[r]);
+                o.flow[r][plane + i] = __fadd_rn(fy, (float)gy[r]);
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 3; k++) red[3 * r + k][t] = acc[k];
+        for (int s = 16; s > 0; s >>= 1) {
+            const unsigned long long m = __shfl_down_sync(0xffffffffu, mbits, s);
+            mbits = m > mbits ? m : mbits;
+        }
+        out = __reduce_add_sync(0xffffffffu, out);
+        if (lane == 0) {
+            if (mbits) atomicMax(o.max_bits + r, mbits);
+            if (out) atomicAdd(o.outside + r, (unsigned long long)out);
+        }
+    }
+    for (int s = 16; s > 0; s >>= 1) {
+        const unsigned long long b = __shfl_down_sync(0xffffffffu, bad, s);
+        bad = b < bad ? b : bad;
+    }
+    if (lane == 0 && bad != ~0ull) atomicMin(o.bad, bad);
+
+    // ---- the source samples of this pixel: luma, and with 4:2:0 the chroma sample of its 2 x 2 block
+    const bool own420 = lane == (lane & ~17) && inside;  // the lane that counts a 4:2:0 chroma sample
+    int ks[3];
+    {
+        const size_t wc = (size_t)(w >> ref_cs), nc = (size_t)(h >> ref_cs) * wc;
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            const size_t k = o.src_hwc ? 3 * i + c
+                                       : (c == 0 ? i : plane + (c - 1) * nc + (size_t)(y >> ref_cs) * wc + (x >> ref_cs));
+            ks[c] = o.src_wide ? (int)__ldg(static_cast<const uint16_t *>(o.src) + k)
+                               : (int)__ldg(static_cast<const uint8_t *>(o.src) + k);
+        }
+    }
+    float res[3];
+#pragma unroll
+    for (int c = 0; c < 3; c++) res[c] = residue[c * plane + i];
+
+    // one variant: alpha * blend(beta, q0, q1) + (residue or 0), the frame tail of k_inter_predict, then the SSE
+    auto variant = [&](int v, float alpha, float beta, const float (&q0)[3], const float (&q1)[3], bool with_residue) {
+        float s[3];
+#pragma unroll
+        for (int c = 0; c < 3; c++)
+            s[c] = quant(__fadd_rn(__fmul_rn(alpha, blend(is_b, beta, q0[c], q1[c])), with_residue ? res[c] : 0.0f), M);
+        unsigned long long e[3];
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            float fin;
+            bool counts;
+            if (c == 0 || !out_420) {
+                fin = quant(clamp01(s[c]), M);
+                counts = inside;
+            } else {  // 2 x 2 average of the rounded chroma samples, as in k_inter_predict
+                const int base = lane & ~17;
+                float a = 0.0f;
+                a = __fadd_rn(a, __shfl_sync(0xffffffffu, s[c], base));
+                a = __fadd_rn(a, __shfl_sync(0xffffffffu, s[c], base + 1));
+                a = __fadd_rn(a, __shfl_sync(0xffffffffu, s[c], base + 16));
+                a = __fadd_rn(a, __shfl_sync(0xffffffffu, s[c], base + 17));
+                fin = quant(clamp01(__fdiv_rn(a, 4.0f)), M);
+                counts = own420;
+            }
+            const int d = (int)rintf(__fmul_rn(fin, M)) - ks[c];
+            e[c] = counts ? (unsigned long long)((long long)d * d) : 0ull;
+        }
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            for (int k = 16; k > 0; k >>= 1) e[c] += __shfl_down_sync(0xffffffffu, e[c], k);
+            if (lane == 0 && e[c]) atomicAdd(o.sse + 3 * v + c, e[c]);
+        }
+    };
+
+    float p0[3], p1[3], beta;
+    const float alpha = predict_refs<N>(residue, motion, ref0, ref1, ref_cs, h, w, is_b, g0x, g0y, g1x, g1y, x, y, p0,
+                                        p1, beta);
+    variant(0, alpha, beta, p0, p1, true);  // decoded
+    if (is_b) {
+        variant(3, alpha, 1.0f, p0, p1, true);  // ref0_only
+        variant(4, alpha, 0.0f, p0, p1, true);  // ref1_only
+    }
+    variant(5, alpha, beta, p0, p1, false);  // no_residue
+    variant(6, 0.0f, beta, p0, p1, true);    // no_prediction
+    // no_local_motion: zero local flow, the global shift kept; no_motion: no flow at all (a zero fractional offset
+    // does not make the sinc warp a copy, so both go through the warp)
+#pragma unroll 1
+    for (int z = 0; z < 2; z++) {
+        const int s0x = z ? 0 : g0x, s0y = z ? 0 : g0y, s1x = z ? 0 : g1x, s1y = z ? 0 : g1y;
+        predict_pixel<N>(ref0, ref_cs, h, w, s0x, s0y, 0.0f, 0.0f, x, y, p0);
+        if (is_b) predict_pixel<N>(ref1, ref_cs, h, w, s1x, s1y, 0.0f, 0.0f, x, y, p1);
+        variant(1 + z, alpha, beta, p0, p1, true);
+    }
+
+    // ---- flow sums: fixed-order tree over the CTA, one partial per CTA and per sum
+    __syncthreads();
+    for (int s = 64; s > 0; s >>= 1) {
+        if (t < s) {
+#pragma unroll
+            for (int k = 0; k < 6; k++) red[k][t] += red[k][t + s];
+        }
+        __syncthreads();
+    }
+    if (t < 6) o.part[6 * ((size_t)blockIdx.y * gridDim.x + blockIdx.x) + t] = red[t][0];
+}
+
 // One launch of a P/B kernel: launch(std::integral_constant<int, N>, grid, block, ref0, ref1) for the warp filter
 // size N of a, on one thread per pixel in CTAs of 128.  Returns -1 for a size no kernel is built for.
 template <class F>
@@ -340,6 +485,14 @@ int ccd_inter_stats_launch(const InterLaunch &a, const InterStatsOut &o, cudaStr
     return launch_inter(a, [&](auto n, dim3 grid, dim3 block, const RefPlanes &r0, const RefPlanes &r1) {
         k_inter_stats<decltype(n)::value><<<grid, block, 0, st>>>(a.residue, a.motion, r0, r1, a.ref_cs, a.h, a.w, a.is_b,
                                                                   a.gf[0], a.gf[1], a.gf[2], a.gf[3], o);
+    });
+}
+
+int ccd_inter_analysis_launch(const InterLaunch &a, const InterAnalysisOut &o, cudaStream_t st) {
+    return launch_inter(a, [&](auto n, dim3 grid, dim3 block, const RefPlanes &r0, const RefPlanes &r1) {
+        k_inter_analysis<decltype(n)::value><<<grid, block, 0, st>>>(a.residue, a.motion, r0, r1, a.ref_cs, a.h, a.w,
+                                                                     a.is_b, a.gf[0], a.gf[1], a.gf[2], a.gf[3], a.M,
+                                                                     a.out_420, o);
     });
 }
 

@@ -296,3 +296,18 @@ struct InterStatsOut {
 };
 int64_t ccd_inter_stats_ctas(int h, int w);
 int ccd_inter_stats_launch(const InterLaunch &a, const InterStatsOut &o, cudaStream_t st);
+// Motion analysis (k_inter_analysis, DESIGN §4.9): the finished frame of every variant (CCD_INTER_VARIANTS, in the
+// order of ccdec.h) against the source as k_frame_dist compares it, and the flow statistics of each reference.
+// Integer results (sse, max bits, outside, bad) are atomics on counters the host sets; the f64 flow sums are one
+// partial per CTA (ccd_inter_stats_ctas of them), d_part[6 * cta + 3 * r + k] for reference r and sum k.
+struct InterAnalysisOut {
+    const void *src;                // source samples (planar, or [h][w][3] for 4:4:4), layout of the frame
+    int src_hwc, src_wide;
+    float *flow[2];                 // optional [2][h][w] total displacement per reference
+    unsigned long long *sse;        // [CCD_INTER_VARIANTS][3], zeroed
+    unsigned long long *max_bits;   // [2] bits of the f64 max |local flow|, zeroed
+    unsigned long long *outside;    // [2], zeroed
+    unsigned long long *bad;        // smallest pixel index with a non-finite flow (~0 if none)
+    double *part;
+};
+int ccd_inter_analysis_launch(const InterLaunch &a, const InterAnalysisOut &o, cudaStream_t st);

@@ -329,6 +329,37 @@ typedef struct CcdInterStats {
 } CcdInterStats;
 int ccd_inter_stats(CcdContext *ctx, const CcdInterFrame *frame, CcdInterStats *stats, void *cuda_stream);
 
+/* Motion analysis of a P/B frame (DESIGN §4.9): what the motion, each reference and the residue buy.  A variant is the
+ * finished frame of ccd_reconstruct_frame with one change to its inputs (bitdepth >= 1):
+ *   0 decoded          none
+ *   1 no_local_motion  every motion channel := 0, global flow kept
+ *   2 no_motion        every motion channel := 0 and global flow := 0
+ *   3 ref0_only        residue channel 4 := +0.5 (beta = 1), B only
+ *   4 ref1_only        residue channel 4 := -0.5 (beta = 0), B only
+ *   5 no_residue       residue channels 0..2 := 0
+ *   6 no_prediction    residue channel 3 := -0.5 (alpha = 0)
+ * sse[v][c] (out): sum of d^2 over plane c of variant v, d = rint(x * M) - ks as ccd_frame_distortion computes it
+ * (exact; 0 for variants 3, 4 of a P frame).  d_src and src_layout as for CcdInterStats, the source is required.
+ * Per reference r (ref 1: B only, else 0), over the H W luma pixels, with (fx, fy) motion channels 2r, 2r + 1 and (gx, gy)
+ * its global flow: flow_sum[r] = sums of fx + gx, fy + gy and sqrt(fx^2 + fy^2), all in f64 (f64 partials per CTA
+ * added in tile order, the same on every run); flow_max[r] = max sqrt(fx^2 + fy^2); outside[r] = pixels whose sample
+ * position x + gx + fx or y + gy + fy (f64) lies outside [0, W - 1] or [0, H - 1].  d_flow[r] (optional): [2][H][W]
+ * fp32 fx + gx, fy + gy.  A non-finite flow makes the call CCD_ERR_ARG with bad_index = the smallest such pixel
+ * (row-major; else -1).  One launch; synchronous. */
+#define CCD_INTER_VARIANTS 7
+typedef struct CcdInterAnalysis {
+    const void *d_src;
+    int32_t src_layout;
+    float *d_flow[2];
+    uint64_t sse[CCD_INTER_VARIANTS][3];
+    double flow_sum[2][3];
+    double flow_max[2];
+    uint64_t outside[2];
+    int64_t bad_index;
+    int32_t status;
+} CcdInterAnalysis;
+int ccd_inter_analysis(CcdContext *ctx, const CcdInterFrame *frame, CcdInterAnalysis *analysis, void *cuda_stream);
+
 /* Device-side evaluation of the quantised-Laplace left cumulative for testing the f64
  * exp() agreement with the host (SURVEY Appendix C.3): for sc in [sc_lo, sc_hi) and every
  * numerator index n in [0, 32641) (|d| = n/256), writes to host arrays

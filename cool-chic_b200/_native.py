@@ -28,7 +28,7 @@ EXPORTS = [
     "ccd_version", "ccd_sizeof_desc", "ccd_last_error", "ccd_create", "ccd_destroy", "ccd_nn_count",
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
     "ccd_encode_latents", "ccd_synthesize_many", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
-    "ccd_latent_rate", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats", "ccd_inter_analysis",
+    "ccd_latent_rate", "ccd_latent_rate_edited", "ccd_rate_sweep", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats", "ccd_inter_analysis",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
     "ccd_debug_entropy_plan", "ccd_debug_cdf_table",
 ]
@@ -89,6 +89,33 @@ class CcdRateJob(ctypes.Structure):
         ("d_mu_sc", ctypes.c_void_p),
         ("d_spatial", ctypes.c_void_p),
         ("grid_bits", ctypes.c_double * CCD_MAX_GRIDS),
+        ("bad_index", ctypes.c_int64),
+        ("status", ctypes.c_int32),
+    ]
+
+
+class CcdModelEdit(ctypes.Structure):
+    """ARM inputs read as 0 (DESIGN §4.10): spatial inputs (bits of ``zero_ctx``), IFCE features (``zero_ifce_out``),
+    latent grids wherever they are an IFCE input (``zero_ifce_grids``, bit 0 = the finest grid)."""
+    _fields_ = [
+        ("zero_ctx", ctypes.c_uint64),
+        ("zero_ifce_out", ctypes.c_uint32),
+        ("zero_ifce_grids", ctypes.c_uint32),
+    ]
+
+
+SWEEP_MAX_OFFSETS = 32  # CCD_SWEEP_MAX_OFFSETS
+
+
+class CcdSweepJob(ctypes.Structure):
+    _fields_ = [
+        ("desc", ctypes.POINTER(CcdCoolChicDesc)),
+        ("d_latents", ctypes.c_void_p),
+        ("d_mu_sc", ctypes.c_void_p),
+        ("n_offsets", ctypes.c_int32),
+        ("sc_offset", ctypes.c_int32 * SWEEP_MAX_OFFSETS),
+        ("bits", (ctypes.c_double * SWEEP_MAX_OFFSETS) * CCD_MAX_GRIDS),
+        ("hist", (ctypes.c_uint64 * 128) * CCD_MAX_GRIDS),
         ("bad_index", ctypes.c_int64),
         ("status", ctypes.c_int32),
     ]
@@ -235,6 +262,10 @@ def load_library():
         L.ccd_pack_samples.argtypes = [vp, vp, ctypes.c_size_t, ci, ci, vp, vp]
         L.ccd_latent_rate.restype = ci
         L.ccd_latent_rate.argtypes = [vp, ctypes.POINTER(CcdRateJob), ci, vp]
+        L.ccd_latent_rate_edited.restype = ci
+        L.ccd_latent_rate_edited.argtypes = [vp, ctypes.POINTER(CcdRateJob), ctypes.POINTER(CcdModelEdit), ci, vp]
+        L.ccd_rate_sweep.restype = ci
+        L.ccd_rate_sweep.argtypes = [vp, ctypes.POINTER(CcdSweepJob), ci, vp]
         L.ccd_frame_distortion.restype = ci
         L.ccd_frame_distortion.argtypes = [vp, ctypes.POINTER(CcdDistJob), ci, vp]
         L.ccd_frame_ssim.restype = ci
@@ -617,14 +648,17 @@ class Context:
 
     def latent_rate(self, descs: Sequence[CcdCoolChicDesc], nn_ints: Sequence[np.ndarray],
                     latents: Sequence[torch.Tensor], want_freq: bool = False, want_mu_sc: bool = False,
-                    want_spatial: bool = False) -> List[dict]:
+                    want_spatial: bool = False, edits=None) -> List[dict]:
         """Rate of decoded latents (``ccd_latent_rate``): one kernel launch for all Cool-chics, plus one for the
         spatial maps.  ``latents[i]``: int8 CUDA tensor in decode order (what ``decode_many(want_latents=True)``
         returns).  Per Cool-chic a dict with ``bits`` (float32 CUDA [n_symbols], decode order), ``grid_bits``
         (list of f64, grid 0 = finest), and on request ``freq`` / ``mu_sc`` (int32 CUDA holding the uint32
-        values) and ``spatial`` ([1, 1, H, W] float32 CUDA)."""
+        values) and ``spatial`` ([1, 1, H, W] float32 CUDA).  ``want_mu_sc`` may also be one flag per Cool-chic.
+        ``edits[i]`` (``ccd_latent_rate_edited``, DESIGN §4.10): a (zero_ctx, zero_ifce_out, zero_ifce_grids) triple of
+        ARM inputs read as 0 for Cool-chic i; several edits of one Cool-chic are several jobs on the same latents."""
         n = len(descs)
         jobs = (CcdRateJob * n)()
+        mu_sc_flags = [bool(want_mu_sc)] * n if isinstance(want_mu_sc, bool) else [bool(f) for f in want_mu_sc]
         keep, res = [], []
         dev = self.torch_device
         for i in range(n):
@@ -636,7 +670,7 @@ class Context:
             r = {"bits": torch.empty((d.n_symbols(),), dtype=torch.float32, device=dev)}
             if want_freq:
                 r["freq"] = torch.empty((d.n_symbols(),), dtype=torch.int32, device=dev)
-            if want_mu_sc:
+            if mu_sc_flags[i]:
                 r["mu_sc"] = torch.empty((d.n_symbols(),), dtype=torch.int32, device=dev)
             if want_spatial:
                 r["spatial"] = torch.empty((1, 1, d.img_h, d.img_w), dtype=torch.float32, device=dev)
@@ -646,13 +680,44 @@ class Context:
             jobs[i].d_latents = lat.data_ptr()
             jobs[i].d_bits = r["bits"].data_ptr()
             jobs[i].d_freq = r["freq"].data_ptr() if want_freq else None
-            jobs[i].d_mu_sc = r["mu_sc"].data_ptr() if want_mu_sc else None
+            jobs[i].d_mu_sc = r["mu_sc"].data_ptr() if mu_sc_flags[i] else None
             jobs[i].d_spatial = r["spatial"].data_ptr() if want_spatial else None
             res.append(r)
-        _check(self._lib.ccd_latent_rate(self._h, jobs, n, self._stream()), jobs)
+        if edits is None:
+            _check(self._lib.ccd_latent_rate(self._h, jobs, n, self._stream()), jobs)
+        else:
+            ed = (CcdModelEdit * n)(*[CcdModelEdit(*(int(v) for v in e)) for e in edits])
+            _check(self._lib.ccd_latent_rate_edited(self._h, jobs, ed, n, self._stream()), jobs)
         for i in range(n):
             res[i]["grid_bits"] = [float(jobs[i].grid_bits[g]) for g in range(descs[i].n_grids)]
         return res
+
+    def rate_sweep(self, descs: Sequence[CcdCoolChicDesc], latents: Sequence[torch.Tensor],
+                   mu_sc: Sequence[torch.Tensor], sc_offsets: Sequence[int]) -> List[dict]:
+        """Scale-calibration sweep and symbol histograms of decoded latents (``ccd_rate_sweep``, DESIGN §4.10): one
+        launch for all Cool-chics.  ``latents[i]`` as for latent_rate, ``mu_sc[i]`` the (mu_idx, sc_idx) the coder used
+        (latent_rate's ``mu_sc``); ``sc_offsets``: 1 to 32 offsets of sc_idx.  Per Cool-chic a dict with ``bits``
+        (per grid, finest first, the f64 bits at each offset) and ``hist`` (int64 [n_grids, 128], count of symbol
+        s - 64 in bin s)."""
+        n = len(descs)
+        jobs = (CcdSweepJob * n)()
+        offs = [int(o) for o in sc_offsets]
+        if not 1 <= len(offs) <= SWEEP_MAX_OFFSETS:
+            raise ValueError(f"{len(offs)} scale offsets, the sweep takes 1 to {SWEEP_MAX_OFFSETS}")
+        for i in range(n):
+            d, lat, ms = descs[i], latents[i], mu_sc[i]
+            for name, t, dt in (("latents", lat, torch.int8), ("mu_sc", ms, torch.int32)):
+                if not (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == d.n_symbols()):
+                    raise ValueError(f"{name}[{i}] must be a contiguous {dt} CUDA tensor of {d.n_symbols()} symbols")
+            jobs[i].desc = ctypes.pointer(d)
+            jobs[i].d_latents = lat.data_ptr()
+            jobs[i].d_mu_sc = ms.data_ptr()
+            jobs[i].n_offsets = len(offs)
+            jobs[i].sc_offset[:len(offs)] = offs
+        _check(self._lib.ccd_rate_sweep(self._h, jobs, n, self._stream()), jobs)
+        return [{"bits": [list(jobs[i].bits[g])[:len(offs)] for g in range(descs[i].n_grids)],
+                 "hist": np.array([list(jobs[i].hist[g]) for g in range(descs[i].n_grids)], dtype=np.int64)}
+                for i in range(n)]
 
     def _frame_jobs(self, job_type, frames, sources, layouts):
         """The job array of a call that compares finished frames with their source samples (frame_distortion,

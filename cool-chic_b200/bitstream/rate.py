@@ -129,9 +129,8 @@ def _split_coolchic(buf):
     return h, bytes(rest[:n_nn]), bytes(rest[n_nn:n_nn + n_lat]), rest[n_nn + n_lat:]
 
 
-def _rates(headers: List[CoolChicHeader], nn_bytes: List[bytes], lat_bytes: List[bytes], device: int
-           ) -> List[CoolChicRate]:
-    """One decode_many for the latents of every Cool-chic, then one ccd_latent_rate call."""
+def _decode_latents(headers: List[CoolChicHeader], nn_bytes: List[bytes], lat_bytes: List[bytes], device: int):
+    """(context, descriptors, NN integers, decoded latents) of every Cool-chic: one decode_many."""
     ctx = _native.get_context(device)
     descs = [desc_from_header(h) for h in headers]
     for h, nb, lb in zip(headers, nn_bytes, lat_bytes):
@@ -141,6 +140,13 @@ def _rates(headers: List[CoolChicHeader], nn_bytes: List[bytes], lat_bytes: List
     lat_bytes = [bytes(lb[:h.get_value("n_bytes_latent")]) for h, lb in zip(headers, lat_bytes)]
     _, lats = ctx.decode_many(descs, nn_bytes, lat_bytes, want_latents=True)
     nns = [_native.decode_nn(d, nb) for d, nb in zip(descs, nn_bytes)]
+    return ctx, descs, nns, lats
+
+
+def _rates(headers: List[CoolChicHeader], nn_bytes: List[bytes], lat_bytes: List[bytes], device: int
+           ) -> List[CoolChicRate]:
+    """One decode_many for the latents of every Cool-chic, then one ccd_latent_rate call."""
+    ctx, descs, nns, lats = _decode_latents(headers, nn_bytes, lat_bytes, device)
     return _rates_of_latents(ctx, headers, descs, nns, lats)
 
 
@@ -182,10 +188,10 @@ def coolchic_rate(header: CoolChicHeader, bytes_nn: bytes, bytes_latent: bytes, 
     return _rates([header], [bytes_nn], [bytes_latent], device)[0]
 
 
-@torch.no_grad()
-def video_rate(bitstream_bytes: bytes, max_decoding_order: int = -1, device: int = 0) -> Dict[str, FrameRate]:
-    """Rate of every frame of an image / video bitstream: ``{str(display_idx): FrameRate}``.  All Cool-chics
-    (residue, and motion for P / B frames) go through one decode and one rate call."""
+def _split_frames(bitstream_bytes: bytes, max_decoding_order: int = -1):
+    """(coding structure, frames, flat) of an image / video bitstream: per frame in coding order (coding_idx, frame
+    header, {Cool-chic name: index in flat}, bytes of the frame), and flat the (header, nn bytes, latent bytes) of
+    every Cool-chic (residue, and motion for P / B frames) in bitstream order."""
     buf = memoryview(bytes(bitstream_bytes))
     video_header = VideoHeader()
     buf = video_header.read_header(buf)
@@ -204,6 +210,14 @@ def video_rate(bitstream_bytes: bytes, max_decoding_order: int = -1, device: int
             ccs[name] = len(flat)
             flat.append((h, nb, lb))
         frames.append((coding_idx, fh, ccs, n_frame - len(buf)))
+    return cs, frames, flat
+
+
+@torch.no_grad()
+def video_rate(bitstream_bytes: bytes, max_decoding_order: int = -1, device: int = 0) -> Dict[str, FrameRate]:
+    """Rate of every frame of an image / video bitstream: ``{str(display_idx): FrameRate}``.  All Cool-chics
+    (residue, and motion for P / B frames) go through one decode and one rate call."""
+    cs, frames, flat = _split_frames(bitstream_bytes, max_decoding_order)
     rates = _rates([f[0] for f in flat], [f[1] for f in flat], [f[2] for f in flat], device) if flat else []
     out = {}
     for coding_idx, fh, ccs, n_bytes in frames:

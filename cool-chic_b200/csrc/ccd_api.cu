@@ -629,10 +629,35 @@ int prepare_synthesis(PreparedJob &P, const int64_t *nn_ints_opt) {
     return CCD_OK;
 }
 
+// Input i of a fixed-point layer read as 0 (DESIGN §4.10): its row of the transposed weights, the +I entry of a
+// residual layer included, set to 0.  The row feeds nothing else, so the layer's output is exactly the unedited
+// layer's on an input whose entry i is 0.
+void zero_input_row(std::vector<int64_t> &W, int i, int n_out) {
+    for (int o = 0; o < n_out; o++) W[(size_t)i * n_out + o] = 0;
+}
+
+// The checks of ccd_latent_rate_edited on one job's edit, against its descriptor
+int check_edit(const CcdModelEdit &e, const CcdCoolChicDesc *d, int i) {
+    if (int rc = validate_desc(d)) return rc;
+    const int cf = d->flag_ifce ? d->n_ifce_out : 0;
+    if (d->n_ctx < 64 && (e.zero_ctx >> d->n_ctx))
+        return fail(CCD_ERR_ARG, "job %d: zero_ctx 0x%llx has a bit at or above n_ctx %d", i, (unsigned long long)e.zero_ctx,
+                    d->n_ctx);
+    if (!d->flag_ifce && (e.zero_ifce_out || e.zero_ifce_grids))
+        return fail(CCD_ERR_ARG, "job %d: an IFCE edit on a model without IFCE", i);
+    if ((uint64_t)e.zero_ifce_out >> cf)
+        return fail(CCD_ERR_ARG, "job %d: zero_ifce_out 0x%x has a bit at or above n_ifce_out %d", i, e.zero_ifce_out, cf);
+    if ((uint64_t)e.zero_ifce_grids >> d->n_grids)
+        return fail(CCD_ERR_ARG, "job %d: zero_ifce_grids 0x%x has a bit at or above n_grids %d", i, e.zero_ifce_grids,
+                    d->n_grids);
+    return CCD_OK;
+}
+
 // Host preparation of one job: prepare_synthesis, then the entropy stage's ARM / IFCE packing and stream descriptor.
 // The descriptor's grid table covers the decode-order grids [gb, ge) (ge < 0: to the last), each with its absolute
-// latent and IFCE offsets; the shared-memory plan covers those grids.
-int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt, int gb = 0, int ge = -1) {
+// latent and IFCE offsets; the shared-memory plan covers those grids.  edit (rate analysis only, checked by
+// check_edit): the ARM and IFCE inputs it names are read as 0, applied to the integers before the fast-path choice.
+int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt, int gb = 0, int ge = -1, const CcdModelEdit *edit = nullptr) {
     if (int rc = prepare_synthesis(P, nn_ints_opt)) return rc;
     const CcdCoolChicDesc *d = P.d;
     const NNLayout &L = P.L;
@@ -649,6 +674,14 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt, int gb = 0, int ge =
                             d->arm_stab ? nn + L.arm_w[L.n_arm_lin] : nullptr,
                             d->arm_stab ? nn + L.arm_b[L.n_arm_lin] : nullptr, d->qshift[0], d->qshift[1], true,
                             d->n_ifce_out, false);
+    if (edit) {
+        for (int i = 0; i < dim; i++) {
+            const bool z = i < d->n_ctx ? ((edit->zero_ctx >> i) & 1u) : ((edit->zero_ifce_out >> (i - d->n_ctx)) & 1u);
+            if (!z) continue;
+            zero_input_row(arm.W[0], i, arm.n_hidden ? dim : 2);
+            zero_input_row(arm.Ws, i, 2);
+        }
+    }
     std::vector<ArmInts> ifce;
     i128 feat_bound = 0;
     bool fast = ccd_entropy_has_fast(d->n_ctx, d->n_ifce_out);
@@ -658,6 +691,12 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt, int gb = 0, int ge =
         // component/coolchic.py:114-123
         ifce.push_back(build_arm(d->grid_ifce_in[L.ifce_grid[j]], 0, d->n_ifce_out, w1, b1, nullptr, nullptr,
                                  d->qshift[2], d->qshift[3], false, 0, true));
+        if (edit) {  // channel c of grid g reads grid g + 1 + c
+            const int g = L.ifce_grid[j];
+            for (int c = 0; c < d->grid_ifce_in[g]; c++)
+                if (g + 1 + c < d->n_grids && ((edit->zero_ifce_grids >> (g + 1 + c)) & 1u))
+                    zero_input_row(ifce.back().W[0], c, d->n_ifce_out);
+        }
         i128 bnd = 0;
         if (!ifce_bound(ifce.back(), &bnd)) fast = false;
         if (d->grid_ifce_in[L.ifce_grid[j]] > CCD_IFCE_FAST_MAX) fast = false;
@@ -1631,7 +1670,10 @@ int ccd_synthesize_many(CcdContext *ctx, CcdSynthJob *jobs, int n_jobs, void *cu
     return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return synthesize_body(ctx, jobs, n_jobs, st); });
 }
 
-static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaStream_t st) {
+static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, const CcdModelEdit *edits, int n_jobs, cudaStream_t st) {
+    if (edits)
+        for (int i = 0; i < n_jobs; i++)
+            if (int rc = check_edit(edits[i], jobs[i].desc, i)) return jobs[i].status = rc;
     std::vector<PreparedJob> P((size_t)n_jobs);
     std::vector<RateTile> tiles;
     // tiles of job i, decode-order grid gi: [tile_at[i][gi], tile_at[i][gi + 1])
@@ -1646,7 +1688,8 @@ static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaS
         if (!R.desc || !R.nn_ints || !R.d_latents || !R.d_bits) return R.status = fail(CCD_ERR_ARG, "job %d: null pointer", i);
         PreparedJob &J = P[(size_t)i];
         J.d = R.desc;
-        int rc = prepare_job(J, R.nn_ints);  // the decoder's build_arm / pack_arm / pack_ifce and fast-path choice
+        // the decoder's build_arm / pack_arm / pack_ifce and fast-path choice
+        int rc = prepare_job(J, R.nn_ints, 0, -1, edits ? edits + i : nullptr);
         if (rc) return R.status = rc;
         J.off_blob = A.take(J.blob.size());
         smem = std::max(smem, ccd_rate_smem_bytes(J.es.arm_blob_bytes, J.es.ifce_blob_max));
@@ -1729,7 +1772,100 @@ static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, cudaS
 }
 
 int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_stream) {
-    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return latent_rate_body(ctx, jobs, n_jobs, st); });
+    return job_call(ctx, jobs, n_jobs, cuda_stream,
+                    [&](cudaStream_t st) -> int { return latent_rate_body(ctx, jobs, nullptr, n_jobs, st); });
+}
+
+int ccd_latent_rate_edited(CcdContext *ctx, CcdRateJob *jobs, const CcdModelEdit *edits, int n_jobs, void *cuda_stream) {
+    return job_call(ctx, jobs, n_jobs, cuda_stream,
+                    [&](cudaStream_t st) -> int { return latent_rate_body(ctx, jobs, edits, n_jobs, st); });
+}
+
+static int rate_sweep_body(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, cudaStream_t st) {
+    std::vector<RateTile> tiles;
+    std::vector<size_t> tile_at;  // tiles of job i, decode-order grid gi: [tile_at[k], tile_at[k + 1]), k = hist_at[i] + gi
+    std::vector<size_t> hist_at((size_t)n_jobs);  // first decode-order grid of job i in the histogram array
+    std::vector<SweepJobDev> D((size_t)n_jobs);
+    size_t n_hist = 0;
+    for (int i = 0; i < n_jobs; i++) {
+        CcdSweepJob &S = jobs[i];
+        S.bad_index = -1;
+        if (!S.desc || !S.d_latents || !S.d_mu_sc) return S.status = fail(CCD_ERR_ARG, "job %d: null pointer", i);
+        if (int rc = validate_desc(S.desc)) return S.status = rc;
+        if (S.n_offsets < 1 || S.n_offsets > CCD_SWEEP_MAX_OFFSETS)
+            return S.status = fail(CCD_ERR_ARG, "job %d: n_offsets %d outside 1 .. %d", i, S.n_offsets, CCD_SWEEP_MAX_OFFSETS);
+        for (int k = 0; k < S.n_offsets; k++)
+            if (S.sc_offset[k] < -2560 || S.sc_offset[k] > 2560)
+                return S.status = fail(CCD_ERR_ARG, "job %d: scale offset %d outside [-2560, 2560]", i, S.sc_offset[k]);
+        const CcdCoolChicDesc *d = S.desc;
+        SweepJobDev &J = D[(size_t)i];
+        memset(&J, 0, sizeof(J));
+        int64_t off_by_grid[CCD_MAX_GRIDS];
+        ccd_latent_count(d, off_by_grid);
+        J.lat = S.d_latents;
+        J.mu_sc = S.d_mu_sc;
+        J.n_off = S.n_offsets;
+        for (int k = 0; k < S.n_offsets; k++) J.off[k] = S.sc_offset[k];
+        hist_at[(size_t)i] = n_hist;
+        for (int gi = 0; gi < d->n_grids; gi++) {
+            const int g = d->n_grids - 1 - gi;
+            J.h[gi] = d->grid_h[g];
+            J.w[gi] = d->grid_w[g];
+            J.lat_off[gi] = off_by_grid[g];
+            tile_at.push_back(tiles.size());
+            for (int y0 = 0; y0 < J.h[gi]; y0 += CCD_RATE_TH)
+                for (int x0 = 0; x0 < J.w[gi]; x0 += CCD_RATE_TW) tiles.push_back(RateTile{i, gi, y0, x0});
+        }
+        n_hist += (size_t)d->n_grids;
+    }
+    tile_at.push_back(tiles.size());
+    if (tiles.size() > (size_t)INT32_MAX) return fail(CCD_ERR_UNSUPPORTED, "too many rate tiles");
+    Arena A;
+    const size_t off_jobs = A.take(sizeof(SweepJobDev) * (size_t)n_jobs);
+    const size_t off_tiles = A.take(sizeof(RateTile) * tiles.size());
+    // results: the bad words (~0) and the histograms (0) on the way up, then the partials, which are not uploaded
+    const size_t off_bad = A.take(sizeof(unsigned long long) * (size_t)n_jobs);
+    const size_t off_hist = A.take(sizeof(unsigned long long) * 128 * n_hist);
+    const size_t off_part = A.take(sizeof(double) * CCD_SWEEP_MAX_OFFSETS * tiles.size());
+    if (int rc = stage(ctx, A)) return rc;
+    for (int i = 0; i < n_jobs; i++) {
+        D[(size_t)i].bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
+        D[(size_t)i].hist = reinterpret_cast<unsigned long long *>(A.dv + off_hist) + 128 * hist_at[(size_t)i];
+    }
+    memcpy(A.h + off_jobs, D.data(), sizeof(SweepJobDev) * (size_t)n_jobs);
+    memcpy(A.h + off_tiles, tiles.data(), sizeof(RateTile) * tiles.size());
+    memset(A.h + off_bad, 0xff, sizeof(unsigned long long) * (size_t)n_jobs);
+    memset(A.h + off_hist, 0, sizeof(unsigned long long) * 128 * n_hist);
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
+    int e = ccd_rate_sweep_launch(reinterpret_cast<const RateTile *>(A.dv + off_tiles), (int)tiles.size(),
+                                  reinterpret_cast<const SweepJobDev *>(A.dv + off_jobs), ctx->d_cdf, ctx->d_scale,
+                                  reinterpret_cast<double *>(A.dv + off_part), st);
+    if (e != 0) return fail(CCD_ERR_CUDA, "sweep kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    if (int rc = download(A, off_bad, st, "sweep kernel")) return rc;
+    const double *part = reinterpret_cast<const double *>(A.h + off_part);
+    const unsigned long long *hist = reinterpret_cast<const unsigned long long *>(A.h + off_hist);
+    for (int i = 0; i < n_jobs; i++) {
+        CcdSweepJob &S = jobs[i];
+        const int n_grids = S.desc->n_grids;
+        memset(S.bits, 0, sizeof(S.bits));
+        memset(S.hist, 0, sizeof(S.hist));
+        for (int gi = 0; gi < n_grids; gi++) {
+            const int g = n_grids - 1 - gi;
+            const size_t k0 = hist_at[(size_t)i] + (size_t)gi;  // a grid's sum: its tiles in order
+            for (int k = 0; k < S.n_offsets; k++)
+                S.bits[g][k] = ordered_sum(part + CCD_SWEEP_MAX_OFFSETS * tile_at[k0] + k, tile_at[k0 + 1] - tile_at[k0],
+                                           CCD_SWEEP_MAX_OFFSETS);
+            for (int s = 0; s < 128; s++) S.hist[g][s] = hist[128 * k0 + s];
+        }
+    }
+    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {
+        return fail(CCD_ERR_ARG, "job %d: symbol %lld has a latent outside [-64, 63] or a (mu_idx, sc_idx) outside its table",
+                    i, (long long)jobs[i].bad_index);
+    });
+}
+
+int ccd_rate_sweep(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, void *cuda_stream) {
+    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return rate_sweep_body(ctx, jobs, n_jobs, st); });
 }
 
 // The checks of a job that compares a finished frame with its source samples (CcdDistJob, CcdSsimJob)

@@ -1405,18 +1405,10 @@ int launch_t(const EntStream *d_streams, int n, size_t smem, int threads, const 
 // GenericArm on the same row-ring layout, fed from a staged tile instead of the wavefront -- and turns the
 // symbol's cumulative window into freq = left(s+1) - left(s) and bits = 24 - log2(freq).
 // =======================================================================================
-// One symbol: clamp (latent.py:165, rangecoder.py:89-91), then the exact interval the range coder used: the
-// table window for s_lo <= s < s_lo + 31 (what the coder reads), the f64 model outside it.  Returns the f64 bits.
-__device__ __forceinline__ double rate_symbol(long long o0, long long o1, int sym, long long idx, const RateJobDev &J,
-                                              const uint32_t *__restrict__ cdf, const float *__restrict__ scale_tab) {
-    long long im = o0 + 16384, is = o1 + 1280;
-    im = im < 0 ? 0 : (im > 32767 ? 32767 : im);
-    is = is < 0 ? 0 : (is > 2560 ? 2560 : is);
-    const int mu_idx = (int)im, sc_idx = (int)is;
-    if (sym < kSymMin || sym > kSymMax) {
-        atomicMin(J.bad, (unsigned long long)idx);
-        return 0.0;
-    }
+// The exact interval the range coder used for symbol sym in [-64, 63] under clamped (mu_idx, sc_idx): the table window
+// for s_lo <= s < s_lo + 31 (what the coder reads), the f64 model outside it.  Returns freq = left(s+1) - left(s).
+__device__ __forceinline__ uint32_t coder_freq(int sym, int mu_idx, int sc_idx, const uint32_t *__restrict__ cdf,
+                                               const float *__restrict__ scale_tab) {
     const int mu_int = ((mu_idx + 128) >> 8) - 64;
     const int fr = (mu_idx + 128) & 255;
     const int t = sym - (mu_int - CCD_WIN_HALF);
@@ -1431,7 +1423,21 @@ __device__ __forceinline__ double rate_symbol(long long o0, long long o1, int sy
         l0 = laplace_left_exact(sym, mu, b);
         l1 = laplace_left_exact(sym + 1, mu, b);
     }
-    const uint32_t freq = l1 - l0;
+    return l1 - l0;
+}
+
+// One symbol: clamp (latent.py:165, rangecoder.py:89-91), then the coder's interval.  Returns the f64 bits.
+__device__ __forceinline__ double rate_symbol(long long o0, long long o1, int sym, long long idx, const RateJobDev &J,
+                                              const uint32_t *__restrict__ cdf, const float *__restrict__ scale_tab) {
+    long long im = o0 + 16384, is = o1 + 1280;
+    im = im < 0 ? 0 : (im > 32767 ? 32767 : im);
+    is = is < 0 ? 0 : (is > 2560 ? 2560 : is);
+    const int mu_idx = (int)im, sc_idx = (int)is;
+    if (sym < kSymMin || sym > kSymMax) {
+        atomicMin(J.bad, (unsigned long long)idx);
+        return 0.0;
+    }
+    const uint32_t freq = coder_freq(sym, mu_idx, sc_idx, cdf, scale_tab);
     const double bits = 24.0 - log2((double)freq);
     J.bits[idx] = (float)bits;
     if (J.freq) J.freq[idx] = freq;
@@ -1543,6 +1549,66 @@ __global__ void __launch_bounds__(CCD_RATE_THREADS)
     }
 }
 
+// Scale-calibration sweep (DESIGN §4.10): every symbol of the tile is read once (latent and (mu_idx, sc_idx), 5 bytes)
+// into registers and counted in the grid's histogram, then each offset k costs one interval per symbol at the shifted,
+// clamped scale index.  Per k: lanes (butterfly), then the warps in order -- the same partial on every run.
+__global__ void __launch_bounds__(CCD_RATE_THREADS)
+    k_rate_sweep(const RateTile *__restrict__ tiles, const SweepJobDev *__restrict__ jobs, const uint32_t *__restrict__ cdf,
+                 const float *__restrict__ scale_tab, double *__restrict__ part) {
+    __shared__ unsigned int hist[128];
+    __shared__ double wsum[CCD_SWEEP_MAX_OFFSETS][CCD_RATE_THREADS / 32];
+    const RateTile t = tiles[blockIdx.x];
+    const SweepJobDev &J = jobs[t.job];
+    const int tid = threadIdx.x;
+    if (tid < 128) hist[tid] = 0u;
+    __syncthreads();
+    const int w = J.w[t.grid];
+    const long long base = J.lat_off[t.grid];
+    const int nc = min(CCD_RATE_TW, w - t.x0);
+    const int n = min(CCD_RATE_TH, J.h[t.grid] - t.y0) * nc;
+    int sym[CCD_SWEEP_SPT];
+    uint32_t ms[CCD_SWEEP_SPT];
+#pragma unroll
+    for (int j = 0; j < CCD_SWEEP_SPT; j++) {
+        const int s = tid + j * CCD_RATE_THREADS;
+        sym[j] = 0x7fffffff;  // no symbol
+        ms[j] = 0u;
+        if (s >= n) continue;
+        const int ty = s / nc, tx = s - ty * nc;
+        const long long idx = base + (long long)(t.y0 + ty) * w + (t.x0 + tx);
+        const int v = J.lat[idx];
+        ms[j] = __ldg(J.mu_sc + idx);
+        if (v < kSymMin || v > kSymMax || (ms[j] & 0xFFFFu) > 32767u || (ms[j] >> 16) > 2560u) {
+            atomicMin(J.bad, (unsigned long long)idx);
+            continue;
+        }
+        sym[j] = v;
+        atomicAdd(&hist[v - kSymMin], 1u);
+    }
+    const int n_off = J.n_off;
+    for (int k = 0; k < n_off; k++) {
+        const int d = J.off[k];
+        double acc = 0.0;
+#pragma unroll
+        for (int j = 0; j < CCD_SWEEP_SPT; j++) {
+            if (sym[j] == 0x7fffffff) continue;
+            int s2 = (int)(ms[j] >> 16) + d;
+            s2 = s2 < 0 ? 0 : (s2 > 2560 ? 2560 : s2);
+            acc += 24.0 - log2((double)coder_freq(sym[j], (int)(ms[j] & 0xFFFFu), s2, cdf, scale_tab));
+        }
+#pragma unroll
+        for (int m = 16; m > 0; m >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, m);
+        if ((tid & 31) == 0) wsum[k][tid >> 5] = acc;
+    }
+    __syncthreads();
+    if (tid < n_off) {
+        double s = 0.0;
+        for (int i = 0; i < CCD_RATE_THREADS / 32; i++) s += wsum[tid][i];
+        part[(size_t)CCD_SWEEP_MAX_OFFSETS * blockIdx.x + tid] = s;
+    }
+    if (tid < 128 && hist[tid]) atomicAdd(J.hist + 128 * t.grid + tid, (unsigned long long)hist[tid]);
+}
+
 // Spatial rate map (training/test.py:217-235 in a canonical order): per pixel, acc = 0, then for every grid,
 // finest first, acc += bits[nearest(y), nearest(x)] / ((H*W) / (h*w)), all in fp32.  blockIdx.y = job.
 __global__ void k_rate_spatial(const RateSpatialDev *__restrict__ jobs) {
@@ -1624,6 +1690,13 @@ int ccd_rate_launch(const RateTile *d_tiles, int n_tiles, const RateJobDev *d_jo
     cudaError_t e = cudaFuncSetAttribute(k_latent_rate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     k_latent_rate<<<n_tiles, CCD_RATE_THREADS, smem, st>>>(d_tiles, d_jobs, d_cdf, d_scale, d_part);
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
+
+int ccd_rate_sweep_launch(const RateTile *d_tiles, int n_tiles, const SweepJobDev *d_jobs, const uint32_t *d_cdf,
+                          const float *d_scale, double *d_part, cudaStream_t st) {
+    k_rate_sweep<<<n_tiles, CCD_RATE_THREADS, 0, st>>>(d_tiles, d_jobs, d_cdf, d_scale, d_part);
     g_ccd_launches++;
     return (int)cudaGetLastError();
 }

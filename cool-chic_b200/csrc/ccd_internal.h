@@ -146,6 +146,23 @@ int ccd_rate_launch(const RateTile *d_tiles, int n_tiles, const RateJobDev *d_jo
                     const float *d_scale, double *d_part, cudaStream_t st);
 int ccd_rate_spatial_launch(const RateSpatialDev *d_jobs, int n_jobs, int64_t max_pixels, cudaStream_t st);
 
+// Scale-calibration sweep (k_rate_sweep, DESIGN §4.10): the RateTile list of the rate pass (job = sweep job), one CTA
+// per tile.  Each thread holds up to CCD_SWEEP_SPT symbols of its tile; one f64 partial per (tile, offset) in
+// part[CCD_SWEEP_MAX_OFFSETS * tile + k]; the grid histograms are integer atomics on counters the host zeroes.
+#define CCD_SWEEP_SPT ((CCD_RATE_TH * CCD_RATE_TW + CCD_RATE_THREADS - 1) / CCD_RATE_THREADS)
+struct SweepJobDev {
+    const int8_t *lat;            // decoded latents, decode order
+    const uint32_t *mu_sc;        // mu_idx | sc_idx << 16, same layout
+    unsigned long long *hist;     // [n_grids][128], decode-order grids
+    unsigned long long *bad;      // smallest decode-order index of a bad symbol (~0 if none)
+    int32_t n_off;
+    int32_t off[CCD_SWEEP_MAX_OFFSETS];
+    int32_t h[CCD_MAX_GRIDS], w[CCD_MAX_GRIDS];  // decode order
+    int64_t lat_off[CCD_MAX_GRIDS];
+};
+int ccd_rate_sweep_launch(const RateTile *d_tiles, int n_tiles, const SweepJobDev *d_jobs, const uint32_t *d_cdf,
+                          const float *d_scale, double *d_part, cudaStream_t st);
+
 // --------------------------------------------------------------------------------------
 // Synthesis stage (ccd_synth.cu)
 // --------------------------------------------------------------------------------------

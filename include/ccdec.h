@@ -224,6 +224,49 @@ typedef struct CcdRateJob {
  * like ccd_decode_many.  Returns CCD_OK or the first failing job's status. */
 int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_stream);
 
+/* Entropy-model analysis (DESIGN §4.10): the rate of ccd_latent_rate under the coder's model with some ARM inputs read
+ * as 0, the model's own convention for a neighbour outside the grid and for a grid without IFCE input.  The first
+ * operation on an ARM or IFCE input is linear, so an input read as 0 is its row of the first layer's (and the
+ * stabiliser's) fixed-point weights set to 0; the library edits the weights on the host, and the edited model takes the
+ * fast or the generic kernel by the decoder's own rule.
+ *   zero_ctx:        bit t: spatial input t (the neighbour of priority t, core/arm.py:496-562) read as 0;
+ *   zero_ifce_out:   bit c: IFCE feature c (ARM input n_ctx + c) read as 0;
+ *   zero_ifce_grids: bit g (g = 0: the finest grid): latent grid g read as 0 wherever it is an IFCE input (channel c of
+ *                    grid h reads grid h + 1 + c).
+ * edits[i] applies to jobs[i]; edits == NULL edits nothing.  An all-zero edit gives exactly ccd_latent_rate's results.
+ * CCD_ERR_ARG, before any launch: a zero_ctx bit >= n_ctx, a zero_ifce_out bit >= n_ifce_out, any IFCE bit in a model
+ * without IFCE (flag_ifce 0), a zero_ifce_grids bit >= n_grids. */
+typedef struct CcdModelEdit {
+    uint64_t zero_ctx;
+    uint32_t zero_ifce_out;
+    uint32_t zero_ifce_grids;
+} CcdModelEdit;
+int ccd_latent_rate_edited(CcdContext *ctx, CcdRateJob *jobs, const CcdModelEdit *edits, int n_jobs, void *cuda_stream);
+
+/* Scale-calibration sweep and static histogram of decoded latents (DESIGN §4.10), from the (mu_idx, sc_idx) the coder
+ * used (d_mu_sc, as ccd_latent_rate writes it).  For each offset k < n_offsets, bits[g][k] (out) is the f64 sum over
+ * grid g (0 = finest) of 24 - log2(freq) with sc_idx' = clamp(sc_idx + sc_offset[k], 0, 2560) and mu_idx unchanged:
+ * the scale times exp(sc_offset[k] / 256).  The interval is ccd_latent_rate's (the table window, else the exact f64
+ * model).  hist[g][s + 64] (out): the count of symbol s in grid g.  Sums are f64 partials per tile and offset added in
+ * tile order, the histograms integer counts: the same on every run.  CCD_ERR_ARG before any launch: n_offsets outside
+ * 1 .. 32, an offset outside [-2560, 2560]; after the launch, with bad_index = the smallest decode-order index of such a
+ * symbol (else -1): a latent outside [-64, 63], a mu_idx above 32767 or an sc_idx above 2560. */
+#define CCD_SWEEP_MAX_OFFSETS 32
+typedef struct CcdSweepJob {
+    const CcdCoolChicDesc *desc;
+    const int8_t *d_latents;
+    const uint32_t *d_mu_sc;
+    int32_t n_offsets;
+    int32_t sc_offset[CCD_SWEEP_MAX_OFFSETS];
+    double bits[CCD_MAX_GRIDS][CCD_SWEEP_MAX_OFFSETS];
+    uint64_t hist[CCD_MAX_GRIDS][128];
+    int64_t bad_index;
+    int32_t status;
+} CcdSweepJob;
+
+/* All jobs in ONE kernel launch; one copy each way; synchronous.  Returns CCD_OK or the first failing job's status. */
+int ccd_rate_sweep(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, void *cuda_stream);
+
 /* Tail of decode_frame for every frame type (bitstream/decode.py:191-206 with
  * io/format/yuv.py:239-256,274-300): round to the 2^b-1 grid -> (444->420 2x2 average of
  * U,V) -> clamp [0,1] -> round again.  data_type: 0 rgb, 1 yuv420, 2 yuv444.

@@ -5,7 +5,8 @@
     nearest x4 at an odd size, P and B frames with sinc-10 / sinc-14 below the filter length), written by
     coolchic_b200.synth with the oracle as range encoder and DECODED BY THE UNMODIFIED REFERENCE (through
     oracle/refshim): the reference's integer samples;
-  * tests/golden/<name>_raw.npz for those streams and for the older img_* / gop* fixtures: the reference's raw fp32
+  * tests/golden/<name>_raw.npz for those streams and for the older img_* / gop* fixtures (gen_golden_bitdepths.py
+    writes its own): the reference's raw fp32
     output of every Cool-chic, in coding order (key c<i>), as encode_decode_coolchic returned it.
 
 Needs a reference checkout (COOLCHIC_REFERENCE=<path>).  Output is byte for byte reproducible.  TEST INFRASTRUCTURE

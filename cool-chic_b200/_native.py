@@ -30,7 +30,7 @@ EXPORTS = [
     "ccd_encode_latents", "ccd_synthesize_many", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
     "ccd_latent_rate", "ccd_latent_rate_edited", "ccd_rate_sweep", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats", "ccd_inter_analysis",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
-    "ccd_debug_entropy_plan", "ccd_debug_cdf_table",
+    "ccd_debug_entropy_plan", "ccd_debug_cdf_table", "ccd_debug_detmath", "ccd_debug_sinc_coeffs", "ccd_debug_cr_noise",
 ]
 
 
@@ -278,6 +278,12 @@ def load_library():
         L.ccd_debug_laplace_domain.argtypes = [vp, ci, ci, vp, vp]
         L.ccd_debug_cdf_table.restype = ci
         L.ccd_debug_cdf_table.argtypes = [vp, ci, ci, vp]
+        L.ccd_debug_detmath.restype = ci
+        L.ccd_debug_detmath.argtypes = [vp, ci, vp, vp, ctypes.c_size_t]
+        L.ccd_debug_sinc_coeffs.restype = ci
+        L.ccd_debug_sinc_coeffs.argtypes = [vp, ci, vp, vp, ctypes.c_size_t]
+        L.ccd_debug_cr_noise.restype = ci
+        L.ccd_debug_cr_noise.argtypes = [vp, ctypes.c_uint64, ctypes.c_size_t, vp]
         L.ccd_debug_last_status.restype = ci
         L.ccd_debug_last_status.argtypes = [vp, vp]
         L.ccd_debug_launch_count.restype = ctypes.c_uint64
@@ -873,6 +879,28 @@ class Context:
         """The context's cumulative table for the scales [sc_lo, sc_hi): uint32 [sc_hi - sc_lo, 256, 32]."""
         out = np.zeros((sc_hi - sc_lo, 256, 32), dtype=np.uint32)
         _check(self._lib.ccd_debug_cdf_table(self._h, sc_lo, sc_hi, out.ctypes.data_as(ctypes.c_void_p)))
+        return out
+
+    def detmath(self, fn: str, x: np.ndarray) -> np.ndarray:
+        """The device's canonical sin / cos / log (ccd_detmath.h) of every element of x: float64 like x."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        y = np.empty_like(x)
+        _check(self._lib.ccd_debug_detmath(self._h, {"sin": 0, "cos": 1, "log": 2}[fn],
+                                           x.ctypes.data_as(ctypes.c_void_p), y.ctypes.data_as(ctypes.c_void_p), x.size))
+        return y
+
+    def sinc_coeffs(self, taps: int, s: np.ndarray) -> np.ndarray:
+        """The taps the sinc warp forms at fractional offsets s: float32 [len(s), taps]."""
+        s = np.ascontiguousarray(s, dtype=np.float32)
+        c = np.empty((s.size, taps), dtype=np.float32)
+        _check(self._lib.ccd_debug_sinc_coeffs(self._h, taps, s.ctypes.data_as(ctypes.c_void_p),
+                                               c.ctypes.data_as(ctypes.c_void_p), s.size))
+        return c
+
+    def cr_noise(self, first: int, n: int) -> np.ndarray:
+        """Samples [first, first + n) of the device's common-randomness generator: float32 [n]."""
+        out = np.empty(n, dtype=np.float32)
+        _check(self._lib.ccd_debug_cr_noise(self._h, first, n, out.ctypes.data_as(ctypes.c_void_p)))
         return out
 
 

@@ -2219,6 +2219,42 @@ int ccd_debug_cdf_table(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *out) {
     });
 }
 
+int ccd_debug_detmath(CcdContext *ctx, int fn, const double *x, double *y, size_t n) {
+    return guarded(ctx, nullptr, [&](cudaStream_t st) -> int {
+        if (fn < 0 || fn > 2 || !x || !y || n == 0) return fail(CCD_ERR_ARG, "bad argument");
+        if (int rc = ensure_dev(ctx->scratch, n * 16)) return rc;
+        double *dx = reinterpret_cast<double *>(ctx->scratch.p), *dy = dx + n;
+        CUDA_TRY(cudaMemcpy(dx, x, n * 8, cudaMemcpyHostToDevice));
+        if (ccd_detmath(fn, dx, dy, n, st)) return fail(CCD_ERR_CUDA, "launch failed");
+        CUDA_TRY(cudaMemcpy(y, dy, n * 8, cudaMemcpyDeviceToHost));
+        return CCD_OK;
+    });
+}
+
+int ccd_debug_sinc_coeffs(CcdContext *ctx, int taps, const float *s, float *c, size_t n) {
+    return guarded(ctx, nullptr, [&](cudaStream_t st) -> int {
+        if (!s || !c || n == 0) return fail(CCD_ERR_ARG, "bad argument");
+        if (taps < 6 || taps > 14 || (taps & 1)) return fail(CCD_ERR_ARG, "no sinc warp has %d taps", taps);
+        if (int rc = ensure_dev(ctx->scratch, n * 4 * (1 + (size_t)taps))) return rc;
+        float *ds = reinterpret_cast<float *>(ctx->scratch.p), *dc = ds + n;
+        CUDA_TRY(cudaMemcpy(ds, s, n * 4, cudaMemcpyHostToDevice));
+        if (ccd_sinc_coeffs(taps, ds, dc, n, st)) return fail(CCD_ERR_CUDA, "launch failed");
+        CUDA_TRY(cudaMemcpy(c, dc, n * 4 * (size_t)taps, cudaMemcpyDeviceToHost));
+        return CCD_OK;
+    });
+}
+
+int ccd_debug_cr_noise(CcdContext *ctx, uint64_t first, size_t n, float *out) {
+    return guarded(ctx, nullptr, [&](cudaStream_t st) -> int {
+        if (!out || n == 0 || n > (1ull << 40) || first > (1ull << 62)) return fail(CCD_ERR_ARG, "bad argument");
+        if (int rc = ensure_dev(ctx->scratch, n * 4)) return rc;
+        float *d = reinterpret_cast<float *>(ctx->scratch.p);
+        if (ccd_cr_noise(d, first, n, st)) return fail(CCD_ERR_CUDA, "launch failed");
+        CUDA_TRY(cudaMemcpy(out, d, n * 4, cudaMemcpyDeviceToHost));
+        return CCD_OK;
+    });
+}
+
 uint64_t ccd_debug_launch_count(void) { return g_ccd_launches; }
 
 int ccd_debug_entropy_plan(const CcdCoolChicDesc *desc, const int64_t *nn_ints, int64_t out[3]) {

@@ -1,6 +1,6 @@
 // ccd_detmath.h -- device flavour (sm_90a) of the canonical elementary functions.
 // The oracle holds its own copy of the same operation sequence (oracle/detmath.h, plain C);
-// tests/test_gpu_decode.py::test_detmath_device_equals_oracle compares the two bit for bit.
+// tests/test_detmath.py::test_detmath_device_equals_oracle compares the two bit for bit.
 #pragma once
 #include <cuda_runtime.h>
 #define CCDM_FN static __device__ __forceinline__
@@ -16,9 +16,14 @@
  * The reference evaluates these with its platform's libm (glibc / SLEEF), which no other platform
  * reproduces bit for bit; the CPU oracle and the CUDA kernels therefore share THIS algorithm, built
  * only from IEEE-754 operations that are exactly specified (+, *, fma, /, rint, bit moves), in a fixed
- * order: same input -> same 64 bits on x86-64 and on sm_90a.  Accuracy: < 2 ulp (double), i.e. the
- * value rounded to fp32 equals the correctly rounded one except in ~1e-8 of the arguments.
- *   sin / cos: Cody-Waite reduction by pi/2 (two terms, |x| < 64), Taylor kernels on [-pi/4, pi/4]
+ * order: same input -> same 64 bits on x86-64 and on sm_90a.  Accuracy, in ulp of the exact double, over every
+ * argument of the decoder's domain (tools/detmath_scan.c; DESIGN.md, "Canonical elementary functions"):
+ *   sin <= 1.46 ulp at every float 0 < |x| <= fl(7 pi)       (the sinc taps, N <= 14)
+ *   cos <= 1.41 ulp at every float |x| <= fl(pi / 2)         (the sinc window)
+ *   cos <= 1.45 ulp, log <= 2.68 ulp at the Box-Muller arguments fl(2 pi_ref) s / m and s / m, s in [1, m - 1]
+ * No bound holds outside that domain: near k pi / 2 the two-term reduction loses relative accuracy where the
+ * result is tiny (cos is 451 ulp off at the double nearest 29 pi / 2).
+ *   sin / cos: Cody-Waite reduction by pi/2 (two terms), Taylor kernels on [-pi/4, pi/4]
  *   log      : x = m 2^e, m in [sqrt(1/2), sqrt(2)); log m = 2 atanh((m-1)/(m+1)), series to s^23   */
 CCDM_FN double ccdm_sin_k(double r) {
     const double z = CCDM_MUL(r, r);
@@ -44,7 +49,7 @@ CCDM_FN double ccdm_cos_k(double r) {
     p = CCDM_FMA(p, z, -0x1.0000000000000p-1);
     return CCDM_FMA(z, p, 1.0);
 }
-/* x -> (r, quadrant): x = j pi/2 + r, |r| <= pi/4 (+ rounding), valid for |x| < 64 */
+/* x -> (r, quadrant): x = j pi/2 + r, |r| <= pi/4 (+ rounding) */
 CCDM_FN double ccdm_reduce(double x, int *q) {
     const double j = CCDM_RINT(CCDM_MUL(x, 0x1.45f306dc9c883p-1));
     double r = CCDM_FMA(-j, 0x1.921fb54442d18p+0, x);

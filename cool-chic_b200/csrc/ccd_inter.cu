@@ -452,6 +452,17 @@ __global__ void __launch_bounds__(128)
     if (t < 6) o.part[6 * ((size_t)blockIdx.y * gridDim.x + blockIdx.x) + t] = red[t][0];
 }
 
+// The taps sinc_coeffs<N> gives the warp, one offset per thread (ccd_debug_sinc_coeffs): c[N i + k]
+template <int N>
+__global__ void k_sinc_coeffs(const float *__restrict__ s, float *__restrict__ c, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float t[N];
+    sinc_coeffs<N>(s[i], t);
+#pragma unroll
+    for (int k = 0; k < N; k++) c[(size_t)N * i + k] = t[k];
+}
+
 // One launch of a P/B kernel: launch(std::integral_constant<int, N>, grid, block, ref0, ref1) for the warp filter
 // size N of a, on one thread per pixel in CTAs of 128.  Returns -1 for a size no kernel is built for.
 template <class F>
@@ -502,4 +513,18 @@ int ccd_inter_launch(const InterLaunch &a, cudaStream_t st) {
                                                                     a.is_b, a.gf[0], a.gf[1], a.gf[2], a.gf[3], a.M,
                                                                     a.out_420, a.out[0], a.out[1], a.out[2]);
     });
+}
+
+int ccd_sinc_coeffs(int taps, const float *d_s, float *d_c, size_t n, cudaStream_t st) {
+    const unsigned blocks = (unsigned)((n + 127) / 128);
+    switch (taps) {
+        case 6: k_sinc_coeffs<6><<<blocks, 128, 0, st>>>(d_s, d_c, n); break;
+        case 8: k_sinc_coeffs<8><<<blocks, 128, 0, st>>>(d_s, d_c, n); break;
+        case 10: k_sinc_coeffs<10><<<blocks, 128, 0, st>>>(d_s, d_c, n); break;
+        case 12: k_sinc_coeffs<12><<<blocks, 128, 0, st>>>(d_s, d_c, n); break;
+        case 14: k_sinc_coeffs<14><<<blocks, 128, 0, st>>>(d_s, d_c, n); break;
+        default: return -1;
+    }
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
 }

@@ -225,6 +225,10 @@ int ccd_resize_torch(const float *d_in, int c, int h, int w, float *d_out, int H
                      cudaStream_t st);
 // samples [first, first+n) of the common-randomness generator (noise.py)
 int ccd_cr_noise(float *d_out, size_t first, size_t n, cudaStream_t st);
+// canonical sin / cos / log (fn 0 / 1 / 2, ccd_detmath.h) of n doubles
+int ccd_detmath(int fn, const double *d_x, double *d_y, size_t n, cudaStream_t st);
+// the taps of the windowed-sinc warp (N = taps in {6, 8, ..., 14}) at n offsets: d_c[N i + k]; -1 for another N
+int ccd_sinc_coeffs(int taps, const float *d_s, float *d_c, size_t n, cudaStream_t st);
 int ccd_finish(const float *d_in, int h, int w, int bitdepth, int data_type, float *a, float *b, float *c,
                cudaStream_t st);
 // The sample operations of decode_frame's frame tail (bitstream/decode.py:191-206), for k_finish_*, the epilogue of

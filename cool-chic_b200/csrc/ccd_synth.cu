@@ -1124,6 +1124,14 @@ __global__ void k_cr_noise(float *__restrict__ out, size_t first, size_t n) {
     out[i] = (float)__dmul_rn(__dsqrt_rn(__dmul_rn(-2.0, ccdm_log(u1))), ccdm_cos(__dmul_rn(2 * 3.14159265359, u2)));
 }
 
+// Debug image of the canonical elementary functions (ccd_debug_detmath): y[i] = sin / cos / log (fn 0 / 1 / 2) of x[i]
+__global__ void k_detmath(int fn, const double *__restrict__ x, double *__restrict__ y, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double v = x[i];
+    y[i] = fn == 0 ? ccdm_sin(v) : (fn == 1 ? ccdm_cos(v) : ccdm_log(v));
+}
+
 __global__ void k_finish_444(const float *__restrict__ in, size_t n, float M, float *__restrict__ out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = quant(clamp01(quant(in[i], M)), M);
@@ -1421,6 +1429,12 @@ int ccd_resize_torch(const float *d_in, int c, int h, int w, float *d_out, int H
 
 int ccd_cr_noise(float *d_out, size_t first, size_t n, cudaStream_t st) {
     k_cr_noise<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_out, first, n);
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
+
+int ccd_detmath(int fn, const double *d_x, double *d_y, size_t n, cudaStream_t st) {
+    k_detmath<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(fn, d_x, d_y, n);
     g_ccd_launches++;
     return (int)cudaGetLastError();
 }

@@ -417,6 +417,20 @@ int ccd_debug_laplace_domain(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *ou
  * symbol whose mu_idx has (mu_idx + 128) & 255 = f). */
 int ccd_debug_cdf_table(CcdContext *ctx, int sc_lo, int sc_hi, uint32_t *out);
 
+/* Device-side evaluation of the canonical elementary functions (csrc/ccd_detmath.h), for testing them
+ * against the host's copy bit for bit: y[i] = sin / cos / log (fn 0 / 1 / 2) of x[i], host arrays of n
+ * doubles.  One launch; synchronous. */
+int ccd_debug_detmath(CcdContext *ctx, int fn, const double *x, double *y, size_t n);
+
+/* The taps of the windowed-sinc warp as the P/B kernels form them (warp.py:226-268), for taps = N in
+ * {6, 8, 10, 12, 14}: c[N i + k] = tap k at the fractional offset s[i], host arrays.  Any other N is
+ * CCD_ERR_ARG.  One launch; synchronous. */
+int ccd_debug_sinc_coeffs(CcdContext *ctx, int taps, const float *s, float *c, size_t n);
+
+/* Samples [first, first + n) of the common-randomness generator (noise.py:18-34) as the synthesis draws
+ * them, before any resize, into the host array out.  One launch; synchronous. */
+int ccd_debug_cr_noise(CcdContext *ctx, uint64_t first, size_t n, float *out);
+
 /* Number of CUDA kernels this library has launched since it was loaded. */
 uint64_t ccd_debug_launch_count(void);
 

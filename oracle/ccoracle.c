@@ -971,20 +971,41 @@ int cco_resize(const float *in, int c, int h, int w, float *out, int H, int W, i
 
 /* ---- common randomness (--tune=wasserstein): component/core/noise.py:18-55 ------------------------
  * Park-Miller LCG (a = 7^5, m = 2^31 - 1, seed 18101995), two draws per sample, Box-Muller in
- * double precision with pi = 3.14159265359 (log / cos = the canonical ones of detmath.h, within 2 ulp
- * of the libm the reference's math.log / math.cos call), rounded to fp32; one grid per latent resolution
- * (core/coolchic.py:187-191: ceil(img / 2^i)), finest first; fixed_upsampling(bicubic)
- * (upsampling.py:556-595) and a final bicubic interpolate to the image size
+ * double precision with pi = 3.14159265359 (log / cos = the canonical ones of detmath.h), rounded to fp32.
+ * The fp32 samples equal those of the libm calls the reference makes (math.log / math.cos / math.sqrt)
+ * except where the float64 value lies within a few float64 ulp of an fp32 rounding tie: none of the
+ * first 12 000 000 samples, one sample (k = 302 383 943) over the whole period (tests/test_detmath.py).
+ * One grid per latent resolution (core/coolchic.py:187-191: ceil(img / 2^i)), finest first;
+ * fixed_upsampling(bicubic) (upsampling.py:556-595) and a final bicubic interpolate to the image size
  * (bitstream/component/coolchic.py:180-183).  out: [n][H][W], n = latent_res_hi - latent_res_lo + 1. */
+
+/* Samples [first, first + n) of the generator: sample k draws seeds 2k + 1 and 2k + 2 of the sequence */
+int cco_noise_samples(uint64_t first, size_t n, float *out) {
+    const uint64_t a = 16807ULL, m = 2147483647ULL;
+    const double pi = 3.14159265359;
+    if (!out || n > (1ULL << 62) || first > (1ULL << 62) - n) return CCO_ERR_ARG;
+    uint64_t seed = 18101995ULL, b = a;  /* seed_{2 first} = a^(2 first) seed_0 mod m */
+    for (uint64_t e = 2 * first; e; e >>= 1) {
+        if (e & 1) seed = (seed * b) % m;
+        b = (b * b) % m;
+    }
+    for (size_t k = 0; k < n; k++) {
+        seed = (a * seed) % m;
+        double u1 = (double)seed / (double)m;
+        seed = (a * seed) % m;
+        double u2 = (double)seed / (double)m;
+        out[k] = (float)(sqrt(-2 * ccdm_log(u1)) * ccdm_cos(2 * pi * u2));
+    }
+    return CCO_OK;
+}
+
 int cco_cr_noise(const CcoDesc *d, float *out) {
     const int n = d->latent_res_hi - d->latent_res_lo + 1;
     if (n < 1 || n > CCO_MAX_GRIDS) return CCO_ERR_ARG;
     const int H = d->img_h, W = d->img_w;
     int gh[CCO_MAX_GRIDS], gw[CCO_MAX_GRIDS];
     float *g[CCO_MAX_GRIDS];
-    uint64_t seed = 18101995ULL;
-    const uint64_t a = 16807ULL, m = 2147483647ULL;
-    const double pi = 3.14159265359;
+    uint64_t first = 0;
     for (int i = 0; i < n; i++) g[i] = NULL;
     int rc = CCO_OK;
     for (int i = 0; i < n && rc == CCO_OK; i++) {
@@ -994,13 +1015,8 @@ int cco_cr_noise(const CcoDesc *d, float *out) {
         size_t cnt = (size_t)gh[i] * gw[i];
         g[i] = (float *)malloc(cnt * 4 + 16);
         if (!g[i]) { rc = CCO_ERR_NOMEM; break; }
-        for (size_t k = 0; k < cnt; k++) {
-            seed = (a * seed) % m;
-            double u1 = (double)seed / (double)m;
-            seed = (a * seed) % m;
-            double u2 = (double)seed / (double)m;
-            g[i][k] = (float)(sqrt(-2 * ccdm_log(u1)) * ccdm_cos(2 * pi * u2));
-        }
+        rc = cco_noise_samples(first, cnt, g[i]);
+        first += cnt;
     }
     /* cascade, coarsest first; cur holds cc planes of size ch x cw */
     float *cur = NULL, *nxt = NULL;
@@ -1222,8 +1238,9 @@ int cco_finish_frame(const float *in, int h, int w, int bitdepth, int data_type,
  * integer part by clamped gathers, fractional part by N taps cos(pi(s-k)/N) * sinc(s-k),
  * first along x (flow channel 0) for each of the N rows, then along y (flow channel 1).
  * Coefficients are evaluated in double precision with the canonical sin / cos of detmath.h (exactly
- * reproducible on the GPU) and rounded to fp32 (the reference does it in fp32 with its platform's libm:
- * <= 1 ulp apart); products and sums are fp32, sequential, unfused.            */
+ * reproducible on the GPU) and rounded to fp32; the reference does it in fp32 with its platform's libm.
+ * The two are at most 3 fp32 ulp apart for N = 6 ... 14, more than 1 ulp at 12 % (N = 6) to 32 % (N = 14) of
+ * the offsets (tests/test_detmath.py); products and sums are fp32, sequential, unfused.            */
 static void sinc_coeffs(float s, int n, float *c) {
     const float PIf = 3.14159265358979323846f;
     int lt = -(n / 2) + 1;
@@ -1234,6 +1251,19 @@ static void sinc_coeffs(float s, int n, float *c) {
         double sc = (arg == 0.0f) ? 1.0 : ccdm_sin((double)pa) / (double)pa;
         c[k] = (float)win * (float)sc;
     }
+}
+
+/* Debug images of the canonical functions, for comparison with the device (tests/test_detmath.py):
+ * y[i] = sin / cos / log (fn 0 / 1 / 2) of x[i]; c[N i + k] = tap k of the N-tap windowed sinc at offset s[i]. */
+int cco_detmath(int fn, const double *x, double *y, size_t n) {
+    if (fn < 0 || fn > 2 || !x || !y) return CCO_ERR_ARG;
+    for (size_t i = 0; i < n; i++) y[i] = fn == 0 ? ccdm_sin(x[i]) : (fn == 1 ? ccdm_cos(x[i]) : ccdm_log(x[i]));
+    return CCO_OK;
+}
+int cco_sinc_coeffs(int taps, const float *s, float *c, size_t n) {
+    if (taps < 6 || taps > 14 || (taps & 1) || !s || !c) return CCO_ERR_ARG;
+    for (size_t i = 0; i < n; i++) sinc_coeffs(s[i], taps, c + (size_t)taps * i);
+    return CCO_OK;
 }
 
 static void warp_sinc(const float *ref, int h, int w, int gx, int gy, const float *flow, int n, float *out) {

@@ -113,6 +113,12 @@ int cco_resize(const float *in, int c, int h, int w, float *out, int H, int W, i
                int scale_factor_2);
 /* common-randomness synthesis input (noise.py + fixed_upsampling bicubic): out [n][img_h][img_w] */
 int cco_cr_noise(const CcoDesc *d, float *out);
+/* samples [first, first + n) of the common-randomness generator (noise.py:18-34), before any resize */
+int cco_noise_samples(uint64_t first, size_t n, float *out);
+/* the canonical functions of detmath.h: y[i] = sin / cos / log (fn 0 / 1 / 2) of x[i] */
+int cco_detmath(int fn, const double *x, double *y, size_t n);
+/* taps of the windowed sinc warp (warp.py:226-268), N = taps in {6, 8, ..., 14}: c[N i + k] for offset s[i] */
+int cco_sinc_coeffs(int taps, const float *s, float *c, size_t n);
 
 /* decode_frame tail for I frames (bitstream/decode.py:191-206): round -> (444->420 avg pool)
  * -> clamp -> round.  data_type 0 rgb, 1 yuv420, 2 yuv444.  in: [3][H][W]; out planes:

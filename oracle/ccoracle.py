@@ -14,7 +14,7 @@ _SO = os.path.join(_HERE, "_build", "libccoracle.so")
 
 
 def build(force: bool = False) -> str:
-    src = [os.path.join(_HERE, f) for f in ("ccoracle.c", "ccoracle.h", "scale_table.inc")]
+    src = [os.path.join(_HERE, f) for f in ("ccoracle.c", "ccoracle.h", "detmath.h", "scale_table.inc")]
     stale = (not os.path.exists(_SO)) or any(os.path.getmtime(s) > os.path.getmtime(_SO) for s in src)
     if force or stale:
         subprocess.check_call(["make", "-C", _HERE, "-s"] + (["-B"] if force else []))
@@ -60,6 +60,12 @@ def lib():
         L.cco_resize.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp] + [ctypes.c_int] * 4
         L.cco_cr_noise.restype = ctypes.c_int
         L.cco_cr_noise.argtypes = [vp, vp]
+        L.cco_noise_samples.restype = ctypes.c_int
+        L.cco_noise_samples.argtypes = [ctypes.c_uint64, sz, vp]
+        L.cco_detmath.restype = ctypes.c_int
+        L.cco_detmath.argtypes = [ctypes.c_int, vp, vp, sz]
+        L.cco_sinc_coeffs.restype = ctypes.c_int
+        L.cco_sinc_coeffs.argtypes = [ctypes.c_int, vp, vp, sz]
         L.cco_laplace_left.restype = ctypes.c_uint32
         L.cco_laplace_left.argtypes = [ctypes.c_int, ctypes.c_float, ctypes.c_float]
         _lib = L
@@ -226,3 +232,29 @@ def cr_noise(desc) -> np.ndarray:
     out = np.zeros((n, desc.img_h, desc.img_w), dtype=np.float32)
     _chk(lib().cco_cr_noise(ctypes.byref(desc), _p(out)), "cr_noise")
     return out
+
+
+DETMATH_FN = {"sin": 0, "cos": 1, "log": 2}
+
+
+def noise_samples(first: int, n: int) -> np.ndarray:
+    """Samples [first, first + n) of the common-randomness generator (noise.py:18-34): float32 [n]."""
+    out = np.zeros(n, dtype=np.float32)
+    _chk(lib().cco_noise_samples(first, n, _p(out)), "noise_samples")
+    return out
+
+
+def detmath(fn: str, x: np.ndarray) -> np.ndarray:
+    """The canonical sin / cos / log of detmath.h, element by element: float64 like x."""
+    x = np.ascontiguousarray(x, dtype=np.float64)
+    y = np.empty_like(x)
+    _chk(lib().cco_detmath(DETMATH_FN[fn], _p(x), _p(y), x.size), "detmath")
+    return y
+
+
+def sinc_coeffs(taps: int, s: np.ndarray) -> np.ndarray:
+    """Taps of the windowed-sinc warp at fractional offsets s: float32 [len(s), taps]."""
+    s = np.ascontiguousarray(s, dtype=np.float32)
+    c = np.empty((s.size, taps), dtype=np.float32)
+    _chk(lib().cco_sinc_coeffs(taps, _p(s), _p(c), s.size), "sinc_coeffs")
+    return c

@@ -275,22 +275,26 @@ bool ifce_bound(const ArmInts &a, i128 *bound) {
     return true;
 }
 
-// Can the ARM run with int32 operands (weights, activations) and int64 accumulators?
-bool arm_fits_int32(const ArmInts &a, int n_ctx, i128 ifce_feat_bound) {
+// Can the fast path evaluate the ARM in f64 (DMMA) and get the int64 result bit for bit?  Yes if every weight, bias
+// and input, every product and every partial sum of every layer is an integer below 2^53 in magnitude, whatever the
+// summation order: the worst case |B| + sum |W| |X| over the actual weights, with X the worst-case |input| of the
+// layer.  The last layer's and the stabiliser's products share one sum per output (the per-lane partial sums).
+bool arm_fits_f64(const ArmInts &a, int n_ctx, i128 ifce_feat_bound) {
+    const i128 lim = (i128)1 << 53;
     std::vector<i128> X((size_t)a.dim);
     for (int i = 0; i < a.dim; i++) X[i] = (i < n_ctx) ? ((i128)64 << 16) : (ifce_feat_bound << 16);
     for (int i = 0; i < a.dim; i++)
-        if (X[i] > INT32_MAX) return false;
+        if (X[i] >= lim) return false;
     auto layer_ok = [&](const std::vector<int64_t> &W, const std::vector<int64_t> &B, int out,
                         const std::vector<i128> &Xin, std::vector<i128> *acc) {
         acc->assign((size_t)out, 0);
         for (int o = 0; o < out; o++) {
             i128 s = iabs128(B[o]);
             for (int i = 0; i < a.dim; i++) {
-                if (iabs128(W[(size_t)i * out + o]) > INT32_MAX) return false;
+                if (iabs128(W[(size_t)i * out + o]) >= lim) return false;
                 s += iabs128(W[(size_t)i * out + o]) * Xin[i];
             }
-            if (s >= ((i128)1 << 61)) return false;
+            if (s >= lim) return false;
             (*acc)[o] = s;
         }
         return true;
@@ -299,12 +303,11 @@ bool arm_fits_int32(const ArmInts &a, int n_ctx, i128 ifce_feat_bound) {
     if (!layer_ok(a.Ws, a.Bs, a.n_out, X, &stab)) return false;
     for (int l = 0; l < a.n_hidden; l++) {
         if (!layer_ok(a.W[l], a.B[l], a.dim, X, &acc)) return false;
-        for (int o = 0; o < a.dim; o++) {
-            X[o] = acc[o] >> 16;
-            if (X[o] > INT32_MAX) return false;
-        }
+        for (int o = 0; o < a.dim; o++) X[o] = acc[o] >> 16;
     }
     if (!layer_ok(a.W[a.n_hidden], a.B[a.n_hidden], a.n_out, X, &acc)) return false;
+    for (int o = 0; o < a.n_out; o++)
+        if (acc[o] + stab[o] >= lim) return false;
     return true;
 }
 
@@ -313,6 +316,10 @@ void put_i32(std::vector<unsigned char> &b, int64_t v) {
     b.insert(b.end(), (unsigned char *)&t, (unsigned char *)&t + 4);
 }
 void put_i64(std::vector<unsigned char> &b, int64_t v) { b.insert(b.end(), (unsigned char *)&v, (unsigned char *)&v + 8); }
+void put_f64(std::vector<unsigned char> &b, int64_t v) {
+    const double t = (double)v;  // exact: arm_fits_f64 holds
+    b.insert(b.end(), (const unsigned char *)&t, (const unsigned char *)&t + 8);
+}
 void pad_to(std::vector<unsigned char> &b, size_t a) {
     while (b.size() % a) b.push_back(0);
 }
@@ -320,21 +327,27 @@ void pad_to(std::vector<unsigned char> &b, size_t a) {
 void pack_arm(const ArmInts &a, bool fast, std::vector<unsigned char> &b) {
     const int dim = a.dim;
     if (fast) {
-        const int opm = (dim + 3) / 4, opmp = opm <= 2 ? 2 : (opm <= 4 ? 4 : 8), dimp = 4 * opm;
+        // accumulator column 8j + c of a hidden layer holds unit 8j + 4 (c & 1) + (c >> 1): lane t of a quad receives
+        // units 4 (2j + e) + t, its A operands of k-step 2j + e in the next layer
+        const int ks = (dim + 3) / 4, nt = (ks + 1) / 2;
+        auto unit = [](int j, int c) { return 8 * j + 4 * (c & 1) + (c >> 1); };
         for (int l = 0; l < a.n_hidden; l++)
-            for (int i = 0; i < dim; i++)
-                for (int m = 0; m < 4; m++)
-                    for (int o = 0; o < opmp; o++) {
-                        const int out = m * opm + o;
-                        put_i32(b, (o < opm && out < dim) ? a.W[l][(size_t)i * dim + out] : 0);
+            for (int s = 0; s < ks; s++)
+                for (int j = 0; j < nt; j++)
+                    for (int lane = 0; lane < 32; lane++) {  // B fragment: row (input) lane & 3, column lane >> 2
+                        const int i = 4 * s + (lane & 3), o = unit(j, lane >> 2);
+                        put_f64(b, (i < dim && o < dim) ? a.W[l][(size_t)i * dim + o] : 0);
                     }
-        for (int i = 0; i < dimp; i++)
-            for (int o = 0; o < 2; o++) put_i32(b, i < dim ? a.W[a.n_hidden][(size_t)i * 2 + o] : 0);
-        for (int i = 0; i < dimp; i++)
-            for (int o = 0; o < 2; o++) put_i32(b, i < dim ? a.Ws[(size_t)i * 2 + o] : 0);
-        pad_to(b, 8);
         for (int l = 0; l < a.n_hidden; l++)
-            for (int o = 0; o < dimp; o++) put_i64(b, o < dim ? a.B[l][o] : 0);
+            for (int j = 0; j < nt; j++)
+                for (int c = 0; c < 8; c++) {  // C fragment of member t: columns 2t, 2t + 1
+                    const int o = unit(j, c);
+                    put_f64(b, o < dim ? a.B[l][o] : 0);
+                }
+        for (int i = 0; i < 4 * ks; i++) {
+            for (int o = 0; o < 2; o++) put_f64(b, i < dim ? a.W[a.n_hidden][(size_t)i * 2 + o] : 0);
+            for (int o = 0; o < 2; o++) put_f64(b, i < dim ? a.Ws[(size_t)i * 2 + o] : 0);
+        }
     } else {
         for (int l = 0; l < a.n_hidden; l++)
             for (size_t t = 0; t < (size_t)dim * dim; t++) put_i64(b, a.W[l][t]);
@@ -702,7 +715,7 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt, int gb = 0, int ge =
         if (d->grid_ifce_in[L.ifce_grid[j]] > CCD_IFCE_FAST_MAX) fast = false;
         feat_bound = std::max(feat_bound, bnd);
     }
-    if (fast) fast = arm_fits_int32(arm, d->n_ctx, feat_bound);
+    if (fast) fast = arm_fits_f64(arm, d->n_ctx, feat_bound);
     P.fast = fast;
     P.blob.clear();
     pack_arm(arm, fast, P.blob);

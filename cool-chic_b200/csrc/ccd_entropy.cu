@@ -9,10 +9,10 @@
 //
 //   * producer warps, a QUAD of lanes per symbol (8 symbols per warp): wait until the
 //     symbol's left neighbour is decoded (shared-memory progress counter), gather the causal
-//     neighbourhood from a shared-memory row ring, evaluate IFCE + ARM in integer arithmetic
-//     (IMAD.WIDE, int32 operands proven safe by the host, int64 accumulators, activations
-//     exchanged with quad shuffles), then fetch the symbol's 32-entry cumulative window from
-//     the device-resident quantised-Laplace table and publish it in a shared-memory ring.
+//     neighbourhood from a shared-memory row ring, evaluate the IFCE in integer arithmetic and the
+//     ARM on the FP64 tensor cores (integers below 2^53, exact by a bound the host proves), then
+//     fetch the symbol's 32-entry cumulative window from the device-resident quantised-Laplace
+//     table and publish it in a shared-memory ring.
 //   * 1 range-coder warp (speculative): its lanes enumerate the sequences of the next three
 //     symbols drawn from {M-1, M, M+1} (M = the most probable symbol), each runs the exact
 //     recursion on its own hypothesis, and the one lane that matches hands its state to the
@@ -217,32 +217,34 @@ __device__ __forceinline__ SmemLayout carve(unsigned char *base, int ring, int r
 
 // ---------------------------------------------------------------------------------------
 // ARM / IFCE evaluation (armint.py:180-203).
-// FAST path: int32 operands (proven safe by the host), int64 accumulators (IMAD.WIDE), and
-// each symbol is spread over a QUAD of lanes: member m owns activations [m*OPM, m*OPM+OPM).
-// One warp = 8 symbols.  This cuts the ARM latency ~8x w.r.t. one thread per symbol, which
-// is what bounds the short diagonals (the next diagonal cannot start before its ARM is done).
-template <int NCTX, int CF>
-struct QuadArm {
-    static constexpr int DIM = NCTX + CF;
-    static constexpr int OPM = (DIM + 3) / 4;                       // activations per member
-    static constexpr int OPMP = OPM <= 2 ? 2 : (OPM <= 4 ? 4 : 8);  // padded for vector LDS
-    static constexpr int DIMP = 4 * OPM;
-    static constexpr int CFP = (CF + 3) & ~3;
-    static_assert(OPM <= 8, "ARM too wide for the quad layout");
+// FAST path: the MLP runs on the FP64 tensor cores (DMMA m8n8k4) and each symbol is spread over a QUAD of lanes: a row
+// of the 8 x 4 A fragment is a symbol (8 per warp), lane t = lane & 3 of its quad supplies input 4s + t of k-step s,
+// so member t owns the inputs t, t + 4, t + 8, ...  The host proves that every product and every partial sum of every
+// layer is an integer below 2^53 in magnitude (arm_fits_f64): f64 then gives the int64 result bit for bit, in any
+// summation order.  It also permutes every hidden layer's units so that accumulator column 8j + 2t + e holds unit
+// 4(2j + e) + t: a lane's outputs are exactly its A operands of the next layer, and between layers there are no
+// shuffles, only ReLU and floor(a * 2^-16), both exact in f64.  The short diagonals wait on this evaluation (the next
+// diagonal cannot start before its ARM is done), and the finest grid's producers are issue-bound on it.
+__device__ __forceinline__ void dmma_m8n8k4(double (&d)[2], double a, double b) {
+    asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
+        : "+d"(d[0]), "+d"(d[1])
+        : "d"(a), "d"(b));
+}
 
-    static __device__ __forceinline__ void ld_w(const int32_t *p, int32_t (&w)[8]) {
-        if constexpr (OPMP == 2) {
-            int2 a = *reinterpret_cast<const int2 *>(p);
-            w[0] = a.x; w[1] = a.y;
-        } else if constexpr (OPMP == 4) {
-            int4 a = *reinterpret_cast<const int4 *>(p);
-            w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w;
-        } else {
-            int4 a = *reinterpret_cast<const int4 *>(p);
-            int4 b = *reinterpret_cast<const int4 *>(p + 4);
-            w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w;
-            w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-        }
+template <int NCTX, int CF>
+struct DmmaArm {
+    static constexpr int DIM = NCTX + CF;
+    static constexpr int KS = (DIM + 3) / 4;  // k-steps: inputs per member
+    static constexpr int NT = (KS + 1) / 2;   // n-tiles of 8 accumulator columns: two units per member each
+    static constexpr int CFP = (CF + 3) & ~3;
+    static_assert(KS <= 8, "ARM too wide for the quad layout");
+
+    // does member m own an IFCE feature (an input NCTX <= 4s + m < DIM)?
+    static __device__ __forceinline__ bool owns_feature(int m) {
+        bool r = false;
+#pragma unroll
+        for (int s = 0; s < KS; s++) r |= (4 * s + m >= NCTX && 4 * s + m < DIM);
+        return r;
     }
 
     // IFCE inputs of the pixel (y, x): the already decoded coarser grids at (y>>1 >> sh, x>>1 >> sh)
@@ -254,7 +256,7 @@ struct QuadArm {
         for (int c = 0; c < CCD_IFCE_FAST_MAX; c++) ifv[c] = 0;
         if constexpr (CF > 0) {
             const int n_in = g->ifce_in;
-            if (n_in > 0 && (m + 1) * OPM > NCTX) {
+            if (n_in > 0 && owns_feature(m)) {
                 const int yy = y >> 1, xx = x >> 1;
 #pragma unroll
                 for (int c = 0; c < CCD_IFCE_FAST_MAX; c++) {
@@ -267,110 +269,106 @@ struct QuadArm {
         }
     }
 
-    // returns (mu, log-scale) in 1/256 units, identical on the 4 lanes of the quad
+    // returns (mu, log-scale) in 1/256 units, identical on the 4 lanes of the quad; every lane of the warp takes part
     static __device__ __forceinline__ void run(const EntGrid *g, const unsigned char *arm_blob,
                                                const unsigned char *ifce_blob, const int (&ifv)[CCD_IFCE_FAST_MAX],
                                                uint32_t rows, uint32_t row_mask, int n_hidden, int y, int x,
                                                int m, long long &o0, long long &o1) {
         const int w = g->w;
-        int32_t x0[OPM];
+        const int lane = (int)(threadIdx.x & 31);
+        long long xi[KS];
         // ---- my share of the context: causal neighbours (latent.py:148-153) ...
 #pragma unroll
-        for (int o = 0; o < OPM; o++) {
-            const int i = m * OPM + o;
+        for (int s = 0; s < KS; s++) {
+            const int i = 4 * s + m;
             int v = 0;
             if (i < NCTX) {
                 const int yy = y + c_ctx_dy[i], xx = x + c_ctx_dx[i];
                 if (yy >= 0 && xx >= 0 && xx < w)
                     v = lds_s8(rows + ((((uint32_t)yy & row_mask) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))));
             }
-            x0[o] = v;
+            xi[s] = v;
         }
         // ---- ... and IFCE features (component/coolchic.py:105-146) from the prefetched inputs
         if constexpr (CF > 0) {
             const int n_in = g->ifce_in;
-            if (n_in > 0 && (m + 1) * OPM > NCTX) {
+            if (n_in > 0 && owns_feature(m)) {
                 const int32_t *W = reinterpret_cast<const int32_t *>(ifce_blob);
                 const long long *B =
                     reinterpret_cast<const long long *>(ifce_blob + (((size_t)n_in * CFP * 4 + 7) & ~(size_t)7));
-                long long acc[OPM];
+                long long acc[KS];
 #pragma unroll
-                for (int o = 0; o < OPM; o++) {
-                    const int f = m * OPM + o - NCTX;
-                    acc[o] = (f >= 0 && f < CF) ? B[f] : 0;
+                for (int s = 0; s < KS; s++) {
+                    const int f = 4 * s + m - NCTX;
+                    acc[s] = (f >= 0 && f < CF) ? B[f] : 0;
                 }
 #pragma unroll
                 for (int c = 0; c < CCD_IFCE_FAST_MAX; c++) {
                     if (c < n_in) {
-                        const int xi = ifv[c] << 16;
+                        const int v = ifv[c] << 16;
 #pragma unroll
-                        for (int o = 0; o < OPM; o++) {
-                            const int f = m * OPM + o - NCTX;
-                            if (f >= 0 && f < CF) acc[o] += (long long)W[c * CFP + f] * xi;
+                        for (int s = 0; s < KS; s++) {
+                            const int f = 4 * s + m - NCTX;
+                            if (f >= 0 && f < CF) acc[s] += (long long)W[c * CFP + f] * v;
                         }
                     }
                 }
 #pragma unroll
-                for (int o = 0; o < OPM; o++) {
-                    const int f = m * OPM + o - NCTX;
-                    if (f >= 0 && f < CF) {
-                        // F.interpolate(ctx.to(torch.float)).to(int64): fp32 round trip (coolchic.py:142-144)
-                        x0[o] = (int32_t)__float2ll_rz(__ll2float_rn(acc[o] >> 24));
-                    }
+                for (int s = 0; s < KS; s++) {
+                    const int f = 4 * s + m - NCTX;
+                    // F.interpolate(ctx.to(torch.float)).to(int64): fp32 round trip (coolchic.py:142-144)
+                    if (f >= 0 && f < CF) xi[s] = __float2ll_rz(__ll2float_rn(acc[s] >> 24));
                 }
             }
         }
         // ---- MLP
-        const int32_t *Wh = reinterpret_cast<const int32_t *>(arm_blob);
-        const int32_t *Wl = Wh + (size_t)n_hidden * DIM * 4 * OPMP;
-        const int32_t *Ws = Wl + DIMP * 2;
-        const size_t wbytes = ((size_t)(n_hidden * DIM * 4 * OPMP + DIMP * 4) * 4 + 7) & ~(size_t)7;
-        const long long *Bh = reinterpret_cast<const long long *>(arm_blob + wbytes);
-        const long long *Bl = Bh + (size_t)n_hidden * DIMP;
-        int32_t xo[OPM];
+        const double *Wh = reinterpret_cast<const double *>(arm_blob);
+        const double *Bh = Wh + (size_t)n_hidden * KS * NT * 32;
+        const double *Wo = Bh + (size_t)n_hidden * NT * 8;
+        const long long *Bo = reinterpret_cast<const long long *>(Wo + 16 * KS);
+        double x0[KS], xo[2 * NT];
 #pragma unroll
-        for (int o = 0; o < OPM; o++) {
-            x0[o] <<= 16;
-            xo[o] = x0[o];
-        }
+        for (int s = 0; s < KS; s++) x0[s] = (double)(xi[s] * 65536);
+#pragma unroll
+        for (int s = 0; s < 2 * NT; s++) xo[s] = s < KS ? x0[s] : 0.0;
         for (int l = 0; l < n_hidden; l++) {
-            long long acc[OPM];
-            const long long *B = Bh + (size_t)l * DIMP + m * OPM;
+            double acc[NT][2];
+            const double2 *B = reinterpret_cast<const double2 *>(Bh + (size_t)l * NT * 8) + m;
 #pragma unroll
-            for (int o = 0; o < OPM; o++) acc[o] = B[o];
-            const int32_t *W = Wh + ((size_t)l * DIM * 4 + m) * OPMP;
-#pragma unroll
-            for (int i = 0; i < DIM; i++) {
-                const int xi = __shfl_sync(0xffffffffu, xo[i % OPM], i / OPM, 4);
-                int32_t wv[8];
-                ld_w(W + (size_t)i * 4 * OPMP, wv);
-#pragma unroll
-                for (int o = 0; o < OPM; o++) acc[o] += (long long)wv[o] * xi;
+            for (int j = 0; j < NT; j++) {
+                const double2 b = B[4 * j];
+                acc[j][0] = b.x;
+                acc[j][1] = b.y;
             }
+            const double *W = Wh + (size_t)l * KS * NT * 32 + lane;
 #pragma unroll
-            for (int o = 0; o < OPM; o++) {
-                long long a = acc[o];
-                a = a < 0 ? 0 : a;
-                xo[o] = (int32_t)(a >> 16);
-            }
+            for (int s = 0; s < KS; s++)
+#pragma unroll
+                for (int j = 0; j < NT; j++) dmma_m8n8k4(acc[j], xo[s], W[(s * NT + j) * 32]);
+#pragma unroll
+            for (int j = 0; j < NT; j++)
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const double a = acc[j][e];
+                    xo[2 * j + e] = floor((a < 0.0 ? 0.0 : a) * (1.0 / 65536.0));
+                }
         }
         // last layer (on the hidden state) + stabiliser (on the input): partial sums over my inputs
-        long long t0 = 0, t1 = 0;
+        double t0 = 0.0, t1 = 0.0;
 #pragma unroll
-        for (int o = 0; o < OPM; o++) {
-            const int i = m * OPM + o;
-            const int2 wl = *reinterpret_cast<const int2 *>(Wl + 2 * i);
-            const int2 ws = *reinterpret_cast<const int2 *>(Ws + 2 * i);
-            t0 += (long long)wl.x * xo[o] + (long long)ws.x * x0[o];
-            t1 += (long long)wl.y * xo[o] + (long long)ws.y * x0[o];
+        for (int s = 0; s < KS; s++) {
+            const double2 wl = *reinterpret_cast<const double2 *>(Wo + 4 * (4 * s + m));
+            const double2 ws = *reinterpret_cast<const double2 *>(Wo + 4 * (4 * s + m) + 2);
+            t0 = fma(wl.x, xo[s], fma(ws.x, x0[s], t0));
+            t1 = fma(wl.y, xo[s], fma(ws.y, x0[s], t1));
         }
 #pragma unroll
         for (int d = 1; d < 4; d <<= 1) {
-            t0 += (long long)shfl_xor_u64((uint64_t)t0, d);
-            t1 += (long long)shfl_xor_u64((uint64_t)t1, d);
+            t0 += __shfl_xor_sync(0xffffffffu, t0, d);
+            t1 += __shfl_xor_sync(0xffffffffu, t1, d);
         }
-        o0 = (t0 + Bl[0] + Bl[2]) >> 24;
-        o1 = (t1 + Bl[1] + Bl[3]) >> 24;
+        o0 = (__double2ll_rz(t0) + Bo[0] + Bo[2]) >> 24;
+        o1 = (__double2ll_rz(t1) + Bo[1] + Bo[3]) >> 24;
     }
 };
 
@@ -467,7 +465,7 @@ __device__ __forceinline__ void produce_chunk(const SLoc &S, const SmemLayout &s
     const uint32_t need_ring = ord + 1u - (uint32_t)S.ring;          // slot reuse: ord - ring consumed
     if ((int32_t)(need_ring - need) > 0) need = need_ring;
     int ifv[CCD_IFCE_FAST_MAX];
-    if constexpr (FAST) QuadArm<NCTX, CF>::ifce_prefetch(g, S.latents, valid ? y : y0, valid ? x : x0, member, ifv);
+    if constexpr (FAST) DmmaArm<NCTX, CF>::ifce_prefetch(g, S.latents, valid ? y : y0, valid ? x : x0, member, ifv);
     // needs grow with the lane: one warp-wide wait on the maximum
     int32_t rel = valid ? (int32_t)(need - ord_diag) : INT32_MIN;
     rel = __reduce_max_sync(0xffffffffu, rel);
@@ -479,9 +477,9 @@ __device__ __forceinline__ void produce_chunk(const SLoc &S, const SmemLayout &s
     PROF_T(t1);
     long long o0 = 0, o1 = 0;
     if constexpr (FAST) {
-        // all 32 lanes take part (quad shuffles); out-of-range symbols compute on clamped coordinates
+        // all 32 lanes take part (warp-wide DMMA, quad shuffles); out-of-range symbols compute on clamped coordinates
         const int yc = valid ? y : y0, xc = valid ? x : x0;
-        QuadArm<NCTX, CF>::run(g, sm.arm, sm.ifce, ifv, sm.rows, row_mask, S.n_hidden, yc, xc, member, o0, o1);
+        DmmaArm<NCTX, CF>::run(g, sm.arm, sm.ifce, ifv, sm.rows, row_mask, S.n_hidden, yc, xc, member, o0, o1);
     } else {
         if (valid) {
             const int n_ctx = S.n_ctx, cf = S.cf;
@@ -1401,7 +1399,7 @@ int launch_t(const EntStream *d_streams, int n, size_t smem, int threads, const 
 }
 
 // =======================================================================================
-// Rate pass: k_latent_rate evaluates the ARM of every decoded symbol again -- with the decoder's own QuadArm /
+// Rate pass: k_latent_rate evaluates the ARM of every decoded symbol again -- with the decoder's own DmmaArm /
 // GenericArm on the same row-ring layout, fed from a staged tile instead of the wavefront -- and turns the
 // symbol's cumulative window into freq = left(s+1) - left(s) and bits = 24 - log2(freq).
 // =======================================================================================
@@ -1485,15 +1483,15 @@ __device__ __forceinline__ void rate_tile(const RateTile &t, const RateJobDev &J
     if constexpr (FAST) {
         const int member = tid & 3;
         for (int s0 = 0; s0 < n; s0 += nthr >> 2) {
-            // uniform trip count: every lane of a warp takes part in the quad shuffles
+            // uniform trip count: every lane of a warp takes part in the DMMAs and quad shuffles
             const int s = s0 + (tid >> 2);
             const bool valid = s < n;
             const int ty = valid ? s / nc : 0, tx = valid ? s - ty * nc : 0;
             const int y = t.y0 + ty, x = t.x0 + tx;
             int ifv[CCD_IFCE_FAST_MAX];
-            QuadArm<NCTX, CF>::ifce_prefetch(g, lat, y, x, member, ifv);
+            DmmaArm<NCTX, CF>::ifce_prefetch(g, lat, y, x, member, ifv);
             long long o0, o1;
-            QuadArm<NCTX, CF>::run(g, arm, ifce, ifv, rows, row_mask, n_hidden, y, x, member, o0, o1);
+            DmmaArm<NCTX, CF>::run(g, arm, ifce, ifv, rows, row_mask, n_hidden, y, x, member, o0, o1);
             if (valid && member == 0) {
                 const int sym = lds_s8(rows + (((uint32_t)y & row_mask) << 6 | ((uint32_t)x & (CCD_ROW_COLS - 1))));
                 acc += rate_symbol(o0, o1, sym, base + (long long)y * w + x, J, cdf, scale_tab);

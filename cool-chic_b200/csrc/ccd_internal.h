@@ -78,14 +78,13 @@ struct EntStream {
 };
 
 // Blob layouts ---------------------------------------------------------------------------
-// FAST (int32 operands, proven not to overflow by the host-side bound analysis); a symbol is
-// evaluated by a quad of lanes, member m owning activations [m*opm, (m+1)*opm):
-//   opm = ceil(dim/4), opmp = 2|4|8 (opm padded for vector loads), dimp = 4*opm
-//   int32 Wh[n_hidden][dim][4][opmp]   weight of input i for the outputs of member m
-//   int32 Wl[dimp][2]                  last layer   (rows >= dim are zero)
-//   int32 Ws[dimp][2]                  stabiliser   (zeros if absent)
-//   (pad to 8 bytes)
-//   int64 Bh[n_hidden][dimp], Bl[2], Bs[2]
+// FAST (f64 on the DMMA m8n8k4 tensor cores, every value an integer below 2^53: proven by arm_fits_f64); a symbol
+// is evaluated by a quad of lanes, member t owning inputs t, t + 4, ...:
+//   ks = ceil(dim/4) k-steps, nt = ceil(ks/2) n-tiles; unit(j, c) = 8j + 4(c & 1) + (c >> 1) (column c of tile j)
+//   f64 Wh[n_hidden][ks][nt][32]   B fragments: lane L holds W[4s + (L & 3)][unit(j, L >> 2)]
+//   f64 Bh[n_hidden][nt][8]        C fragments: column c of tile j holds B[unit(j, c)]
+//   f64 Wo[4 ks][4]                last layer (2 outputs), then stabiliser (2 outputs); rows >= dim are zero
+//   int64 Bl[2], Bs[2]
 // IFCE arm (FAST): int32 W[n_in][cfp] (cfp = cf rounded up to 4), pad8, int64 B[cf]
 // GENERIC (all int64): W64h[n_hidden][dim][dim], Wl[dim][2], Ws[dim][2], Bh, Bl, Bs;
 //   IFCE: int64 W[n_in][cf], B[cf]

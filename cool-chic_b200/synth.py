@@ -113,22 +113,29 @@ def _fit(src: np.ndarray, shape: Sequence[int]) -> np.ndarray:
     return out
 
 
+def _source(src: Dict[str, Dict[str, np.ndarray]], key: str, idx: int, name: str) -> Optional[np.ndarray]:
+    """The sample's tensor that adapt_nn copies into tensor ``name`` (position ``idx`` of section ``key``), or None."""
+    src_names = list(src[key].keys())
+    if name in src[key]:
+        return src[key][name]
+    if key.startswith("ifce") and src_names:
+        return src[key][src_names[min(idx, len(src_names) - 1)]]
+    if key.startswith("upsampling") and src_names:
+        kind = [n for n in src_names if n.rstrip("0123456789") == name.rstrip("0123456789")] or src_names
+        return src[key][kind[idx % len(kind)]]
+    return None
+
+
 def adapt_nn(src_d: CcdCoolChicDesc, src_ints: np.ndarray, dst_d: CcdCoolChicDesc) -> np.ndarray:
-    """Re-shape the sample's network integers for another architecture of the same family."""
+    """Re-shape the sample's network integers for another architecture of the same family.  Every entry the sample
+    does not have is zero (liven_nn fills them)."""
     src = split_nn(src_d, src_ints)
     dst: Dict[str, Dict[str, np.ndarray]] = {}
     for key, items in nn_sections(dst_d).items():
         dst[key] = {}
-        src_names = list(src[key].keys())
         for idx, (name, shape) in enumerate(items):
-            if name in src[key]:
-                cand = src[key][name]
-            elif key.startswith("ifce") and src_names:
-                cand = src[key][src_names[min(idx, len(src_names) - 1)]]
-            elif key.startswith("upsampling") and src_names:
-                kind = [n for n in src_names if n.rstrip("0123456789") == name.rstrip("0123456789")] or src_names
-                cand = src[key][kind[idx % len(kind)]]
-            else:
+            cand = _source(src, key, idx, name)
+            if cand is None:
                 cand = np.zeros(shape, dtype=np.int64)
             dst[key][name] = _fit(cand, shape) if cand.shape != tuple(shape) else cand.copy()
     if dst_d.common_randomness and not src_d.common_randomness:
@@ -138,6 +145,59 @@ def adapt_nn(src_d: CcdCoolChicDesc, src_ints: np.ndarray, dst_d: CcdCoolChicDes
         w0[:, half:] = w0[:, :half] // 3 + 1
     ints, _ = join_nn(dst_d, dst)
     return ints
+
+
+def liven_nn(src_d: CcdCoolChicDesc, src_ints: np.ndarray, dst_d: CcdCoolChicDesc, seed: int) -> np.ndarray:
+    """adapt_nn with every entry it padded made live: residue channels 3 and 4, the second flow, synthesis units past
+    the sample's width, latent grids past its count and ARM units past its 14 + 6 otherwise only ever meet zero
+    weights.  A padded entry gets a value drawn from the nonzero values of the same tensor (of its section, when the
+    tensor has none) with a random sign; the sample's own zeros stay zero."""
+    src = split_nn(src_d, src_ints)
+    dst = split_nn(dst_d, adapt_nn(src_d, src_ints, dst_d))
+    rng = np.random.default_rng(seed)
+    for key, items in nn_sections(dst_d).items():
+        for idx, (name, shape) in enumerate(items):
+            t = dst[key][name]
+            cand = _source(src, key, idx, name)
+            pad = np.ones(t.shape, dtype=bool)
+            if cand is not None:
+                pad[tuple(slice(0, min(a, b)) for a, b in zip(cand.shape, t.shape))] = False
+            if key == "synthesis.weight" and name == "l0" and dst_d.common_randomness and not src_d.common_randomness:
+                pad[:, dst_d.syn_in // 2:] = pad[:, :dst_d.syn_in // 2]  # adapt_nn's copies of the latent half
+            if not pad.any():
+                continue
+            pool = np.abs(t[t != 0])
+            if pool.size == 0:
+                pool = np.abs(np.concatenate([v[v != 0] for v in dst[key].values()] + [np.ones(1, np.int64)]))
+            n = int(pad.sum())
+            t[pad] = rng.choice(pool, size=n) * rng.choice(np.array([-1, 1]), size=n)
+    ints, _ = join_nn(dst_d, dst)
+    return ints
+
+
+# 5th / 95th percentiles the output channels are moved to by scale_outputs, per kind of Cool-chic; channels 3 / 4 of a
+# residue are alpha / beta - 0.5, so that alpha and beta have samples below 0, inside (0, 1) and above 1; a motion
+# Cool-chic's outputs are flows in pixels
+OUTPUT_TARGETS = {"intra": [(-0.06, 1.06)] * 3,
+                  "residue": [(-0.45, 0.45)] * 3 + [(-0.8, 0.8)] * 2,
+                  "motion": [(-3.5, 3.5)] * 4}
+
+
+def scale_outputs(desc: CcdCoolChicDesc, ints: np.ndarray, raw: np.ndarray, kind: str) -> np.ndarray:
+    """The network integers with every output channel c mapped affinely so that its 5th / 95th percentiles (on ``raw``,
+    the unmodified output [C, H, W]) go to about OUTPUT_TARGETS[kind][c]: rows of the output transform scaled, its
+    biases shifted."""
+    t = split_nn(desc, ints)
+    w, b = t["synthesis.weight"]["out"], t["synthesis.bias"]["out"]
+    qb = 2.0 ** desc.qshift[NN_MODULES.index("synthesis") * len(NN_KINDS) + NN_KINDS.index("bias")]
+    for c in range(w.shape[0]):
+        lo, hi = OUTPUT_TARGETS[kind][c]
+        p5, p95 = np.percentile(raw[c].astype(np.float64), [5, 95])
+        a = (hi - lo) / max(p95 - p5, 1e-3)
+        w[c] = np.round(a * w[c])
+        b[c] = int(round(a * b[c] + (lo - a * p5) / qb))
+    out, _ = join_nn(desc, t)
+    return out
 
 
 # ---- latents ---------------------------------------------------------------------------------
@@ -239,13 +299,22 @@ class SeedStream:
 
 def make_coolchic(ctx, seed_stream: SeedStream, img_size, latent_resolution=(0, 6), hyperlatent_resolution=None,
                   seed: int = 0, final_upsampling_type=None, overrides=None, latents: Optional[torch.Tensor] = None,
-                  nn: Optional[np.ndarray] = None) -> Tuple[bytes, CoolChicHeader, torch.Tensor]:
+                  nn: Optional[np.ndarray] = None,
+                  live: Optional[str] = None) -> Tuple[bytes, CoolChicHeader, torch.Tensor]:
     """One Cool-chic section (header + NN payload + latent payload) for an image of ``img_size``.  ``nn``: the
-    network integers to write (in bitstream order, for the header's architecture) instead of the sample's."""
+    network integers to write (in bitstream order, for the header's architecture) instead of the sample's.
+    ``live`` ("intra", "residue" or "motion"): the sample's network through liven_nn (seeded by ``seed``), its outputs
+    then moved by scale_outputs to look like those of that kind of Cool-chic, measured on ``ctx.synthesize``."""
     header = make_coolchic_header(seed_stream.header, img_size, latent_resolution, hyperlatent_resolution,
                                   final_upsampling_type, overrides)
     desc = desc_from_header(header)
-    if nn is None:
+    if latents is None:
+        latents = tile_latents(seed_stream.desc, seed_stream.latents, desc, seed)
+    if nn is None and live is not None:
+        nn = liven_nn(seed_stream.desc, seed_stream.nn, desc, seed)
+        raw = ctx.synthesize([desc], [nn], [latents], [0])[0][0].cpu().numpy()
+        nn = scale_outputs(desc, nn, raw, live)
+    elif nn is None:
         nn = adapt_nn(seed_stream.desc, seed_stream.nn, desc)
     nn = np.asarray(nn, dtype=np.int64)
     _, counts = join_nn(desc, split_nn(desc, nn))
@@ -253,8 +322,6 @@ def make_coolchic(ctx, seed_stream: SeedStream, img_size, latent_resolution=(0, 
     header.set_value("nn_n_bytes", len(nn_bytes))
     header.set_value("nn_n_bit_pad", pad)
     desc = desc_from_header(header)
-    if latents is None:
-        latents = tile_latents(seed_stream.desc, seed_stream.latents, desc, seed)
     lat_dev, payload, _ = ctx.encode_latents(desc, nn, latents=latents)
     header.set_value("n_bytes_latent", len(payload))
     return header.to_bytes() + nn_bytes + payload, header, lat_dev
@@ -262,16 +329,18 @@ def make_coolchic(ctx, seed_stream: SeedStream, img_size, latent_resolution=(0, 
 
 def make_image_stream(ctx, seed_stream: SeedStream, height: int, width: int, frame_data_type: str = "rgb",
                       bitdepth: int = 8, latent_resolution=(0, 6), hyperlatent_resolution=None, seed: int = 0,
-                      final_upsampling_type: Optional[str] = None, overrides: Optional[dict] = None) -> bytes:
+                      final_upsampling_type: Optional[str] = None, overrides: Optional[dict] = None,
+                      live: bool = False) -> bytes:
     """A complete single-frame (intra) bitstream.  ``overrides`` sets Cool-chic header fields, e.g.
-    ``{"flag_common_randomness": 1}``; ``final_upsampling_type`` matters when latent_resolution[0] > 0."""
+    ``{"flag_common_randomness": 1}``; ``final_upsampling_type`` matters when latent_resolution[0] > 0.  ``live``:
+    every weight of the network live (make_coolchic)."""
     v = VideoHeader()
     v.set_header(1, [0], [])
     f = FrameHeader()
     f._values.update(display_index=0, frame_type="I", frame_data_type=frame_data_type, bitdepth=bitdepth,
                      index_references=[], global_flow=[])
     cc, _, _ = make_coolchic(ctx, seed_stream, (height, width), latent_resolution, hyperlatent_resolution, seed,
-                             final_upsampling_type, overrides)
+                             final_upsampling_type, overrides, live="intra" if live else None)
     return v.to_bytes() + f.to_bytes() + cc
 
 
@@ -287,11 +356,12 @@ def _syn_overrides(width: int, out_ch: int, n_layers: int) -> dict:
 
 def make_video_stream(ctx, seed_stream: SeedStream, height: int, width: int, n_frames: int,
                       frame_data_type: str = "yuv420", bitdepth: int = 8, warp_filter_size: int = 8,
-                      seed: int = 0) -> bytes:
+                      seed: int = 0, live: bool = False) -> bytes:
     """A GOP: I frame, last frame P, hierarchical B in between (codingstructure.py:267-436).
     Architectures follow cfg/dec: intra = hop; residue of P/B = mop widths (ARM 10+2, 16-wide
     synthesis, 4 / 5 output channels); motion = mop (latent_resolution 2-6, ARM 6+2, 16-wide
-    synthesis with 2 / 4 outputs, nearest final upsampling)."""
+    synthesis with 2 / 4 outputs, nearest final upsampling).  ``live``: every weight of every network live, with
+    residue alpha / beta and flows that vary (make_coolchic)."""
     from .utils.codingstructure import CodingStructure
 
     p_pos = [n_frames - 1] if n_frames > 1 else []
@@ -312,16 +382,18 @@ def make_video_stream(ctx, seed_stream: SeedStream, height: int, width: int, n_f
         out += f.to_bytes()
         s = 100 * seed + coding_idx
         if fr.frame_type == "I":
-            cc, _, _ = make_coolchic(ctx, seed_stream, (height, width), (0, 6), None, seed=s)
+            cc, _, _ = make_coolchic(ctx, seed_stream, (height, width), (0, 6), None, seed=s,
+                                     live="intra" if live else None)
             out += cc
         else:
             ov = {"spatial_context_arm": 10, "output_feature_ifce": 2}
             ov.update(_syn_overrides(16, 3 + n_ref, 4))
-            cc, _, _ = make_coolchic(ctx, seed_stream, (height, width), (0, 6), None, seed=s, overrides=ov)
+            cc, _, _ = make_coolchic(ctx, seed_stream, (height, width), (0, 6), None, seed=s, overrides=ov,
+                                     live="residue" if live else None)
             out += cc
             ov = {"spatial_context_arm": 6, "output_feature_ifce": 2, "ifce_resolution": [2, 2]}
             ov.update(_syn_overrides(16, 2 * n_ref, 2))
             cc, _, _ = make_coolchic(ctx, seed_stream, (height, width), (2, 6), None, seed=s + 50,
-                                     final_upsampling_type="nearest", overrides=ov)
+                                     final_upsampling_type="nearest", overrides=ov, live="motion" if live else None)
             out += cc
     return out

@@ -8,7 +8,14 @@ import ccoracle
 
 
 class OracleBackend:
-    """Same three methods as coolchic_b200._native.Context, computed by the oracle."""
+    """Same methods as coolchic_b200._native.Context, computed by the oracle (the raw output only)."""
+
+    def synthesize(self, descs, nn_ints, latents, zero_grids):
+        outs = []
+        for d, nn, lat, z in zip(descs, nn_ints, latents, zero_grids):
+            assert z == 0
+            outs.append(torch.from_numpy(ccoracle.synthesize(d, nn, np.asarray(lat.cpu().numpy(), np.int8)))[None])
+        return outs
 
     def decode_nn(self, desc, nn_bytes):
         return ccoracle.decode_nn(desc, nn_bytes)

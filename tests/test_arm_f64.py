@@ -85,14 +85,20 @@ def fits_f64(a):
     return last is not None and all(int(v) < LIM for v in last + stab)
 
 
-def unit(j, c):
+def _unit(j, c):
     """The hidden unit in accumulator column c of n-tile j."""
     return 8 * j + 4 * (c & 1) + (c >> 1)
 
 
-def pack(a):
-    """pack_arm's fast layout, as arrays: Wh [l][s][j][lane], Bh [l][j][column], Wo [input][wl0, wl1, ws0, ws1]."""
+def pack(a, bug=None):
+    """pack_arm's fast layout, as arrays: Wh [l][s][j][lane], Bh [l][j][column], Wo [input][wl0, wl1, ws0, ws1].
+    ``bug="tile3_perm"`` (a negative control): the fourth n-tile (units 24 ... 31) packed with its column pairs
+    swapped."""
     dim, hidden = a["dim"], a["layers"][:-1]
+
+    def unit(j, c):
+        return _unit(j, c ^ 1 if bug == "tile3_perm" and j == 3 else c)
+
     ks = (dim + 3) // 4
     nt = (ks + 1) // 2
     Wh = np.zeros((len(hidden), ks, nt, 32))

@@ -17,7 +17,9 @@ from conftest import GOLDEN, ROOT
 ORIGINALS = {"kodim15_192x128_01p_yuv420_10b.yuv": 1, "kodim15_192x128_01p_yuv444_8b.yuv": 1,
              "192x128_kodim15.png": 1, "D-BQSquare-3frames_224x128_60p_yuv420_8b.yuv": 3}
 GOPS = [("gop5_64x96_yuv420", "yuv420"), ("gop3_40x56_rgb", "rgb"), ("gop3_48x72_yuv420_bilinear", "yuv420"),
-        ("gop3_40x56_rgb_bicubic", "rgb"), ("gop3_48x72_yuv420_sinc6", "yuv420"), ("gop4_40x56_rgb_sinc12", "rgb")]
+        ("gop3_40x56_rgb_bicubic", "rgb"), ("gop3_48x72_yuv420_sinc6", "yuv420"), ("gop4_40x56_rgb_sinc12", "rgb"),
+        # every network weight live (oracle/gen_golden_dense.py): alpha and beta vary per pixel and differ
+        ("gop3_40x56_rgb_sinc8_dense", "rgb"), ("gop3_48x72_yuv420_bicubic_dense", "yuv420")]
 
 
 # ---- checker: the reference's formulas restated on integer errors ------------------------------------------------

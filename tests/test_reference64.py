@@ -284,8 +284,11 @@ def synthesis(p, P, x, bug=None):
     """synthesis.py:272-294."""
     h = x
     for i, (_, _, res, relu) in enumerate(p.parsed_synthesis_layers()):
-        y = _syn_conv(h, P[("synthesis", f"main_branch.{2 * i}", "weight")],
-                      P[("synthesis", f"main_branch.{2 * i}", "bias")])
+        w, b = P[("synthesis", f"main_branch.{2 * i}", "weight")], P[("synthesis", f"main_branch.{2 * i}", "bias")]
+        if bug == "drop_hidden48" and i == 0:
+            w, b = w.clone(), b.clone()
+            w[48:], b[48:] = 0, 0
+        y = _syn_conv(h, w, b)
         if res:
             y = _add(y, h)  # synthesis.py:73-74: the residual adds the layer's input, before the non-linearity
         if relu:
@@ -347,6 +350,8 @@ def intra(header, ints, lat, bug=None):
     P = dequantise(header, ints)
     grids = latent_grids(p, lat)
     coded = [g for g, hyp in zip(grids, p.flag_is_hyperlatent) if not hyp]
+    if bug == "drop_grids7":
+        coded = coded[:7] + [torch.zeros_like(g) for g in coded[7:]]
     x = upsampling(p, P, coded, bug)
     if p.flag_common_randomness:
         x = _cat(x, cr_noise(p))
@@ -430,15 +435,19 @@ def inter(residue, motion, refs, gf, fs, bug=None):
     if bug == "neg_gf1":
         g[1] = [-x for x in g[1]]
     shifted = [global_shift(torch.from_numpy(np.asarray(rf, dtype=np.float64)), g[i]) for i, rf in enumerate(refs)]
-    alpha = torch.clamp(r[3] + 0.5, 0, 1)
+    ia, ib = (4, 3) if is_b and bug == "swap_ab" else (3, 4)
+    if is_b and bug == "drop_flow1_y":
+        mo = mo.clone()
+        mo[3] = 0
+    alpha = torch.clamp(r[ia] + 0.5, 0, 1)
     pred = warp(shifted[0], mo[0:2], fs, bug)
     if is_b:
-        beta = torch.clamp(r[4] + 0.5, 0, 1)
-        bm = r[4].abs() + 0.5
+        beta = torch.clamp(r[ib] + 0.5, 0, 1)
+        bm = r[ib].abs() + 0.5
         p2 = warp(shifted[1], mo[2:4], fs, bug)
         pred = T(beta * pred.v + (1 - beta) * p2.v, bm * pred.m + (1 + bm) * p2.m, bm * pred.e + (1 + bm) * p2.e,
                  max(pred.k, p2.k) + 4)
-    am = r[3].abs() + 0.5
+    am = r[ia].abs() + 0.5
     return T(alpha * pred.v + r[0:3], am * pred.m + r[0:3].abs(), am * pred.e, pred.k + 3)
 
 
@@ -786,12 +795,15 @@ REF_FIXTURES = ["img_48x72_rgb_common_randomness", "img_50x70_rgb_final_bicubic"
                 "gop3_40x56_yuv420_16bit", "gop3_39x57_rgb_13bit"]
 
 
-def reference_fixture(oracle, name, bug=None):
+def reference_fixture(oracle, name, bug=None, measured_window=False, failures=None):
     """Each Cool-chic of the stream restated and compared with the reference's raw output under the bound; each frame's
     integer samples against the reference's, within the measured error of the raw output of a tie (I frames), or
     within the prediction's bound (P / B frames, predicted from the reference's own residue, motion and decoded
     references).  Returns the largest max |err| / bound; with ``bug`` nothing is asserted, and a frame whose
-    integer samples differ off a tie counts as infinitely far."""
+    integer samples differ off a tie counts as infinitely far.  The tie windows then come from the restatement without
+    the bug, so that what catches a bug is the reference's samples, not a window the bug itself widened; ``failures``
+    (a list) receives the message of each frame's failed check.  ``measured_window``: the P / B tie window is the
+    oracle's measured error at every bit depth (below, see bd > 10)."""
     from coolchic_b200.bitstream.header import FrameHeader, VideoHeader
 
     data = open(os.path.join(GOLDEN, name + ".cool"), "rb").read()
@@ -809,8 +821,8 @@ def reference_fixture(oracle, name, bug=None):
         for cc in ccs:
             x, r = _restate_coolchic(oracle, *cc, bug=bug), raw[f"c{i}"]
             worst = max(worst, ratio(r, x))
-            err = (torch.from_numpy(r).to(torch.float64) - x.v).abs() if bug else assert_within(
-                r, x, f"{name} Cool-chic {i}")
+            err = (torch.from_numpy(r).to(torch.float64) - _restate_coolchic(oracle, *cc).v).abs() if bug else (
+                assert_within(r, x, f"{name} Cool-chic {i}"))
             outs.append((x, r, err))
             i += 1
         M = 2**bd - 1
@@ -827,20 +839,23 @@ def reference_fixture(oracle, name, bug=None):
             gf, fs = f.get_value("global_flow"), f.get_value("warp_filter_size")
             x = inter(outs[0][1], outs[1][1], refs, gf, fs, bug)
             window = None
-            if bd > 10:
+            if bd > 10 or measured_window:
                 # the a-priori bound of a prediction is some 30 times its measured error, which at these bit depths
                 # puts most samples within M * bound of a tie; the window is then four times the error the oracle's
                 # fp32 prediction of the same inputs measures, sample by sample (itself checked against the bound)
                 pre = oracle.inter_predict(outs[0][1], outs[1][1], refs[0], refs[1] if len(refs) == 2 else None, gf, fs)
-                err = (torch.from_numpy(pre).to(torch.float64) - x.v).abs() if bug else assert_within(
+                x0 = inter(outs[0][1], outs[1][1], refs, gf, fs) if bug else x
+                err = (torch.from_numpy(pre).to(torch.float64) - x0.v).abs() if bug else assert_within(
                     pre, x, f"{name} frame {f.get_value('display_index')} oracle prediction")
                 window = 4 * err
         try:
             t, d = check_levels(frame(f.get_value("display_index")), x, bd, fmt,
                                 f"{name} frame {f.get_value('display_index')}", window=window)
-        except AssertionError:
+        except AssertionError as e:
             if bug is None:
                 raise
+            if failures is not None:
+                failures.append(str(e).splitlines()[0])
             worst = math.inf
             continue
         n_tie += t

@@ -29,6 +29,7 @@
 #include "ccd_internal.h"
 
 #ifdef CCD_PROFILE
+#include <cstdio>
 #define PROF_T(var) long long var = clock64()
 #define PROF_ADD(acc, t0) acc += clock64() - (t0)
 #else
@@ -796,18 +797,17 @@ __device__ __forceinline__ uint2 lds_v2(uint32_t a) {
     return v;
 }
 
-// TIER 2 as a function (out of line, rare): symbol j, state and word position by value in, by value out (registers;
-// a reference into the kernel's state would put it in local memory).  A taken branch costs the coder warp ~40 cycles
-// (instruction refetch: no other warp on its scheduler hides it), so the steady loop of the coder is straight-line
-// code that reaches this function only when a round fails.  The word a renormalisation shifts in is loaded from
-// global memory (the _g of the name).
-struct T2Out {
-    uint32_t d_lo, d_hi, r_lo, r_hi, w0, wpos;
-    uint32_t flags;  // 2: outside the window (exact search), 4: desynchronised, 8: far (instrumented build)
+// TIER 2 of one symbol j: M-1 / M / M+1 by selects, the far path (coder_far) otherwise, renormalisation with the word
+// w0 = word[wpos] shifted in; the symbol's result word is written unless it is the mode.  Inline in both of its
+// callers below, which are out of line themselves.
+struct T2Step {
+    uint64_t D, R;
+    uint32_t renorm;  // 1: the step shifted w0 in
+    uint32_t flags;   // 2: outside the window (exact search), 4: desynchronised, 8: far (instrumented build)
 };
-__device__ __noinline__ T2Out coder_tier2_g(uint32_t res_a, uint32_t win_a, uint32_t meta_a, const float *__restrict__ scale_tab,
-                                            uint32_t ring_mask, int lane, uint32_t j, const uint4 h, uint64_t D, uint64_t R,
-                                            uint32_t w0, uint32_t wpos, const uint32_t *__restrict__ words, uint32_t wmax) {
+__device__ __forceinline__ T2Step tier2_step(uint32_t res_a, uint32_t win_a, uint32_t meta_a,
+                                             const float *__restrict__ scale_tab, uint32_t ring_mask, int lane, uint32_t j,
+                                             const uint4 h, uint64_t D, uint64_t R, uint32_t w0) {
     const uint64_t scale = R >> 24;
     const uint64_t P0 = scale * h.x, P1 = scale * h.y, P2 = scale * h.z, P3 = scale * h.w;
     const bool c1 = D >= P1, c2 = D >= P2;
@@ -818,63 +818,152 @@ __device__ __noinline__ T2Out coder_tier2_g(uint32_t res_a, uint32_t win_a, uint
     // 2^64 + D < P1), D >= P3 leaves Dn >= P3 - P2 = Rn; an empty candidate interval (left(M-1) == left(M) at the
     // lower end of the alphabet) wraps as well
     uint32_t rw = c2 ? (CCD_WIN_HALF + 1u) : (c1 ? (uint32_t)CCD_WIN_HALF : (CCD_WIN_HALF - 1u));
-    uint32_t flags = 0u;
+    T2Step o;
+    o.flags = 0u;
     if (Dn >= Rn) {
         const uint32_t slot = j & ring_mask;
-        const FarOut o = coder_far(win_a + slot * (CCD_WIN * 4), meta_a + slot * 16u, scale_tab, lane, scale, D);
-        Dn = D - o.lo;
-        Rn = o.hi - o.lo;
-        rw = o.rw;
-        flags = o.flags | 8u;
+        const FarOut f = coder_far(win_a + slot * (CCD_WIN * 4), meta_a + slot * 16u, scale_tab, lane, scale, D);
+        Dn = D - f.lo;
+        Rn = f.hi - f.lo;
+        rw = f.rw;
+        o.flags = f.flags | 8u;
     }
-    if ((Rn >> 32) == 0) {
+    o.renorm = (Rn >> 32) == 0 ? 1u : 0u;
+    if (o.renorm) {
         Dn = (Dn << 32) | w0;
         Rn <<= 32;
+    }
+    if (rw != (uint32_t)CCD_WIN_HALF) sts_u32(res_a + (j & ring_mask) * 4u, res_tag(j) | rw);
+    o.D = Dn;
+    o.R = Rn;
+    return o;
+}
+
+// TIER 2 as a function, for the single-symbol steps of short diagonals: state and word position by value in, by value
+// out (registers; a reference into the kernel's state would put it in local memory).  The word after a
+// renormalisation is loaded from global memory (the _g of the name): these steps do not keep the word window current.
+struct T2Out {
+    uint32_t d_lo, d_hi, r_lo, r_hi, w0, wpos;
+    uint32_t flags;  // as T2Step::flags
+};
+__device__ __noinline__ T2Out coder_tier2_g(uint32_t res_a, uint32_t win_a, uint32_t meta_a, const float *__restrict__ scale_tab,
+                                            uint32_t ring_mask, int lane, uint32_t j, const uint4 h, uint64_t D, uint64_t R,
+                                            uint32_t w0, uint32_t wpos, const uint32_t *__restrict__ words, uint32_t wmax) {
+    const T2Step s = tier2_step(res_a, win_a, meta_a, scale_tab, ring_mask, lane, j, h, D, R, w0);
+    if (s.renorm) {
         wpos++;
         w0 = coder_word(words, wmax, wpos);
     }
-    if (rw != (uint32_t)CCD_WIN_HALF) sts_u32(res_a + (j & ring_mask) * 4u, res_tag(j) | rw);
     T2Out r;
-    r.d_lo = (uint32_t)Dn;
-    r.d_hi = (uint32_t)(Dn >> 32);
-    r.r_lo = (uint32_t)Rn;
-    r.r_hi = (uint32_t)(Rn >> 32);
+    r.d_lo = (uint32_t)s.D;
+    r.d_hi = (uint32_t)(s.D >> 32);
+    r.r_lo = (uint32_t)s.R;
+    r.r_hi = (uint32_t)(s.R >> 32);
     r.w0 = w0;
     r.wpos = wpos;
-    r.flags = flags;
+    r.flags = s.flags;
     return r;
 }
 
-// A round none of whose sequences matched: the longest decided prefix (0, 1 or 2 symbols) is taken from a lane that
-// matched it -- its state after that prefix, its result words -- and the next symbol goes through tier 2.
-struct PrefixOut {
-    uint32_t d_lo, d_hi, r_lo, r_hi, k, n;
+// THE RARE PATH of a speculative round, one out-of-line call (DESIGN §4.1).  The round's caller accepts a matched round
+// with selects and tests one predicate: the round did not match, or the word window must move, or fewer than `need`
+// symbols past j are known to be ready.  Under it, this function does all three, in that order:
+//   * a failed round: the longest decided prefix (0, 1 or 2 symbols) is taken from a lane that matched it -- its state
+//     after that prefix, its result words -- and the next symbol goes through tier 2; `done` is published;
+//   * the window move: lane l loads word[wpos + l];
+//   * the refresh of `limit` from `ready`; still fewer than `need` ready: the caller leaves the steady loop (flag 1).
+// Everything in and out by value (registers).  The caller reloads the words of the window and the round's intervals.
+struct RareOut {
+    uint32_t d_lo, d_hi, r_lo, r_hi, j, wpos, wbase, wcur, limit;
+    uint32_t flags;  // 1: leave the steady loop, otherwise as T2Step::flags
+#ifdef CCD_PROFILE
+    uint32_t n_pre, cyc_fail, cyc_move, cyc_ref;  // decided prefix; cycles of the three parts
+#endif
 };
-__device__ __noinline__ PrefixOut spec_prefix(uint32_t res_a, uint32_t ring_mask, int lane, uint32_t j, uint32_t ok1,
-                                              uint32_t ok12, uint64_t d1, uint64_t r1, uint32_t k1, uint64_t d2,
-                                              uint64_t r2, uint32_t k2) {
-    PrefixOut o;
-    const uint32_t b1 = __ballot_sync(0xffffffffu, ok1 != 0u), b2 = __ballot_sync(0xffffffffu, ok12 != 0u);
-    o.n = b2 ? 2u : (b1 ? 1u : 0u);
-    o.d_lo = o.d_hi = o.r_lo = o.r_hi = o.k = 0u;
-    if (o.n) {
-        const int src = __ffs((int)(b2 ? b2 : b1)) - 1;
-        const uint64_t ds = b2 ? d2 : d1, rs = b2 ? r2 : r1;
-        o.d_lo = __shfl_sync(0xffffffffu, (uint32_t)ds, src);
-        o.d_hi = __shfl_sync(0xffffffffu, (uint32_t)(ds >> 32), src);
-        o.r_lo = __shfl_sync(0xffffffffu, (uint32_t)rs, src);
-        o.r_hi = __shfl_sync(0xffffffffu, (uint32_t)(rs >> 32), src);
-        o.k = __shfl_sync(0xffffffffu, b2 ? k2 : k1, src);
-        const uint32_t q1 = (uint32_t)src % 3u, q2 = ((uint32_t)src / 3u) % 3u;
-        if (lane == 0) {
-            if (q1 != 1u) sts_u32(res_a + (j & ring_mask) * 4u, res_tag(j) | (CCD_WIN_HALF - 1u + q1));
-            if (o.n == 2u && q2 != 1u)
-                sts_u32(res_a + ((j + 1u) & ring_mask) * 4u, res_tag(j + 1u) | (CCD_WIN_HALF - 1u + q2));
+__device__ __noinline__ RareOut coder_rare(uint32_t ctrl, uint32_t hot, uint32_t res, uint32_t win, uint32_t meta,
+                                           const float *__restrict__ scale_tab, uint32_t ring_mask, int lane, uint32_t need,
+                                           uint32_t miss, uint32_t ok1, uint32_t ok12, uint64_t d1, uint64_t r1, uint32_t k1,
+                                           uint64_t d2, uint64_t r2, uint32_t k2, uint64_t D, uint64_t R, uint32_t j,
+                                           uint32_t wpos, uint32_t wbase, uint32_t wcur, uint32_t limit, uint32_t ord_end,
+                                           const uint32_t *__restrict__ words, uint32_t wmax) {
+    RareOut o;
+    o.flags = 0u;
+#ifdef CCD_PROFILE
+    o.n_pre = o.cyc_fail = o.cyc_move = o.cyc_ref = 0u;
+    long long t0 = clock64();
+#endif
+    if (miss) {
+        const uint32_t b1 = __ballot_sync(0xffffffffu, ok1 != 0u), b2 = __ballot_sync(0xffffffffu, ok12 != 0u);
+        const uint32_t n = b2 ? 2u : (b1 ? 1u : 0u);
+        if (n) {
+            const int src = __ffs((int)(b2 ? b2 : b1)) - 1;
+            const uint64_t ds = b2 ? d2 : d1, rs = b2 ? r2 : r1;
+            D = ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(ds >> 32), src) << 32) |
+                __shfl_sync(0xffffffffu, (uint32_t)ds, src);
+            R = ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(rs >> 32), src) << 32) |
+                __shfl_sync(0xffffffffu, (uint32_t)rs, src);
+            wpos += __shfl_sync(0xffffffffu, b2 ? k2 : k1, src);
+            const uint32_t q1 = (uint32_t)src % 3u, q2 = ((uint32_t)src / 3u) % 3u;
+            if (lane == 0) {
+                if (q1 != 1u) sts_u32(res + (j & ring_mask) * 4u, res_tag(j) | (CCD_WIN_HALF - 1u + q1));
+                if (n == 2u && q2 != 1u)
+                    sts_u32(res + ((j + 1u) & ring_mask) * 4u, res_tag(j + 1u) | (CCD_WIN_HALF - 1u + q2));
+            }
+            __syncwarp();
+            j += n;
         }
-        __syncwarp();
+        const uint4 h = lds_v4(hot + (j & ring_mask) * 16u);
+        const uint32_t wj = __shfl_sync(0xffffffffu, wcur, (int)(wpos - wbase));
+        const T2Step s = tier2_step(res, win, meta, scale_tab, ring_mask, lane, j, h, D, R, wj);
+        D = s.D;
+        R = s.R;
+        wpos += s.renorm;
+        o.flags = s.flags;
+        j++;
+        sts_done(ctrl + 8u, j);
+#ifdef CCD_PROFILE
+        o.n_pre = n;
+        const long long t1 = clock64();
+        o.cyc_fail = (uint32_t)(t1 - t0);
+        t0 = t1;
+#endif
     }
+    if (wpos - wbase >= 24u) {
+        wbase = wpos;
+        wcur = coder_word(words, wmax, wbase + (uint32_t)lane);
+#ifdef CCD_PROFILE
+        const long long t1 = clock64();
+        o.cyc_move = (uint32_t)(t1 - t0);
+        t0 = t1;
+#endif
+    }
+    if ((int32_t)(limit - j) < (int32_t)need) {
+        const uint32_t r = lds_acq_u32(ctrl + 4u);
+        limit = ((int32_t)(r - ord_end) > 0) ? ord_end : r;
+        if ((int32_t)(limit - j) < (int32_t)need) o.flags |= 1u;
+#ifdef CCD_PROFILE
+        o.cyc_ref = (uint32_t)(clock64() - t0);
+#endif
+    }
+    o.d_lo = (uint32_t)D;
+    o.d_hi = (uint32_t)(D >> 32);
+    o.r_lo = (uint32_t)R;
+    o.r_hi = (uint32_t)(R >> 32);
+    o.j = j;
+    o.wpos = wpos;
+    o.wbase = wbase;
+    o.wcur = wcur;
+    o.limit = limit;
     return o;
 }
+
+#ifdef CCD_PROFILE
+// per-grid breakdown of the coder warp's cycles (instrumented build; printed by lane 0 at the end of each grid)
+struct CoderProf {
+    long long steady = 0, rare = 0, rare_one = 0, fail = 0, move = 0, ref = 0, wait = 0, one = 0, single = 0;
+    uint32_t n_steady = 0, n_one_ok = 0, n_fail = 0, n_move = 0, n_ref = 0, n_wait = 0, n_one = 0, n_single = 0, n_pre = 0;
+};
+#endif
 
 __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout &sm, const float *__restrict__ scale_tab,
                                                 int lane, uint32_t ord_begin, uint32_t ord_end, DecState &c,
@@ -896,12 +985,15 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
     // the mode: value = 0x40 | the lane's number (its three digits)
     const uint32_t CR = (1u << 10) | 0x200u | 0x40u | (uint32_t)lane;
     const uint32_t ner = (live != 0u && lane != 13) ? 1u : 0u;
+#ifdef CCD_PROFILE
+    CoderProf cp;
+#endif
     auto refresh = [&]() {
         const uint32_t r = lds_acq_u32(ready_a);
         limit = ((int32_t)(r - ord_end) > 0) ? ord_end : r;
     };
     // the words a round may shift in come from REGISTERS: lane l holds word[wbase + l]; the window moves (one global
-    // load per lane) when fewer than 8 words are left in it -- two rounds take at most 6 and look 2 ahead
+    // load per lane) when 24 or more of its words are consumed -- a round takes at most 3 and looks 2 ahead
     uint32_t wcur = c.wcur, wbase = c.wbase;
     auto move_window = [&]() {
         wbase = wpos;
@@ -917,7 +1009,7 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         if (fl & 2u) c.slow++;
         if (fl & 4u) c.err = CCD_ERR_DESYNC;
 #ifdef CCD_PROFILE
-        c.n_far++;
+        if (fl & 8u) c.n_far++;
 #endif
     };
     if (lane == 0) sts_v2(rec_a + 16u, make_uint2(0u, 0xffffffffu));
@@ -948,16 +1040,19 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         X##a2 = lds_u32(hb2 + so_), X##b2 = lds_u32(hb2 + so_ + 4u);                                                  \
         X##a3 = lds_u32(hb3 + so_), X##b3 = lds_u32(hb3 + so_ + 4u);                                                  \
     }
-// one round on set X; failed != 0 afterwards when no sequence matched (state advanced over the decided prefix)
+// one round on set X, then its straight-line result: a matched round's state from the record (selects: a round that
+// did not match leaves D, R, wpos and j as they were), `done`, the next words.  rare_ != 0 afterwards when the round
+// did not match, the window must move or fewer than NEED symbols past j are known to be ready; the round's prefix
+// states (ok1_ ... k2_) and miss_ stay for the rare path, in variables that both sets of intervals share.
 // (shared-memory accesses of one warp are performed in program order: the record is read back without a barrier)
-#define CCD_RSTEPS(X)                                                                                                 \
+#define CCD_ROUND(X, NEED)                                                                                            \
         uint32_t dl = (uint32_t)D, dh = (uint32_t)(D >> 32), rl = (uint32_t)R, rh = (uint32_t)(R >> 32);              \
         uint32_t ok = live, k = 0u;                                                                                   \
         CCD_SSTEP(X##a1, X##b1, w0)                                                                                   \
-        const uint32_t dl1_ = dl, dh1_ = dh, rl1_ = rl, rh1_ = rh, k1_ = k, ok1_ = ok;                                \
+        dl1_ = dl, dh1_ = dh, rl1_ = rl, rh1_ = rh, k1_ = k, ok1_ = ok;                                               \
         const uint32_t wk2_ = k ? w1 : w0;                                                                            \
         CCD_SSTEP(X##a2, X##b2, wk2_)                                                                                 \
-        const uint32_t dl2_ = dl, dh2_ = dh, rl2_ = rl, rh2_ = rh, k2_ = k, ok12_ = ok;                               \
+        dl2_ = dl, dh2_ = dh, rl2_ = rl, rh2_ = rh, k2_ = k, ok12_ = ok;                                              \
         const uint32_t wk3_ = (k & 2u) ? w2 : ((k & 1u) ? w1 : w0);                                                   \
         CCD_SSTEP(X##a3, X##b3, wk3_)                                                                                 \
         const uint32_t tag_ = j + NS;                                                                                 \
@@ -966,55 +1061,58 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         sts_v4_if(ok, rec_a, dl, dh, rl, rh);                                                                         \
         sts_v2_if(ok, rec_a + 16u, k, tag_);                                                                          \
         const uint4 rv_ = lds_v4(rec_a);                                                                              \
-        const uint2 rt_ = lds_v2(rec_a + 16u);
-// (the three macros share the names the steps define)
-#define CCD_MATCHED() (rt_.y == tag_)
-#define CCD_ACCEPT()                                                                                                  \
-    {                                                                                                                 \
-        D = ((uint64_t)rv_.y << 32) | rv_.x;                                                                          \
-        R = ((uint64_t)rv_.w << 32) | rv_.z;                                                                          \
-        wpos += rt_.x;                                                                                                \
-        j = tag_;                                                                                                     \
+        const uint2 rt_ = lds_v2(rec_a + 16u);                                                                        \
+        miss_ = rt_.y != tag_ ? 1u : 0u;                                                                              \
+        D = miss_ ? D : (((uint64_t)rv_.y << 32) | rv_.x);                                                            \
+        R = miss_ ? R : (((uint64_t)rv_.w << 32) | rv_.z);                                                            \
+        wpos += miss_ ? 0u : rt_.x;                                                                                   \
+        j = miss_ ? j : tag_;                                                                                         \
         sts_done(done_a, j);                                                                                          \
         load_words();                                                                                                 \
-        PROF_COUNT_OK();                                                                                              \
-    }
-// no sequence matched: the decided prefix, then the symbol outside {M-1, M, M+1} through tier 2
-#define CCD_FAILED()                                                                                                  \
-    {                                                                                                                 \
-        const PrefixOut po_ = spec_prefix(sm.res, ring_mask, lane, j, ok1_, ok12_, ((uint64_t)dh1_ << 32) | dl1_,     \
-                                          ((uint64_t)rh1_ << 32) | rl1_, k1_, ((uint64_t)dh2_ << 32) | dl2_,          \
-                                          ((uint64_t)rh2_ << 32) | rl2_, k2_);                                        \
-        if (po_.n) {                                                                                                  \
-            D = ((uint64_t)po_.d_hi << 32) | po_.d_lo;                                                                \
-            R = ((uint64_t)po_.r_hi << 32) | po_.r_lo;                                                                \
-            wpos += po_.k;                                                                                            \
-            j += po_.n;                                                                                               \
-        }                                                                                                             \
-        {                                                                                                             \
-            const uint4 hh_ = lds_v4(sm.hot + (j & ring_mask) * 16u);                                                 \
-            const uint32_t wj_ = __shfl_sync(0xffffffffu, wcur, (int)(wpos - wbase));                                 \
-            const T2Out t2_ = coder_tier2_g(sm.res, sm.win, sm.meta, scale_tab, ring_mask, lane, j, hh_, D, R, wj_, wpos, \
-                                            words, wmax);                                                             \
-            D = ((uint64_t)t2_.d_hi << 32) | t2_.d_lo;                                                                \
-            R = ((uint64_t)t2_.r_hi << 32) | t2_.r_lo;                                                                \
-            wpos = t2_.wpos;                                                                                          \
-            if (t2_.flags != 0u) note_flags(t2_.flags);                                                               \
-        }                                                                                                             \
-        j++;                                                                                                          \
-        sts_done(done_a, j);                                                                                          \
-        if (wpos - wbase >= 24u) move_window();                                                                       \
+        rare_ = miss_ | (wpos - wbase >= 24u ? 1u : 0u) | ((int32_t)(limit - j) < (int32_t)(NEED) ? 1u : 0u);
+// the rare path of the last round; leave_ != 0 afterwards: fewer than NEED symbols ready
+#define CCD_RARE(NEED, ACC)                                                                                              \
+        PROF_T(tr_);                                                                                                  \
+        const RareOut ro_ = coder_rare(sm.ctrl, sm.hot, sm.res, sm.win, sm.meta, scale_tab, ring_mask, lane, (NEED),  \
+                                       miss_, ok1_, ok12_, ((uint64_t)dh1_ << 32) | dl1_, ((uint64_t)rh1_ << 32) | rl1_, \
+                                       k1_, ((uint64_t)dh2_ << 32) | dl2_, ((uint64_t)rh2_ << 32) | rl2_, k2_, D, R, j,   \
+                                       wpos, wbase, wcur, limit, ord_end, words, wmax);                               \
+        D = ((uint64_t)ro_.d_hi << 32) | ro_.d_lo;                                                                    \
+        R = ((uint64_t)ro_.r_hi << 32) | ro_.r_lo;                                                                    \
+        j = ro_.j;                                                                                                    \
+        wpos = ro_.wpos;                                                                                              \
+        wbase = ro_.wbase;                                                                                            \
+        wcur = ro_.wcur;                                                                                              \
+        limit = ro_.limit;                                                                                            \
+        if (ro_.flags & ~1u) note_flags(ro_.flags);                                                                   \
         load_words();                                                                                                 \
-        PROF_COUNT_FAIL(po_.n);                                                                                       \
-    }
+        PROF_RARE(tr_, ACC);                                                                                          \
+        const uint32_t leave_ = ro_.flags & 1u;
 #ifdef CCD_PROFILE
-#define PROF_COUNT_FAIL(N) do { pc.seg[3] += (N); c.n_redo++; } while (0)
-#define PROF_COUNT_OK() do { pc.seg[3] += NS; } while (0)
+#define PROF_RARE(T0, ACC)                                                                                            \
+    do {                                                                                                              \
+        ACC += clock64() - (T0);                                                                                      \
+        cp.fail += ro_.cyc_fail;                                                                                      \
+        cp.move += ro_.cyc_move;                                                                                      \
+        cp.ref += ro_.cyc_ref;                                                                                        \
+        cp.n_fail += miss_;                                                                                           \
+        cp.n_move += ro_.cyc_move != 0u;                                                                              \
+        cp.n_ref += ro_.cyc_ref != 0u;                                                                                \
+        cp.n_pre += ro_.n_pre;                                                                                        \
+        c.n_redo += miss_;                                                                                            \
+        pc.seg[3] += ro_.n_pre;                                                                                       \
+    } while (0)
+#define PROF_ROUND(N)                                                                                                 \
+    do {                                                                                                              \
+        N += 1u - miss_;                                                                                              \
+        pc.seg[3] += miss_ ? 0u : NS;                                                                                 \
+    } while (0)
 #else
-#define PROF_COUNT_FAIL(N)
-#define PROF_COUNT_OK()
+#define PROF_RARE(T0, ACC)
+#define PROF_ROUND(N)
 #endif
     uint32_t pa1, pb1, pa2, pb2, pa3, pb3, qa1, qb1, qa2, qb2, qa3, qb3;  // two sets of candidate intervals
+    uint32_t dl1_, dh1_, rl1_, rh1_, k1_, ok1_, dl2_, dh2_, rl2_, rh2_, k2_, ok12_, miss_, rare_;  // the last round's
     while (j != ord_end) {
         if ((int32_t)(limit - j) <= 0) {
             PROF_T(t0);
@@ -1022,9 +1120,14 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
                 refresh();
             } while ((int32_t)(limit - j) <= 0);
             PROF_ADD(pc.wait, t0);
+#ifdef CCD_PROFILE
+            cp.wait += clock64() - t0;
+            cp.n_wait++;
+#endif
         }
         if ((int32_t)(limit - j) < (int32_t)NS) {
             // one symbol: tier-1 test, tier 2 through the function (short diagonals)
+            PROF_T(t1);
             const uint4 hh = lds_v4(sm.hot + (j & ring_mask) * 16u);
             {
                 const uint64_t scale_ = R >> 24;
@@ -1047,6 +1150,8 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
             sts_done(done_a, j);
 #ifdef CCD_PROFILE
             pc.seg[4]++;
+            cp.single += clock64() - t1;
+            cp.n_single++;
 #endif
             continue;
         }
@@ -1055,52 +1160,70 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         CCD_SLOAD(p, j)
         if ((int32_t)(limit - j) < (int32_t)(3u * NS)) {
             // fewer symbols ready than the steady loop wants: one round
-            CCD_RSTEPS(p)
-            if (CCD_MATCHED()) CCD_ACCEPT() else CCD_FAILED()
+            PROF_T(t1);
+            {
+                CCD_ROUND(p, 0u)
+            }
+            PROF_ROUND(cp.n_one_ok);
+            if (miss_) {
+                CCD_RARE(0u, cp.rare_one)
+                (void)leave_;
+            }
+#ifdef CCD_PROFILE
+            cp.one += clock64() - t1;
+            cp.n_one++;
+#endif
             continue;
         }
         // ---- steady state: two rounds per iteration, the two sets of intervals swapping roles (no copies); the
-        // intervals of the next round are requested before the steps of the current one.  The common path is the
-        // fall-through all the way to the back-edge (a taken branch costs this warp 10 ... 40 cycles).
+        // intervals of the next round are requested before the steps of the current one.  Each round needs 2 NS symbols
+        // ready past its j: its own intervals and those of the next round.  A matched round is straight-line code: its
+        // one conditional leaves the inner loop for the rare path, and the iteration's one taken branch is the back-edge
+        // (a taken branch costs this warp 10 ... 40 cycles; tools/sass_coder_path.py checks the SASS).  The rare test is
+        // a vote: a warp-uniform branch needs no reconvergence region, which would keep the rare path in line.  After
+        // the rare path the loop starts again at the round j.
+        PROF_T(ts);
         while (true) {
-            if (((int32_t)(limit - j) < (int32_t)(3u * NS)) | (wpos - wbase >= 24u)) {  // (two rare cases, one test)
-                if (wpos - wbase >= 24u) {
-                    move_window();
-                    load_words();
+            while (true) {
+                CCD_SLOAD(q, j + NS)
+                {
+                    CCD_ROUND(p, 2u * NS)
                 }
-                if ((int32_t)(limit - j) < (int32_t)(3u * NS)) {
-                    refresh();
-                    if ((int32_t)(limit - j) < (int32_t)(3u * NS)) break;
+                PROF_ROUND(cp.n_steady);
+                if (__builtin_expect(__any_sync(0xffffffffu, rare_ != 0u), 0)) break;
+                CCD_SLOAD(p, j + NS)
+                {
+                    CCD_ROUND(q, 2u * NS)
                 }
+                PROF_ROUND(cp.n_steady);
+                if (__builtin_expect(__any_sync(0xffffffffu, rare_ != 0u), 0)) break;
             }
-            CCD_SLOAD(q, j + NS)
-            {
-                CCD_RSTEPS(p)
-                if (__builtin_expect(CCD_MATCHED(), 1)) {
-                    CCD_ACCEPT()
-                    CCD_SLOAD(p, j + NS)
-                    {
-                        CCD_RSTEPS(q)
-                        if (__builtin_expect(CCD_MATCHED(), 1)) {
-                            CCD_ACCEPT()
-                            continue;
-                        }
-                        CCD_FAILED()
-                        CCD_SLOAD(p, j)
-                        continue;
-                    }
-                }
-                CCD_FAILED()
-                CCD_SLOAD(p, j)
-            }
+            CCD_RARE(2u * NS, cp.rare)
+            if (leave_) break;
+            CCD_SLOAD(p, j)
         }
+#ifdef CCD_PROFILE
+        cp.steady += clock64() - ts;
+#endif
     }
 #undef CCD_SSTEP
 #undef CCD_SLOAD
-#undef CCD_RSTEPS
-#undef CCD_MATCHED
-#undef CCD_ACCEPT
-#undef CCD_FAILED
+#undef CCD_ROUND
+#undef CCD_RARE
+#undef PROF_RARE
+#undef PROF_ROUND
+#ifdef CCD_PROFILE
+    // one line per grid (tools/gpu_1080.py tabulates them): symbols, then cycles / count of matched steady rounds
+    // (the steady loop less its rare path), failed rounds (all of them, with the symbols of their decided prefixes),
+    // window moves and refreshes of the rare path, waits of the outer loop, one-round steps (matched ones counted
+    // apart) and single-symbol steps, and the rare path's total in the steady loop (call and reloads included)
+    if (lane == 0)
+        printf("CCDPROF grid_begin %u n %u steady %lld %u fail %lld %u pre %u move %lld %u ref %lld %u wait %lld %u "
+               "one %lld %u %u single %lld %u rare %lld\n",
+               ord_begin, ord_end - ord_begin, cp.steady - cp.rare, cp.n_steady, cp.fail, cp.n_fail, cp.n_pre, cp.move,
+               cp.n_move, cp.ref, cp.n_ref, cp.wait, cp.n_wait, cp.one, cp.n_one, cp.n_one_ok, cp.single, cp.n_single,
+               cp.rare);
+#endif
     c.D = D;
     c.R = R;
     c.w0 = w0;

@@ -1,5 +1,9 @@
-"""Development tool: 1080p synthetic stream: timings + entropy-kernel status / profile counters."""
-import os, sys, time
+"""Development tool: 1080p synthetic stream: timings + entropy-kernel status / profile counters.
+
+With the instrumented library (CCD_LIB=cool-chic_b200/csrc/libccdec_prof.so, `make prof`) it also tabulates the coder
+warp's per-grid breakdown, which the kernel prints once per grid (CCDPROF lines): cycles and counts of matched steady
+rounds, failed rounds, window moves, refreshes, waits, one-round and single-symbol steps."""
+import os, re, sys, tempfile, time
 import numpy as np, torch
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
@@ -21,12 +25,60 @@ h2 = type(h)(); rest = h2.read_header(cc); d = desc_from_header(h2)
 nnb = rest[:h2.get_value("nn_n_bytes")]; lb = rest[h2.get_value("nn_n_bytes"):][:h2.get_value("n_bytes_latent")]
 nn = _native.decode_nn(d, nnb)
 print("symbols", d.n_symbols(), "payload", len(lb), "bpp %.3f" % (len(lb) * 8 / (1080 * 1920)))
+
+
+def decode_capturing():
+    """one decode with the process's C-level stdout (where device printf lands) captured; returns (latents, text)"""
+    sys.stdout.flush()
+    saved = os.dup(1)
+    with tempfile.TemporaryFile(mode="w+b") as f:
+        os.dup2(f.fileno(), 1)
+        try:
+            o = ctx.decode_latents(d, nn, lb); torch.cuda.synchronize()
+        finally:
+            sys.stdout.flush()
+            os.dup2(saved, 1)
+            os.close(saved)
+        f.seek(0)
+        return o, f.read().decode(errors="replace")
+
+
+def prof_table(text):
+    rows = []
+    for line in text.splitlines():
+        if line.startswith("CCDPROF"):
+            v = [int(x) for x in re.findall(r"-?\d+", line)]
+            rows.append(dict(zip(("ord", "n", "st_c", "st_n", "fa_c", "fa_n", "pre", "mv_c", "mv_n", "rf_c", "rf_n", "wt_c",
+                                  "wt_n", "one_c", "one_n", "one_ok", "sg_c", "sg_n", "rare_c"), v)))
+    if not rows:
+        return
+    print("coder warp per grid (decode order; kcyc = kilo-cycles; cyc/x = cycles per round / case):")
+    print("%6s %9s | %9s %8s %6s | %8s %6s %6s | %6s %5s | %7s %6s | %7s %6s | %7s %6s %7s | %7s %6s | %8s"
+          % ("grid", "symbols", "matched", "rounds", "cyc/r", "fail", "n", "cyc/f", "move", "n", "refresh", "n", "wait",
+             "n", "1-round", "n", "matched", "single", "n", "rare"))
+    tot = dict.fromkeys(rows[0], 0)
+    for i, r in enumerate(rows):
+        for k_ in r:
+            tot[k_] += r[k_]
+    for name, r in [(str(i), r) for i, r in enumerate(rows)] + [("all", tot)]:
+        print("%6s %9d | %9.1f %8d %6.1f | %8.1f %6d %6.0f | %6.1f %5d | %7.1f %6d | %7.1f %6d | %7.1f %6d %7d | %7.1f %6d | %8.1f"
+              % (name, r["n"], r["st_c"] / 1e3, r["st_n"], r["st_c"] / max(1, r["st_n"]), r["fa_c"] / 1e3, r["fa_n"],
+                 r["fa_c"] / max(1, r["fa_n"]), r["mv_c"] / 1e3, r["mv_n"], r["rf_c"] / 1e3, r["rf_n"], r["wt_c"] / 1e3,
+                 r["wt_n"], r["one_c"] / 1e3, r["one_n"], r["one_ok"], r["sg_c"] / 1e3, r["sg_n"], r["rare_c"] / 1e3))
+    print("  matched: the steady loop less its rare path; fail / move / refresh: the three parts of the rare path "
+          "(inside the call); rare: the steady loop's rare path in all (call, argument moves and reloads)")
+
+
 for it in range(3):
-    out = ctx.decode_latents(d, nn, lb); torch.cuda.synchronize()
+    if it == 2:
+        out, text = decode_capturing()
+    else:
+        out = ctx.decode_latents(d, nn, lb); torch.cuda.synchronize()
     st = ctx.last_status()
     print(ctx.last_timing(), st[:4])
     if any(st[4:]):
         print("  prof kcyc: coder wait %d total %d | producers wait %d arm %d win %d total %d | far %d redo-groups %d singles %d fast %d chunks %d | helper total %d" % tuple(st[4:16]))
+prof_table(text)
 print("round trip ok:", torch.equal(out, lat))
 l = lat.cpu().numpy().astype(int); off = 0
 for g in range(d.n_grids - 1, -1, -1):

@@ -59,6 +59,7 @@ __device__ __forceinline__ uint32_t step_cmp_rn(uint64_t &D, uint64_t &R, uint4 
     t = c2 ? 15u : (c1 ? 14u : 13u);
     return far;
 }
+// V6: V0 with a taken branch per block of K steps (in k below)
 // V5: mode first with ONE select level: R' = mode ? Q1 : Qx where Qx = (D < P1) ? Q0 : Q2 is formed off the mode chain
 __device__ __forceinline__ uint32_t step_mode_first(uint64_t &D, uint64_t &R, uint4 h, uint32_t &t) {
     const uint64_t s = R >> 24;
@@ -110,7 +111,7 @@ __global__ void k(long long *out, int n, int noise) {
 #pragma unroll
         for (int i = 0; i < K; i++) {
             uint32_t t = 14u;
-            if (VAR == 0 || VAR == 1) bad |= step_mode(D, R, a[i]);
+            if (VAR == 0 || VAR == 1 || VAR == 6) bad |= step_mode(D, R, a[i]);
             else if (VAR == 2) bad |= step_cmp(D, R, a[i], t);
             else if (VAR == 3) bad |= step_diff(D, R, a[i], t);
             else if (VAR == 4) bad |= step_cmp_rn(D, R, a[i], t, 0x12345678u, wpos);
@@ -119,6 +120,16 @@ __global__ void k(long long *out, int n, int noise) {
         }
         if (VAR == 1) { if (bad) { bad_all++; D ^= 1; } }          // fresh predicate
         else { if (badp) { bad_all++; D ^= 1; } }                 // verified one group late
+        if (VAR == 6) {
+            // a block on fresh data that is never entered, too long to predicate: ptxas places it in line, so the branch
+            // around it is taken once per block; V6 - V0 = the cost of one taken branch to this warp
+            if ((uint32_t)(D >> 8) == 0x12345u) {
+                uint32_t x = (uint32_t)R;
+#pragma unroll
+                for (int q = 0; q < 24; q++) x = x * 1664525u + (uint32_t)(D >> q);
+                bad_all += x;
+            }
+        }
         badp = bad;
         tsum += tt;
         sts(ctrl + 8, j);
@@ -152,6 +163,8 @@ int main() {
     run<1, 4>("mode only, fresh check", d_out);
     run<0, 2>("mode only, lagged check", d_out);
     run<0, 8>("mode only, lagged check", d_out);
+    run<6, 4>("mode only, taken branch per block", d_out);
+    run<6, 2>("mode only, taken branch per block", d_out);
     run<2, 4>("3 cand, compare + 2-level select", d_out);
     run<3, 4>("3 cand, differences", d_out);
     run<4, 4>("3 cand, compare + renorm selects", d_out);

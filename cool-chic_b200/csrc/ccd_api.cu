@@ -77,6 +77,14 @@ int validate_desc(const CcdCoolChicDesc *d) {
         if (d->flag_ifce && d->grid_ifce_in[g] > 0 && d->grid_ifce_in[g] != std::max(d->n_grids - 1 - g, 1))
             return fail(CCD_ERR_ARG, "grid %d: ifce_in=%d inconsistent", g, d->grid_ifce_in[g]);
     }
+    // The IFCE reads grid g + 1 at (y >> 1, x >> 1) of grid g, and each coarser grid through one nearest x2 step per
+    // change of size (core/upsampling.py:575-593): a grid less than half the size of the next finer one (latent and
+    // hyperlatent resolutions with a gap between them, which the reference cannot decode either) would be read
+    // outside its bounds.
+    for (int g = 0; d->flag_ifce && g + 1 < d->n_grids; g++)
+        if (2 * d->grid_h[g + 1] < d->grid_h[g] || 2 * d->grid_w[g + 1] < d->grid_w[g])
+            return fail(CCD_ERR_ARG, "grid %d (%dx%d) is less than half of grid %d (%dx%d): the IFCE cannot read it",
+                        g + 1, d->grid_h[g + 1], d->grid_w[g + 1], g, d->grid_h[g], d->grid_w[g]);
     for (int i = 0; i < 8; i++) {
         if (d->expgol[i] < 0 || d->expgol[i] > 12) return fail(CCD_ERR_ARG, "exp-Golomb order out of range");
         if (d->qshift[i] > 0 || d->qshift[i] < -24) return fail(CCD_ERR_ARG, "q_step out of range");

@@ -581,6 +581,10 @@ static int code_all_grids(const CcoDesc *d, const int64_t *nn, Coder *cd, int8_t
     if (rc) return rc;
     int dim = L.dim;
     if (dim < 1 || dim > 71) return CCO_ERR_ARG;
+    /* the IFCE context plane of grid g has grid g+1's size and is read at (y >> 1, x >> 1): a grid less than half
+     * the next finer one (a gap between the latent and hyperlatent resolutions) cannot be read */
+    for (int g = 0; d->flag_ifce && g + 1 < d->n_grids; g++)
+        if (2 * d->grid_h[g + 1] < d->grid_h[g] || 2 * d->grid_w[g + 1] < d->grid_w[g]) return CCO_ERR_ARG;
     ArmFP arm;
     ArmFP ifce[CCO_MAX_GRIDS];
     memset(ifce, 0, sizeof(ifce));

@@ -47,8 +47,25 @@ def _fixed_point(q, b, s_w, s_b, ifce_cols, residual, subtract_last=False):
     return W, B * (1 << (32 + s_b))
 
 
-def model_indices(d, nn, latents):
-    """(mu_idx, sc_idx) of every symbol (decode order) after the clamp of latent.py:165 / rangecoder.py:89-91."""
+def mac(B, x, W):
+    """B + x @ W in int64, after proving that no partial sum can wrap: |B| + |x| @ |W| in float64 (relative error
+    below 2^-40 at these sizes) stays under 2^62.  A wrap would go unnoticed, on the device as here."""
+    bound = np.abs(B).astype(np.float64) + np.abs(x).astype(np.float64) @ np.abs(W).astype(np.float64)
+    assert bound.size == 0 or bound.max() < 2.0**62, f"an ARM / IFCE sum reaches {bound.max():.3g}"
+    return B + x @ W
+
+
+# negative controls of the checker (tests/test_arm_space.py), each outside the ARMs the older fixtures have:
+#   ctx_swap         spatial contexts 24 and 25 read each other's neighbour
+#   ifce_grid        IFCE channels 12 and up read the grid one finer than theirs
+#   linear_identity  an ARM without hidden layer evaluated through one identity layer (a ReLU of its inputs)
+#   residual_drop    hidden layers from the third on lose their residual connection
+CHECKER_BUGS = ("ctx_swap", "ifce_grid", "linear_identity", "residual_drop")
+
+
+def model_indices(d, nn, latents, bug=None):
+    """(mu_idx, sc_idx) of every symbol (decode order) after the clamp of latent.py:165 / rangecoder.py:89-91.
+    ``bug``: one of CHECKER_BUGS (a negative control), or None."""
     from coolchic_b200 import synth
 
     sec = synth.split_nn(d, nn)
@@ -58,7 +75,13 @@ def model_indices(d, nn, latents):
     ifce_cols = np.arange(dim) >= dim - cf if cf else np.zeros(dim, dtype=bool)
     aw, ab = sec["arm.weight"], sec["arm.bias"]
     layers = [_fixed_point(aw[f"mlp.{2 * l}"], ab[f"mlp.{2 * l}"], s_w, s_b,
-                           ifce_cols if l == 0 else np.zeros(dim, dtype=bool), True, l == H) for l in range(H + 1)]
+                           ifce_cols if l == 0 else np.zeros(dim, dtype=bool), not (bug == "residual_drop" and l >= 2),
+                           l == H) for l in range(H + 1)]
+    if bug == "linear_identity" and H == 0:
+        layers.insert(0, (np.eye(dim, dtype=np.int64) << 16, np.zeros(dim, np.int64)))
+    dy, dx = list(CTX_DY), list(CTX_DX)
+    if bug == "ctx_swap":
+        dy[24], dy[25], dx[24], dx[25] = dy[25], dy[24], dx[25], dx[24]
     if d.arm_stab:
         Ws, Bs = _fixed_point(aw["stab"], ab["stab"], s_w, s_b, ifce_cols, False)
     else:
@@ -72,7 +95,7 @@ def model_indices(d, nn, latents):
         X = np.zeros((h, w, dim), np.int64)
         P = np.pad(grids[g], ((4, 0), (4, 4)))
         for t in range(d.n_ctx):
-            X[:, :, t] = P[4 + CTX_DY[t]:4 + CTX_DY[t] + h, 4 + CTX_DX[t]:4 + CTX_DX[t] + w]
+            X[:, :, t] = P[4 + dy[t]:4 + dy[t] + h, 4 + dx[t]:4 + dx[t] + w]
         n_in = int(d.grid_ifce_in[g]) if cf else 0
         if n_in:
             # IFCE features at (y >> 1, x >> 1) from the coarser grids g+1+c, each read at >> sh[c] (coolchic.py:95-146)
@@ -85,14 +108,18 @@ def model_indices(d, nn, latents):
                 for c in range(n_in):
                     if c > 0 and (d.grid_h[g + c], d.grid_w[g + c]) != (d.grid_h[g + 1 + c], d.grid_w[g + 1 + c]):
                         sh += 1
+                    if bug == "ifce_grid" and c >= 12:
+                        G = grids[g + c]
+                        V[:, :, c] = G[(yy >> sh)[:, None] % G.shape[0], (xx >> sh)[None, :] % G.shape[1]]
+                        continue
                     V[:, :, c] = grids[g + 1 + c][(yy >> sh)[:, None], (xx >> sh)[None, :]]
-            acc = Bi + (V << 16) @ Wi
+            acc = mac(Bi, V << 16, Wi)
             X[:, :, d.n_ctx:] = (acc >> 24).astype(np.float32).astype(np.int64)  # fp32 round trip
         x = X.reshape(h * w, dim) << 16
-        s = Bs + x @ Ws
+        s = mac(Bs, x, Ws)
         for W, B in layers[:-1]:
-            x = np.maximum(B + x @ W, 0) >> 16
-        o = (layers[-1][1] + x @ layers[-1][0] + s) >> 24
+            x = np.maximum(mac(B, x, W), 0) >> 16
+        o = (mac(layers[-1][1], x, layers[-1][0]) + s) >> 24
         sl = slice(offs[g], offs[g] + h * w)
         mu_idx[sl] = np.clip(o[:, 0] + 16384, 0, 32767)
         sc_idx[sl] = np.clip(o[:, 1] + 1280, 0, 2560)

@@ -727,26 +727,34 @@ __device__ __forceinline__ uint32_t res_tag(uint32_t j) { return ((j + 1u) << 10
 // ---------------------------------------------------------------------------------------------------------------
 // Exact path of one symbol that is not M-1 / M / M+1: the whole 32-entry window at once (lane per entry:
 // one conflict-free LDS, one product, one vote -- the cost does not depend on how far from the mode the
-// symbol is), then the exact f64 model (warp-cooperative) outside the window.  Out of line, by value.
+// symbol is), then the exact f64 model (warp-cooperative) outside the window.  The window test is in line in its
+// callers; only the exact model is out of line, by value.
 struct FarOut {
     uint64_t lo, hi;  // scale * left(sym), scale * left(sym + 1)
     uint32_t rw;      // result word (without the tag)
     uint32_t flags;   // 2: outside the window (exact search), 4: desynchronised
 };
-__device__ __noinline__ FarOut coder_far(uint32_t wrow, uint32_t meta_slot, const float *__restrict__ scale_tab, int lane,
-                                         uint64_t scale, uint64_t D) {
-    FarOut o;
-    o.flags = 0;
-    const uint32_t Lt = lds_u32(wrow + 4u * (uint32_t)lane);
+__device__ __noinline__ FarOut coder_exact(uint32_t meta_slot, const float *__restrict__ scale_tab, int lane,
+                                           uint64_t scale, uint64_t D);
+// Lt = this lane's window entry left(s_lo + lane) of the symbol
+__device__ __forceinline__ FarOut coder_far(uint32_t Lt, uint32_t meta_slot, const float *__restrict__ scale_tab, int lane,
+                                            uint64_t scale, uint64_t D) {
     const uint32_t b = __ballot_sync(0xffffffffu, scale * Lt <= D);  // lefts are non-decreasing: bits 0..t
     if (b != 0u && b != 0xffffffffu) {
+        FarOut o;
         const int t = 31 - __clz((int)b);
         o.lo = scale * (uint64_t)__shfl_sync(0xffffffffu, Lt, t);
         o.hi = scale * (uint64_t)__shfl_sync(0xffffffffu, Lt, t + 1);
         o.rw = (uint32_t)t;
+        o.flags = 0u;
         return o;
     }
-    // outside the window, or corrupt stream
+    return coder_exact(meta_slot, scale_tab, lane, scale, D);
+}
+// outside the window, or corrupt stream
+__device__ __noinline__ FarOut coder_exact(uint32_t meta_slot, const float *__restrict__ scale_tab, int lane,
+                                           uint64_t scale, uint64_t D) {
+    FarOut o;
     o.flags = 2;
     uint64_t q = D / scale;
     if (q >= (1ull << 24)) {
@@ -798,8 +806,8 @@ __device__ __forceinline__ uint2 lds_v2(uint32_t a) {
 }
 
 // TIER 2 of one symbol j: M-1 / M / M+1 by selects, the far path (coder_far) otherwise, renormalisation with the word
-// w0 = word[wpos] shifted in; the symbol's result word is written unless it is the mode.  Inline in both of its
-// callers below, which are out of line themselves.
+// w0 = word[wpos] shifted in; the symbol's result word is written unless it is the mode.  Inline in its caller below,
+// which is out of line itself.
 struct T2Step {
     uint64_t D, R;
     uint32_t renorm;  // 1: the step shifted w0 in
@@ -822,7 +830,8 @@ __device__ __forceinline__ T2Step tier2_step(uint32_t res_a, uint32_t win_a, uin
     o.flags = 0u;
     if (Dn >= Rn) {
         const uint32_t slot = j & ring_mask;
-        const FarOut f = coder_far(win_a + slot * (CCD_WIN * 4), meta_a + slot * 16u, scale_tab, lane, scale, D);
+        const uint32_t Lt = lds_u32(win_a + slot * (CCD_WIN * 4) + 4u * (uint32_t)lane);
+        const FarOut f = coder_far(Lt, meta_a + slot * 16u, scale_tab, lane, scale, D);
         Dn = D - f.lo;
         Rn = f.hi - f.lo;
         rw = f.rw;
@@ -865,103 +874,12 @@ __device__ __noinline__ T2Out coder_tier2_g(uint32_t res_a, uint32_t win_a, uint
     return r;
 }
 
-// THE RARE PATH of a speculative round, one out-of-line call (DESIGN §4.1).  The round's caller accepts a matched round
-// with selects and tests one predicate: the round did not match, or the word window must move, or fewer than `need`
-// symbols past j are known to be ready.  Under it, this function does all three, in that order:
-//   * a failed round: the longest decided prefix (0, 1 or 2 symbols) is taken from a lane that matched it -- its state
-//     after that prefix, its result words -- and the next symbol goes through tier 2; `done` is published;
-//   * the window move: lane l loads word[wpos + l];
-//   * the refresh of `limit` from `ready`; still fewer than `need` ready: the caller leaves the steady loop (flag 1).
-// Everything in and out by value (registers).  The caller reloads the words of the window and the round's intervals.
-struct RareOut {
-    uint32_t d_lo, d_hi, r_lo, r_hi, j, wpos, wbase, wcur, limit;
-    uint32_t flags;  // 1: leave the steady loop, otherwise as T2Step::flags
-#ifdef CCD_PROFILE
-    uint32_t n_pre, cyc_fail, cyc_move, cyc_ref;  // decided prefix; cycles of the three parts
-#endif
-};
-__device__ __noinline__ RareOut coder_rare(uint32_t ctrl, uint32_t hot, uint32_t res, uint32_t win, uint32_t meta,
-                                           const float *__restrict__ scale_tab, uint32_t ring_mask, int lane, uint32_t need,
-                                           uint32_t miss, uint32_t ok1, uint32_t ok12, uint64_t d1, uint64_t r1, uint32_t k1,
-                                           uint64_t d2, uint64_t r2, uint32_t k2, uint64_t D, uint64_t R, uint32_t j,
-                                           uint32_t wpos, uint32_t wbase, uint32_t wcur, uint32_t limit, uint32_t ord_end,
-                                           const uint32_t *__restrict__ words, uint32_t wmax) {
-    RareOut o;
-    o.flags = 0u;
-#ifdef CCD_PROFILE
-    o.n_pre = o.cyc_fail = o.cyc_move = o.cyc_ref = 0u;
-    long long t0 = clock64();
-#endif
-    if (miss) {
-        const uint32_t b1 = __ballot_sync(0xffffffffu, ok1 != 0u), b2 = __ballot_sync(0xffffffffu, ok12 != 0u);
-        const uint32_t n = b2 ? 2u : (b1 ? 1u : 0u);
-        if (n) {
-            const int src = __ffs((int)(b2 ? b2 : b1)) - 1;
-            const uint64_t ds = b2 ? d2 : d1, rs = b2 ? r2 : r1;
-            D = ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(ds >> 32), src) << 32) |
-                __shfl_sync(0xffffffffu, (uint32_t)ds, src);
-            R = ((uint64_t)__shfl_sync(0xffffffffu, (uint32_t)(rs >> 32), src) << 32) |
-                __shfl_sync(0xffffffffu, (uint32_t)rs, src);
-            wpos += __shfl_sync(0xffffffffu, b2 ? k2 : k1, src);
-            const uint32_t q1 = (uint32_t)src % 3u, q2 = ((uint32_t)src / 3u) % 3u;
-            if (lane == 0) {
-                if (q1 != 1u) sts_u32(res + (j & ring_mask) * 4u, res_tag(j) | (CCD_WIN_HALF - 1u + q1));
-                if (n == 2u && q2 != 1u)
-                    sts_u32(res + ((j + 1u) & ring_mask) * 4u, res_tag(j + 1u) | (CCD_WIN_HALF - 1u + q2));
-            }
-            __syncwarp();
-            j += n;
-        }
-        const uint4 h = lds_v4(hot + (j & ring_mask) * 16u);
-        const uint32_t wj = __shfl_sync(0xffffffffu, wcur, (int)(wpos - wbase));
-        const T2Step s = tier2_step(res, win, meta, scale_tab, ring_mask, lane, j, h, D, R, wj);
-        D = s.D;
-        R = s.R;
-        wpos += s.renorm;
-        o.flags = s.flags;
-        j++;
-        sts_done(ctrl + 8u, j);
-#ifdef CCD_PROFILE
-        o.n_pre = n;
-        const long long t1 = clock64();
-        o.cyc_fail = (uint32_t)(t1 - t0);
-        t0 = t1;
-#endif
-    }
-    if (wpos - wbase >= 24u) {
-        wbase = wpos;
-        wcur = coder_word(words, wmax, wbase + (uint32_t)lane);
-#ifdef CCD_PROFILE
-        const long long t1 = clock64();
-        o.cyc_move = (uint32_t)(t1 - t0);
-        t0 = t1;
-#endif
-    }
-    if ((int32_t)(limit - j) < (int32_t)need) {
-        const uint32_t r = lds_acq_u32(ctrl + 4u);
-        limit = ((int32_t)(r - ord_end) > 0) ? ord_end : r;
-        if ((int32_t)(limit - j) < (int32_t)need) o.flags |= 1u;
-#ifdef CCD_PROFILE
-        o.cyc_ref = (uint32_t)(clock64() - t0);
-#endif
-    }
-    o.d_lo = (uint32_t)D;
-    o.d_hi = (uint32_t)(D >> 32);
-    o.r_lo = (uint32_t)R;
-    o.r_hi = (uint32_t)(R >> 32);
-    o.j = j;
-    o.wpos = wpos;
-    o.wbase = wbase;
-    o.wcur = wcur;
-    o.limit = limit;
-    return o;
-}
-
 #ifdef CCD_PROFILE
 // per-grid breakdown of the coder warp's cycles (instrumented build; printed by lane 0 at the end of each grid)
 struct CoderProf {
-    long long steady = 0, rare = 0, rare_one = 0, fail = 0, move = 0, ref = 0, wait = 0, one = 0, single = 0;
-    uint32_t n_steady = 0, n_one_ok = 0, n_fail = 0, n_move = 0, n_ref = 0, n_wait = 0, n_one = 0, n_single = 0, n_pre = 0;
+    long long steady = 0, rare = 0, fail = 0, wait = 0, one = 0, single = 0;
+    uint32_t n_steady = 0, n_one_ok = 0, n_fail = 0, n_pre = 0, n_move = 0, n_ref = 0, n_starve = 0, n_wait = 0, n_one = 0,
+             n_single = 0;
 };
 #endif
 
@@ -1070,37 +988,53 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         sts_done(done_a, j);                                                                                          \
         load_words();                                                                                                 \
         rare_ = miss_ | (wpos - wbase >= 24u ? 1u : 0u) | ((int32_t)(limit - j) < (int32_t)(NEED) ? 1u : 0u);
-// the rare path of the last round; leave_ != 0 afterwards: fewer than NEED symbols ready
-#define CCD_RARE(NEED, ACC)                                                                                              \
-        PROF_T(tr_);                                                                                                  \
-        const RareOut ro_ = coder_rare(sm.ctrl, sm.hot, sm.res, sm.win, sm.meta, scale_tab, ring_mask, lane, (NEED),  \
-                                       miss_, ok1_, ok12_, ((uint64_t)dh1_ << 32) | dl1_, ((uint64_t)rh1_ << 32) | rl1_, \
-                                       k1_, ((uint64_t)dh2_ << 32) | dl2_, ((uint64_t)rh2_ << 32) | rl2_, k2_, D, R, j,   \
-                                       wpos, wbase, wcur, limit, ord_end, words, wmax);                               \
-        D = ((uint64_t)ro_.d_hi << 32) | ro_.d_lo;                                                                    \
-        R = ((uint64_t)ro_.r_hi << 32) | ro_.r_lo;                                                                    \
-        j = ro_.j;                                                                                                    \
-        wpos = ro_.wpos;                                                                                              \
-        wbase = ro_.wbase;                                                                                            \
-        wcur = ro_.wcur;                                                                                              \
-        limit = ro_.limit;                                                                                            \
-        if (ro_.flags & ~1u) note_flags(ro_.flags);                                                                   \
-        load_words();                                                                                                 \
-        PROF_RARE(tr_, ACC);                                                                                          \
-        const uint32_t leave_ = ro_.flags & 1u;
+// a failed round (miss_), in line: the longest decided prefix (0, 1 or 2 symbols) is taken from a lane that matched it
+// -- its state after that prefix, its words consumed, its result words --, then the next symbol.  That symbol is
+// outside {M-1, M, M+1} (else a lane would have matched a longer prefix), so it goes straight to the 32-entry window:
+// one LDS (requested as soon as the prefix is known), one product, one vote; the exact f64 model outside the window is
+// the only call.  The words it may shift in are w0, w1, w2 (word[wpos ...], current after the round).  `done` is
+// published; the caller reloads the words and the round's intervals.
+#define CCD_FAIL()                                                                                                    \
+    {                                                                                                                 \
+        const uint32_t b1_ = __ballot_sync(0xffffffffu, ok1_ != 0u), b2_ = __ballot_sync(0xffffffffu, ok12_ != 0u);    \
+        const uint32_t bs_ = b2_ ? b2_ : b1_;                                                                         \
+        const uint32_t n_ = b2_ ? 2u : (b1_ ? 1u : 0u);                                                               \
+        const int src_ = bs_ ? __ffs((int)bs_) - 1 : 0;                                                               \
+        const uint32_t jf_ = j + n_, sf_ = jf_ & ring_mask;                                                           \
+        const uint32_t lt_ = lds_u32(sm.win + sf_ * (CCD_WIN * 4u) + 4u * (uint32_t)lane);                            \
+        const uint32_t xdl_ = __shfl_sync(0xffffffffu, b2_ ? dl2_ : dl1_, src_);                                      \
+        const uint32_t xdh_ = __shfl_sync(0xffffffffu, b2_ ? dh2_ : dh1_, src_);                                      \
+        const uint32_t xrl_ = __shfl_sync(0xffffffffu, b2_ ? rl2_ : rl1_, src_);                                      \
+        const uint32_t xrh_ = __shfl_sync(0xffffffffu, b2_ ? rh2_ : rh1_, src_);                                      \
+        const uint32_t xk_ = __shfl_sync(0xffffffffu, b2_ ? k2_ : k1_, src_);                                         \
+        const uint32_t q1_ = (uint32_t)src_ % 3u, q2_ = ((uint32_t)src_ / 3u) % 3u;                                   \
+        sts_u32_if(lane == 0 && n_ != 0u && q1_ != 1u, sm.res + ((j & ring_mask) << 2),                               \
+                   res_tag(j) | (CCD_WIN_HALF - 1u + q1_));                                                           \
+        sts_u32_if(lane == 0 && n_ == 2u && q2_ != 1u, sm.res + (((j + 1u) & ring_mask) << 2),                        \
+                   res_tag(j + 1u) | (CCD_WIN_HALF - 1u + q2_));                                                      \
+        const uint64_t df_ = n_ ? (((uint64_t)xdh_ << 32) | xdl_) : D;                                                \
+        const uint64_t rf_ = n_ ? (((uint64_t)xrh_ << 32) | xrl_) : R;                                                \
+        const uint32_t kf_ = n_ ? xk_ : 0u;                                                                           \
+        const FarOut f_ = coder_far(lt_, sm.meta + sf_ * 16u, scale_tab, lane, rf_ >> 24, df_);                       \
+        uint64_t dn_ = df_ - f_.lo, rn_ = f_.hi - f_.lo;                                                              \
+        const uint32_t wf_ = kf_ == 0u ? w0 : (kf_ == 1u ? w1 : w2);                                                  \
+        const uint32_t sh_ = (rn_ >> 32) == 0 ? 1u : 0u;                                                              \
+        D = sh_ ? ((dn_ << 32) | wf_) : dn_;                                                                          \
+        R = sh_ ? (rn_ << 32) : rn_;                                                                                  \
+        wpos += kf_ + sh_;                                                                                            \
+        sts_u32_if(f_.rw != (uint32_t)CCD_WIN_HALF, sm.res + (sf_ << 2), res_tag(jf_) | f_.rw);                        \
+        j = jf_ + 1u;                                                                                                 \
+        sts_done(done_a, j);                                                                                          \
+        if (f_.flags) note_flags(f_.flags);                                                                           \
+        PROF_FAIL(n_);                                                                                                \
+    }
 #ifdef CCD_PROFILE
-#define PROF_RARE(T0, ACC)                                                                                            \
+#define PROF_FAIL(N)                                                                                                  \
     do {                                                                                                              \
-        ACC += clock64() - (T0);                                                                                      \
-        cp.fail += ro_.cyc_fail;                                                                                      \
-        cp.move += ro_.cyc_move;                                                                                      \
-        cp.ref += ro_.cyc_ref;                                                                                        \
-        cp.n_fail += miss_;                                                                                           \
-        cp.n_move += ro_.cyc_move != 0u;                                                                              \
-        cp.n_ref += ro_.cyc_ref != 0u;                                                                                \
-        cp.n_pre += ro_.n_pre;                                                                                        \
-        c.n_redo += miss_;                                                                                            \
-        pc.seg[3] += ro_.n_pre;                                                                                       \
+        c.n_far++;                                                                                                    \
+        c.n_redo++;                                                                                                   \
+        pc.seg[3] += (N);                                                                                             \
+        cp.n_pre += (N);                                                                                              \
     } while (0)
 #define PROF_ROUND(N)                                                                                                 \
     do {                                                                                                              \
@@ -1108,7 +1042,7 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         pc.seg[3] += miss_ ? 0u : NS;                                                                                 \
     } while (0)
 #else
-#define PROF_RARE(T0, ACC)
+#define PROF_FAIL(N)
 #define PROF_ROUND(N)
 #endif
     uint32_t pa1, pb1, pa2, pb2, pa3, pb3, qa1, qb1, qa2, qb2, qa3, qb3;  // two sets of candidate intervals
@@ -1166,8 +1100,8 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
             }
             PROF_ROUND(cp.n_one_ok);
             if (miss_) {
-                CCD_RARE(0u, cp.rare_one)
-                (void)leave_;
+                CCD_FAIL()
+                load_words();  // w0 for a single-symbol step
             }
 #ifdef CCD_PROFILE
             cp.one += clock64() - t1;
@@ -1180,13 +1114,22 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         // ready past its j: its own intervals and those of the next round.  A matched round is straight-line code: its
         // one conditional leaves the inner loop for the rare path, and the iteration's one taken branch is the back-edge
         // (a taken branch costs this warp 10 ... 40 cycles; tools/sass_coder_path.py checks the SASS).  The rare test is
-        // a vote: a warp-uniform branch needs no reconvergence region, which would keep the rare path in line.  After
-        // the rare path the loop starts again at the round j.
+        // a vote: a warp-uniform branch needs no reconvergence region, which would keep the rare path in line.
+        // `ready` is read once per iteration and folded into `limit` before the first round's rare test: the load goes
+        // out ahead of the round's record round trip and only the fold waits for it, so the loop leaves for want of
+        // symbols only when the producers are behind (DESIGN §4.1 has why a plain LDS is the acquire here).  The rare
+        // path follows the inner loop in this function, with no call: a failed round, the window move, and a refresh
+        // that still finds fewer than 2 NS ready leaves the steady loop; otherwise the loop starts again at the round j.
         PROF_T(ts);
         while (true) {
             while (true) {
+                const uint32_t rdy_ = lds_acq_u32(ready_a);
+#ifdef CCD_PROFILE
+                cp.n_ref++;
+#endif
                 CCD_SLOAD(q, j + NS)
                 {
+                    limit = ((int32_t)(rdy_ - ord_end) > 0) ? ord_end : rdy_;
                     CCD_ROUND(p, 2u * NS)
                 }
                 PROF_ROUND(cp.n_steady);
@@ -1198,9 +1141,38 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
                 PROF_ROUND(cp.n_steady);
                 if (__builtin_expect(__any_sync(0xffffffffu, rare_ != 0u), 0)) break;
             }
-            CCD_RARE(2u * NS, cp.rare)
-            if (leave_) break;
+            PROF_T(tr);
+            if (miss_) {
+                CCD_FAIL()
+            }
+            if (wpos - wbase >= 24u) {
+                move_window();
+#ifdef CCD_PROFILE
+                cp.n_move++;
+#endif
+            }
+            if ((int32_t)(limit - j) < (int32_t)(2u * NS)) {
+                refresh();
+                if ((int32_t)(limit - j) < (int32_t)(2u * NS)) {
+#ifdef CCD_PROFILE
+                    cp.n_starve++;
+                    cp.rare += clock64() - tr;
+#endif
+                    break;
+                }
+            }
+            load_words();
             CCD_SLOAD(p, j)
+#ifdef CCD_PROFILE
+            {
+                const long long dt = clock64() - tr;
+                cp.rare += dt;
+                if (miss_) {
+                    cp.fail += dt;
+                    cp.n_fail++;
+                }
+            }
+#endif
         }
 #ifdef CCD_PROFILE
         cp.steady += clock64() - ts;
@@ -1209,20 +1181,21 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
 #undef CCD_SSTEP
 #undef CCD_SLOAD
 #undef CCD_ROUND
-#undef CCD_RARE
-#undef PROF_RARE
+#undef CCD_FAIL
+#undef PROF_FAIL
 #undef PROF_ROUND
 #ifdef CCD_PROFILE
     // one line per grid (tools/gpu_1080.py tabulates them): symbols, then cycles / count of matched steady rounds
-    // (the steady loop less its rare path), failed rounds (all of them, with the symbols of their decided prefixes),
-    // window moves and refreshes of the rare path, waits of the outer loop, one-round steps (matched ones counted
-    // apart) and single-symbol steps, and the rare path's total in the steady loop (call and reloads included)
+    // (the steady loop less its rare path), failed rounds of the steady loop timed from the loop's exit to the start of
+    // the next round, the decided-prefix symbols of all failed rounds, the steady loop's window moves, its reads of
+    // `ready` and its exits for want of ready symbols, waits of the outer loop, one-round steps (matched ones counted
+    // apart) and single-symbol steps, and the steady loop's rare path in all (from each exit to the next round or out)
     if (lane == 0)
-        printf("CCDPROF grid_begin %u n %u steady %lld %u fail %lld %u pre %u move %lld %u ref %lld %u wait %lld %u "
+        printf("CCDPROF grid_begin %u n %u steady %lld %u fail %lld %u pre %u move %u ref %u starve %u wait %lld %u "
                "one %lld %u %u single %lld %u rare %lld\n",
-               ord_begin, ord_end - ord_begin, cp.steady - cp.rare, cp.n_steady, cp.fail, cp.n_fail, cp.n_pre, cp.move,
-               cp.n_move, cp.ref, cp.n_ref, cp.wait, cp.n_wait, cp.one, cp.n_one, cp.n_one_ok, cp.single, cp.n_single,
-               cp.rare);
+               ord_begin, ord_end - ord_begin, cp.steady - cp.rare, cp.n_steady, cp.fail, cp.n_fail, cp.n_pre,
+               cp.n_move, cp.n_ref, cp.n_starve, cp.wait, cp.n_wait, cp.one, cp.n_one, cp.n_one_ok, cp.single,
+               cp.n_single, cp.rare);
 #endif
     c.D = D;
     c.R = R;

@@ -2,7 +2,8 @@
 
 With the instrumented library (CCD_LIB=cool-chic_b200/csrc/libccdec_prof.so, `make prof`) it also tabulates the coder
 warp's per-grid breakdown, which the kernel prints once per grid (CCDPROF lines): cycles and counts of matched steady
-rounds, failed rounds, window moves, refreshes, waits, one-round and single-symbol steps."""
+rounds, failed rounds, window moves, reads of `ready`, exits for want of ready symbols, waits, one-round and
+single-symbol steps."""
 import os, re, sys, tempfile, time
 import numpy as np, torch
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -48,25 +49,26 @@ def prof_table(text):
     for line in text.splitlines():
         if line.startswith("CCDPROF"):
             v = [int(x) for x in re.findall(r"-?\d+", line)]
-            rows.append(dict(zip(("ord", "n", "st_c", "st_n", "fa_c", "fa_n", "pre", "mv_c", "mv_n", "rf_c", "rf_n", "wt_c",
-                                  "wt_n", "one_c", "one_n", "one_ok", "sg_c", "sg_n", "rare_c"), v)))
+            rows.append(dict(zip(("ord", "n", "st_c", "st_n", "fa_c", "fa_n", "pre", "mv_n", "rf_n", "sv_n", "wt_c", "wt_n",
+                                  "one_c", "one_n", "one_ok", "sg_c", "sg_n", "rare_c"), v)))
     if not rows:
         return
     print("coder warp per grid (decode order; kcyc = kilo-cycles; cyc/x = cycles per round / case):")
-    print("%6s %9s | %9s %8s %6s | %8s %6s %6s | %6s %5s | %7s %6s | %7s %6s | %7s %6s %7s | %7s %6s | %8s"
-          % ("grid", "symbols", "matched", "rounds", "cyc/r", "fail", "n", "cyc/f", "move", "n", "refresh", "n", "wait",
+    print("%6s %9s | %9s %8s %6s | %8s %6s %6s | %5s | %7s %5s | %7s %6s | %7s %6s %7s | %7s %6s | %8s"
+          % ("grid", "symbols", "matched", "rounds", "cyc/r", "fail", "n", "cyc/f", "move", "ready", "starve", "wait",
              "n", "1-round", "n", "matched", "single", "n", "rare"))
     tot = dict.fromkeys(rows[0], 0)
     for i, r in enumerate(rows):
         for k_ in r:
             tot[k_] += r[k_]
     for name, r in [(str(i), r) for i, r in enumerate(rows)] + [("all", tot)]:
-        print("%6s %9d | %9.1f %8d %6.1f | %8.1f %6d %6.0f | %6.1f %5d | %7.1f %6d | %7.1f %6d | %7.1f %6d %7d | %7.1f %6d | %8.1f"
+        print("%6s %9d | %9.1f %8d %6.1f | %8.1f %6d %6.0f | %5d | %7d %5d | %7.1f %6d | %7.1f %6d %7d | %7.1f %6d | %8.1f"
               % (name, r["n"], r["st_c"] / 1e3, r["st_n"], r["st_c"] / max(1, r["st_n"]), r["fa_c"] / 1e3, r["fa_n"],
-                 r["fa_c"] / max(1, r["fa_n"]), r["mv_c"] / 1e3, r["mv_n"], r["rf_c"] / 1e3, r["rf_n"], r["wt_c"] / 1e3,
-                 r["wt_n"], r["one_c"] / 1e3, r["one_n"], r["one_ok"], r["sg_c"] / 1e3, r["sg_n"], r["rare_c"] / 1e3))
-    print("  matched: the steady loop less its rare path; fail / move / refresh: the three parts of the rare path "
-          "(inside the call); rare: the steady loop's rare path in all (call, argument moves and reloads)")
+                 r["fa_c"] / max(1, r["fa_n"]), r["mv_n"], r["rf_n"], r["sv_n"], r["wt_c"] / 1e3, r["wt_n"],
+                 r["one_c"] / 1e3, r["one_n"], r["one_ok"], r["sg_c"] / 1e3, r["sg_n"], r["rare_c"] / 1e3))
+    print("  matched: the steady loop less its rare path; fail: failed rounds of the steady loop, from the loop's exit "
+          "to the next round; move: window moves; ready: reads of `ready` in the steady loop; starve: exits for want "
+          "of ready symbols; rare: the steady loop's rare path in all")
 
 
 for it in range(3):

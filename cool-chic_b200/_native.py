@@ -7,7 +7,7 @@ of device memory (``tensor.data_ptr()``) and of the CUDA stream.
 import ctypes
 import os
 import threading
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -28,7 +28,7 @@ EXPORTS = [
     "ccd_version", "ccd_sizeof_desc", "ccd_last_error", "ccd_create", "ccd_destroy", "ccd_nn_count",
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
     "ccd_encode_latents", "ccd_synthesize_many", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
-    "ccd_latent_rate", "ccd_latent_rate_edited", "ccd_rate_sweep", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats", "ccd_inter_analysis",
+    "ccd_latent_rate", "ccd_latent_rate_edited", "ccd_rate_sweep", "ccd_rate_candidates", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats", "ccd_inter_analysis",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
     "ccd_debug_entropy_plan", "ccd_debug_cdf_table", "ccd_debug_detmath", "ccd_debug_sinc_coeffs", "ccd_debug_cr_noise",
 ]
@@ -105,6 +105,13 @@ class CcdModelEdit(ctypes.Structure):
 
 
 SWEEP_MAX_OFFSETS = 32  # CCD_SWEEP_MAX_OFFSETS
+
+
+class CcdCandidate(ctypes.Structure):
+    _fields_ = [("nn_index", ctypes.c_int32), ("delta", ctypes.c_int32)]
+
+
+CCD_CAND_MAX = 64
 
 
 class CcdSweepJob(ctypes.Structure):
@@ -265,6 +272,8 @@ def load_library():
         L.ccd_latent_rate_edited.restype = ci
         L.ccd_latent_rate_edited.argtypes = [vp, ctypes.POINTER(CcdRateJob), ctypes.POINTER(CcdModelEdit), ci, vp]
         L.ccd_rate_sweep.restype = ci
+        L.ccd_rate_candidates.restype = ci
+        L.ccd_rate_candidates.argtypes = [vp, pd, vp, vp, ctypes.POINTER(CcdCandidate), ci, vp, vp, vp]
         L.ccd_rate_sweep.argtypes = [vp, ctypes.POINTER(CcdSweepJob), ci, vp]
         L.ccd_frame_distortion.restype = ci
         L.ccd_frame_distortion.argtypes = [vp, ctypes.POINTER(CcdDistJob), ci, vp]
@@ -697,6 +706,25 @@ class Context:
         for i in range(n):
             res[i]["grid_bits"] = [float(jobs[i].grid_bits[g]) for g in range(descs[i].n_grids)]
         return res
+
+    def rate_candidates(self, desc: CcdCoolChicDesc, nn_ints: np.ndarray, latents: torch.Tensor,
+                        cands: Sequence[Tuple[int, int]]):
+        """Exact per-grid latent bits under the model and under one-integer edits of it (``ccd_rate_candidates``,
+        DESIGN §4.11), in one launch.  ``cands``: up to CCD_CAND_MAX (nn_index, delta) pairs, nn_index into the
+        ``decode_nn`` order (ARM and IFCE integers only).  Returns (bits float64 [1 + k][n_grids], grid 0 = finest,
+        row 0 the model itself; fast bool [1 + k]: the model takes the fast entropy kernel)."""
+        nn = np.ascontiguousarray(nn_ints, dtype=np.int64)
+        if not (latents.is_cuda and latents.dtype == torch.int8 and latents.is_contiguous()
+                and latents.numel() == desc.n_symbols()):
+            raise ValueError(f"latents must be a contiguous int8 CUDA tensor of {desc.n_symbols()} symbols")
+        k = len(cands)
+        arr = (CcdCandidate * max(k, 1))(*[CcdCandidate(int(i), int(dl)) for i, dl in cands])
+        bits = np.zeros((k + 1, desc.n_grids), dtype=np.float64)
+        fast = np.zeros(k + 1, dtype=np.int32)
+        _check(self._lib.ccd_rate_candidates(self._h, ctypes.byref(desc), nn.ctypes.data_as(ctypes.c_void_p),
+                                             latents.data_ptr(), arr, k, bits.ctypes.data_as(ctypes.c_void_p),
+                                             fast.ctypes.data_as(ctypes.c_void_p), self._stream()))
+        return bits, fast.astype(bool)
 
     def rate_sweep(self, descs: Sequence[CcdCoolChicDesc], latents: Sequence[torch.Tensor],
                    mu_sc: Sequence[torch.Tensor], sc_offsets: Sequence[int]) -> List[dict]:

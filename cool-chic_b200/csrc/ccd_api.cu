@@ -674,27 +674,55 @@ int check_edit(const CcdModelEdit &e, const CcdCoolChicDesc *d, int i) {
     return CCD_OK;
 }
 
+// The fixed-point ARM of a Cool-chic from its NN integers (component/coolchic.py:72-77)
+ArmInts model_arm(const CcdCoolChicDesc *d, const NNLayout &L, const int64_t *nn) {
+    std::vector<const int64_t *> qw, qb;
+    for (int l = 0; l < L.n_arm_lin; l++) {
+        qw.push_back(nn + L.arm_w[l]);
+        qb.push_back(nn + L.arm_b[l]);
+    }
+    return build_arm(L.dim, d->arm_hidden, 2, qw.data(), qb.data(), d->arm_stab ? nn + L.arm_w[L.n_arm_lin] : nullptr,
+                     d->arm_stab ? nn + L.arm_b[L.n_arm_lin] : nullptr, d->qshift[0], d->qshift[1], true,
+                     d->n_ifce_out, false);
+}
+
+// The fixed-point IFCE j (of grid L.ifce_grid[j]) from the NN integers (component/coolchic.py:114-123)
+ArmInts model_ifce(const CcdCoolChicDesc *d, const NNLayout &L, const int64_t *nn, int j) {
+    const int64_t *w1[1] = {nn + L.ifce_w[j]};
+    const int64_t *b1[1] = {nn + L.ifce_b[j]};
+    return build_arm(d->grid_ifce_in[L.ifce_grid[j]], 0, d->n_ifce_out, w1, b1, nullptr, nullptr, d->qshift[2],
+                     d->qshift[3], false, 0, true);
+}
+
+// The decoder's kernel choice: the fast (DMMA) kernel when the architecture has one, every IFCE has at most
+// CCD_IFCE_FAST_MAX inputs and a bounded feature, and the ARM fits f64 exactly (arm_fits_f64)
+bool model_fast(const CcdCoolChicDesc *d, const NNLayout &L, const ArmInts &arm, const std::vector<ArmInts> &ifce) {
+    bool fast = ccd_entropy_has_fast(d->n_ctx, d->n_ifce_out);
+    i128 feat_bound = 0;
+    for (int j = 0; j < L.n_ifce; j++) {
+        i128 bnd = 0;
+        if (!ifce_bound(ifce[(size_t)j], &bnd)) fast = false;
+        if (d->grid_ifce_in[L.ifce_grid[j]] > CCD_IFCE_FAST_MAX) fast = false;
+        feat_bound = std::max(feat_bound, bnd);
+    }
+    if (fast) fast = arm_fits_f64(arm, d->n_ctx, feat_bound);
+    return fast;
+}
+
 // Host preparation of one job: prepare_synthesis, then the entropy stage's ARM / IFCE packing and stream descriptor.
 // The descriptor's grid table covers the decode-order grids [gb, ge) (ge < 0: to the last), each with its absolute
 // latent and IFCE offsets; the shared-memory plan covers those grids.  edit (rate analysis only, checked by
 // check_edit): the ARM and IFCE inputs it names are read as 0, applied to the integers before the fast-path choice.
-int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt, int gb = 0, int ge = -1, const CcdModelEdit *edit = nullptr) {
+// generic_blob (candidate pricing): the blobs take the generic (int64) layout whatever P.fast says.
+int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt, int gb = 0, int ge = -1, const CcdModelEdit *edit = nullptr,
+                bool generic_blob = false) {
     if (int rc = prepare_synthesis(P, nn_ints_opt)) return rc;
     const CcdCoolChicDesc *d = P.d;
     const NNLayout &L = P.L;
     const int64_t *nn = P.nn.data();
     // ---- ARM + IFCE integers
     const int dim = L.dim;
-    std::vector<const int64_t *> qw, qb;
-    for (int l = 0; l < L.n_arm_lin; l++) {
-        qw.push_back(nn + L.arm_w[l]);
-        qb.push_back(nn + L.arm_b[l]);
-    }
-    // component/coolchic.py:72-77
-    ArmInts arm = build_arm(dim, d->arm_hidden, 2, qw.data(), qb.data(),
-                            d->arm_stab ? nn + L.arm_w[L.n_arm_lin] : nullptr,
-                            d->arm_stab ? nn + L.arm_b[L.n_arm_lin] : nullptr, d->qshift[0], d->qshift[1], true,
-                            d->n_ifce_out, false);
+    ArmInts arm = model_arm(d, L, nn);
     if (edit) {
         for (int i = 0; i < dim; i++) {
             const bool z = i < d->n_ctx ? ((edit->zero_ctx >> i) & 1u) : ((edit->zero_ifce_out >> (i - d->n_ctx)) & 1u);
@@ -704,27 +732,17 @@ int prepare_job(PreparedJob &P, const int64_t *nn_ints_opt, int gb = 0, int ge =
         }
     }
     std::vector<ArmInts> ifce;
-    i128 feat_bound = 0;
-    bool fast = ccd_entropy_has_fast(d->n_ctx, d->n_ifce_out);
     for (int j = 0; j < L.n_ifce; j++) {
-        const int64_t *w1[1] = {nn + L.ifce_w[j]};
-        const int64_t *b1[1] = {nn + L.ifce_b[j]};
-        // component/coolchic.py:114-123
-        ifce.push_back(build_arm(d->grid_ifce_in[L.ifce_grid[j]], 0, d->n_ifce_out, w1, b1, nullptr, nullptr,
-                                 d->qshift[2], d->qshift[3], false, 0, true));
+        ifce.push_back(model_ifce(d, L, nn, j));
         if (edit) {  // channel c of grid g reads grid g + 1 + c
             const int g = L.ifce_grid[j];
             for (int c = 0; c < d->grid_ifce_in[g]; c++)
                 if (g + 1 + c < d->n_grids && ((edit->zero_ifce_grids >> (g + 1 + c)) & 1u))
                     zero_input_row(ifce.back().W[0], c, d->n_ifce_out);
         }
-        i128 bnd = 0;
-        if (!ifce_bound(ifce.back(), &bnd)) fast = false;
-        if (d->grid_ifce_in[L.ifce_grid[j]] > CCD_IFCE_FAST_MAX) fast = false;
-        feat_bound = std::max(feat_bound, bnd);
     }
-    if (fast) fast = arm_fits_f64(arm, d->n_ctx, feat_bound);
-    P.fast = fast;
+    P.fast = model_fast(d, L, arm, ifce);
+    const bool fast = P.fast && !generic_blob;
     P.blob.clear();
     pack_arm(arm, fast, P.blob);
     const int arm_bytes = (int)P.blob.size();
@@ -1882,6 +1900,165 @@ static int rate_sweep_body(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, cudaS
     return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {
         return fail(CCD_ERR_ARG, "job %d: symbol %lld has a latent outside [-64, 63] or a (mu_idx, sc_idx) outside its table",
                     i, (long long)jobs[i].bad_index);
+    });
+}
+
+// One candidate of ccd_rate_candidates as the kernel prices it: which fixed-point weight or bias moves, by how much
+// (the rebuilt model's value minus the model's), and whether the edited model takes the fast kernel.
+static CandDev locate_candidate(const CcdCoolChicDesc *d, const NNLayout &L, std::vector<int64_t> &nn,
+                                const ArmInts &arm, std::vector<ArmInts> &ifce, const CcdCandidate &c, bool *fast) {
+    CandDev C;
+    memset(&C, 0, sizeof(C));
+    const int64_t idx = c.nn_index;
+    const int dim = L.dim, nh = d->arm_hidden;
+    nn[(size_t)idx] += c.delta;
+    if (idx < L.counts[0] + L.counts[1]) {
+        const ArmInts a = model_arm(d, L, nn.data());
+        *fast = model_fast(d, L, a, ifce);
+        for (int l = 0; l < L.n_arm_lin + (d->arm_stab ? 1 : 0); l++) {
+            const bool stab = l == L.n_arm_lin;
+            const int out = (l >= nh) ? 2 : dim;
+            const std::vector<int64_t> &W1 = stab ? a.Ws : a.W[(size_t)l], &W0 = stab ? arm.Ws : arm.W[(size_t)l];
+            const std::vector<int64_t> &B1 = stab ? a.Bs : a.B[(size_t)l], &B0 = stab ? arm.Bs : arm.B[(size_t)l];
+            C.type = stab ? CCD_CAND_STAB : CCD_CAND_ARM;
+            C.l = l;
+            if (idx >= L.arm_w[l] && idx < L.arm_w[l] + (int64_t)out * dim) {  // qw[o][i]
+                C.o = (int)((idx - L.arm_w[l]) / dim);
+                C.i = (int)((idx - L.arm_w[l]) % dim);
+                C.dv = W1[(size_t)C.i * out + C.o] - W0[(size_t)C.i * out + C.o];
+                break;
+            }
+            if (idx >= L.arm_b[l] && idx < L.arm_b[l] + out) {
+                C.o = (int)(idx - L.arm_b[l]);
+                C.i = -1;
+                C.dv = B1[(size_t)C.o] - B0[(size_t)C.o];
+                break;
+            }
+        }
+    } else {
+        const int cf = d->n_ifce_out;
+        C.type = CCD_CAND_IFCE;
+        for (int j = 0; j < L.n_ifce; j++) {
+            const int n_in = d->grid_ifce_in[L.ifce_grid[j]];
+            const bool wt = idx >= L.ifce_w[j] && idx < L.ifce_w[j] + (int64_t)cf * n_in;
+            if (!wt && !(idx >= L.ifce_b[j] && idx < L.ifce_b[j] + cf)) continue;
+            ArmInts e = model_ifce(d, L, nn.data(), j);
+            std::swap(ifce[(size_t)j], e);
+            *fast = model_fast(d, L, arm, ifce);
+            std::swap(ifce[(size_t)j], e);  // e: the edited IFCE again
+            C.l = d->n_grids - 1 - L.ifce_grid[j];
+            if (wt) {  // qw[o][i]
+                C.o = (int)((idx - L.ifce_w[j]) / n_in);
+                C.i = (int)((idx - L.ifce_w[j]) % n_in);
+                C.dv = e.W[0][(size_t)C.i * cf + C.o] - ifce[(size_t)j].W[0][(size_t)C.i * cf + C.o];
+            } else {
+                C.o = (int)(idx - L.ifce_b[j]);
+                C.i = -1;
+                C.dv = e.B[0][(size_t)C.o] - ifce[(size_t)j].B[0][(size_t)C.o];
+            }
+            break;
+        }
+    }
+    nn[(size_t)idx] -= c.delta;
+    // the fast kernel exists only for models with IFCE features or none at all (flag_ifce 0 means n_ifce_out 0), so the
+    // edited model's rate kernel is the fast one exactly when it is fast
+    C.quad_order = *fast ? 1 : 0;
+    return C;
+}
+
+static int rate_candidates_body(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints,
+                                const int8_t *d_latents, const CcdCandidate *cands, int k, double *bits_out,
+                                int32_t *fast_out, cudaStream_t st) {
+    if (!desc || !nn_ints || !d_latents || !cands || !bits_out) return fail(CCD_ERR_ARG, "null pointer");
+    if (k < 1 || k > CCD_CAND_MAX) return fail(CCD_ERR_ARG, "k=%d outside 1 .. %d", k, CCD_CAND_MAX);
+    PreparedJob J;
+    J.d = desc;
+    if (int rc = prepare_job(J, nn_ints, 0, -1, nullptr, true)) return rc;
+    const NNLayout &L = J.L;
+    const int64_t n_model = L.counts[0] + L.counts[1] + L.counts[2] + L.counts[3];  // ARM, then IFCE integers
+    for (int j = 0; j < k; j++) {
+        if (cands[j].nn_index < 0 || cands[j].nn_index >= n_model)
+            return fail(CCD_ERR_ARG, "candidate %d: index %d is not an ARM or IFCE integer (0 .. %lld)", j,
+                        cands[j].nn_index, (long long)n_model - 1);
+        if (cands[j].delta == 0) return fail(CCD_ERR_ARG, "candidate %d: delta 0", j);
+    }
+    const int nk = k + 1;
+    std::vector<CandDev> C((size_t)nk);
+    memset(C.data(), 0, sizeof(CandDev) * (size_t)nk);
+    C[0].type = CCD_CAND_BASE;
+    C[0].quad_order = J.fast ? 1 : 0;
+    if (fast_out) fast_out[0] = J.fast ? 1 : 0;
+    {
+        std::vector<int64_t> nn = J.nn;
+        const ArmInts arm = model_arm(desc, L, nn.data());
+        std::vector<ArmInts> ifce;
+        for (int j = 0; j < L.n_ifce; j++) ifce.push_back(model_ifce(desc, L, nn.data(), j));
+        for (int j = 0; j < k; j++) {
+            bool fast = false;
+            C[(size_t)j + 1] = locate_candidate(desc, L, nn, arm, ifce, cands[j], &fast);
+            if (fast_out) fast_out[j + 1] = fast ? 1 : 0;
+        }
+    }
+    const int n_grids = desc->n_grids;
+    std::vector<RateTile> tiles;
+    std::vector<size_t> tile_at;  // tiles of decode-order grid gi: [tile_at[gi], tile_at[gi + 1])
+    for (int gi = 0; gi < n_grids; gi++) {
+        const EntGrid &G = J.es.grid[gi];
+        tile_at.push_back(tiles.size());
+        for (int y0 = 0; y0 < G.h; y0 += CCD_RATE_TH)
+            for (int x0 = 0; x0 < G.w; x0 += CCD_RATE_TW) tiles.push_back(RateTile{0, gi, y0, x0});
+    }
+    tile_at.push_back(tiles.size());
+    if (tiles.size() > (size_t)INT32_MAX) return fail(CCD_ERR_UNSUPPORTED, "too many rate tiles");
+    const size_t smem = ccd_rate_candidates_smem_bytes(J.es.arm_blob_bytes, J.es.ifce_blob_max, nk);
+    if (smem > CCD_SMEM_MAX)
+        return fail(CCD_ERR_UNSUPPORTED, "candidate pricing needs %zu bytes of shared memory, %d are available", smem,
+                    CCD_SMEM_MAX);
+    Arena A;
+    J.off_blob = A.take(J.blob.size());
+    const size_t off_es = A.take(sizeof(EntStream));
+    const size_t off_job = A.take(sizeof(CandJobDev));
+    const size_t off_cand = A.take(sizeof(CandDev) * (size_t)nk);
+    const size_t off_tiles = A.take(sizeof(RateTile) * tiles.size());
+    // results: the bad word (~0 before the launch), then the partials, which are not uploaded
+    const size_t off_bad = A.take(sizeof(unsigned long long));
+    const size_t off_part = A.take(sizeof(double) * tiles.size() * (size_t)nk);
+    if (int rc = stage(ctx, A)) return rc;
+    memcpy(A.h + J.off_blob, J.blob.data(), J.blob.size());
+    J.es.latents = const_cast<int8_t *>(d_latents);
+    J.es.blob = A.dv + J.off_blob;
+    memcpy(A.h + off_es, &J.es, sizeof(EntStream));
+    CandJobDev D;
+    memset(&D, 0, sizeof(D));
+    D.es = reinterpret_cast<const EntStream *>(A.dv + off_es);
+    D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad);
+    D.n_cand = nk;
+    memcpy(A.h + off_job, &D, sizeof(D));
+    memcpy(A.h + off_cand, C.data(), sizeof(CandDev) * (size_t)nk);
+    memcpy(A.h + off_tiles, tiles.data(), sizeof(RateTile) * tiles.size());
+    memset(A.h + off_bad, 0xff, sizeof(unsigned long long));
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
+    const bool wide = L.dim > 32 || desc->arm_hidden > 3;
+    int e = ccd_rate_candidates_launch(reinterpret_cast<const RateTile *>(A.dv + off_tiles), (int)tiles.size(),
+                                       reinterpret_cast<const CandJobDev *>(A.dv + off_job),
+                                       reinterpret_cast<const CandDev *>(A.dv + off_cand), wide, smem, ctx->d_cdf,
+                                       ctx->d_scale, reinterpret_cast<double *>(A.dv + off_part), st);
+    if (e != 0) return fail(CCD_ERR_CUDA, "candidate kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    if (int rc = download(A, off_bad, st, "candidate kernel")) return rc;
+    const double *part = reinterpret_cast<const double *>(A.h + off_part);
+    for (int c = 0; c < nk; c++)
+        for (int gi = 0; gi < n_grids; gi++)  // a grid's sum: its tiles in order
+            bits_out[(size_t)c * n_grids + (n_grids - 1 - gi)] =
+                ordered_sum(part + tile_at[gi] * (size_t)nk + c, tile_at[gi + 1] - tile_at[gi], (size_t)nk);
+    const unsigned long long bad = *reinterpret_cast<const unsigned long long *>(A.h + off_bad);
+    if (bad != ~0ull) return fail(CCD_ERR_ARG, "latent %lld is outside [-64, 63]", (long long)bad);
+    return CCD_OK;
+}
+
+int ccd_rate_candidates(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints, const int8_t *d_latents,
+                        const CcdCandidate *cands, int k, double *bits_out, int32_t *fast_out, void *cuda_stream) {
+    return guarded(ctx, cuda_stream, [&](cudaStream_t st) -> int {
+        return rate_candidates_body(ctx, desc, nn_ints, d_latents, cands, k, bits_out, fast_out, st);
     });
 }
 

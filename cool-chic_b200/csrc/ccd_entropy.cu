@@ -1722,6 +1722,253 @@ __global__ void k_rate_spatial(const RateSpatialDev *__restrict__ jobs) {
     J.out[p] = acc;
 }
 
+// Candidate pricing (DESIGN §4.11).  A thread per symbol evaluates the model once in int64, GenericArm's arithmetic,
+// keeping every layer's input X[l] and every hidden pre-activation Y[l], then prices each candidate as a change of that
+// evaluation: int64 sums are exact in any order, so a candidate's (o0, o1) is the edited model's bit for bit.
+//   ARM layer l < n_hidden, unit o: Y[l][o] += dv * x (x = X[l][i], or 1 for a bias), then ReLU and >> 16; a changed
+//     activation is a rank-1 change of layer l + 1, every later layer follows from the changed units only;
+//   output layer / stabiliser: the output sums move by dv * x, x from X[n_hidden] / X[0];
+//   IFCE of this tile's grid, feature o: its pre-rounding sum moves by dv * (v << 16) and the fp32 round trip is redone;
+//     a changed feature is a rank-1 change of layer 0 and of the stabiliser.
+// Sums: a candidate's partial is summed in the order of the rate kernel its edited model takes -- symbol s by thread
+// s mod 256 (generic) or by the quad s mod 64 (fast) -- so the host's tile-ordered sum equals ccd_latent_rate's.
+// Each pass of 256 symbols stores every candidate's freq in shared memory, then each candidate's running sums are
+// advanced in that order: thread t for a generic one; thread v + 64 (k & 3) for slot v of a fast one.
+template <int MAXD, int MAXH>
+struct CandEval {
+    const long long *Wh, *Wl, *Ws, *Bh;
+    int dim, nh;
+    long long X[(MAXH + 1) * MAXD];  // X[l]: input of layer l (<< 16 applied to layer 0)
+    long long Y[MAXH * MAXD];        // hidden pre-activations
+    long long D[MAXD], T[MAXD];
+    long long a0, a1, s0, s1;        // output layer + its bias, stabiliser + its bias
+
+    __device__ void base(const long long *Bl, const long long *Bs) {
+        s0 = Bs[0];
+        s1 = Bs[1];
+        for (int i = 0; i < dim; i++) {
+            s0 += Ws[2 * i] * X[i];
+            s1 += Ws[2 * i + 1] * X[i];
+        }
+        for (int l = 0; l < nh; l++) {
+            const long long *W = Wh + (size_t)l * dim * dim;
+            long long *y = Y + l * MAXD;
+            for (int o = 0; o < dim; o++) y[o] = Bh[(size_t)l * dim + o];
+            for (int i = 0; i < dim; i++) {
+                const long long xi = X[l * MAXD + i];
+                for (int o = 0; o < dim; o++) y[o] += W[(size_t)i * dim + o] * xi;
+            }
+            for (int o = 0; o < dim; o++) X[(l + 1) * MAXD + o] = (y[o] < 0 ? 0 : y[o]) >> 16;
+        }
+        a0 = Bl[0];
+        a1 = Bl[1];
+        for (int i = 0; i < dim; i++) {
+            a0 += Wl[2 * i] * X[nh * MAXD + i];
+            a1 += Wl[2 * i + 1] * X[nh * MAXD + i];
+        }
+    }
+
+    // input u of layer l moves by dd: the change of the output sums (r0, r1)
+    __device__ void propagate(int l, int u, long long dd, long long &r0, long long &r1) {
+        if (l == nh) {
+            r0 += Wl[2 * u] * dd;
+            r1 += Wl[2 * u + 1] * dd;
+            return;
+        }
+        bool any = false;
+        {
+            const long long *W = Wh + (size_t)l * dim * dim + (size_t)u * dim;
+            for (int p = 0; p < dim; p++) {
+                const long long y = Y[l * MAXD + p] + W[p] * dd;
+                D[p] = ((y < 0 ? 0 : y) >> 16) - X[(l + 1) * MAXD + p];
+                any |= D[p] != 0;
+            }
+        }
+        for (l = l + 1; l < nh && any; l++) {
+            const long long *W = Wh + (size_t)l * dim * dim;
+            for (int p = 0; p < dim; p++) T[p] = Y[l * MAXD + p];
+            for (int i = 0; i < dim; i++) {
+                const long long di = D[i];
+                if (di == 0) continue;
+                for (int p = 0; p < dim; p++) T[p] += W[(size_t)i * dim + p] * di;
+            }
+            any = false;
+            for (int p = 0; p < dim; p++) {
+                D[p] = ((T[p] < 0 ? 0 : T[p]) >> 16) - X[(l + 1) * MAXD + p];
+                any |= D[p] != 0;
+            }
+        }
+        if (!any) return;
+        for (int i = 0; i < dim; i++) {
+            r0 += Wl[2 * i] * D[i];
+            r1 += Wl[2 * i + 1] * D[i];
+        }
+    }
+};
+
+template <int MAXD, int MAXH>
+__global__ void __launch_bounds__(CCD_RATE_THREADS)
+    k_rate_candidates(const RateTile *__restrict__ tiles, const CandJobDev *__restrict__ job,
+                      const CandDev *__restrict__ cand_g, const uint32_t *__restrict__ cdf,
+                      const float *__restrict__ scale_tab, double *__restrict__ part) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    __shared__ double wsum[CCD_RATE_THREADS / 32];
+    const RateTile t = tiles[blockIdx.x];
+    const CandJobDev &J = *job;
+    const EntStream &G = *J.es;
+    const EntGrid &Gg = G.grid[t.grid];
+    const int tid = threadIdx.x;
+    const int nk = J.n_cand;
+    EntGrid *g = reinterpret_cast<EntGrid *>(smem_raw);
+    unsigned char *arm = smem_raw + align16(sizeof(EntGrid));
+    unsigned char *ifce = arm + align16((size_t)G.arm_blob_bytes);
+    unsigned char *rows_p = ifce + align16((size_t)G.ifce_blob_max);
+    CandDev *cand = reinterpret_cast<CandDev *>(rows_p + CCD_RATE_ROWS * CCD_ROW_COLS);
+    uint32_t *fq = reinterpret_cast<uint32_t *>(cand + nk);  // [nk][CCD_RATE_THREADS]
+    double *red = reinterpret_cast<double *>(fq + (size_t)nk * CCD_RATE_THREADS);
+    const uint32_t rows = (uint32_t)__cvta_generic_to_shared(rows_p);
+    const int8_t *lat = G.latents;
+    const int h = Gg.h, w = Gg.w;
+    const long long base = Gg.lat_off;
+    {
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(&Gg);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(g);
+        for (int i = tid; i < (int)(sizeof(EntGrid) / 4); i += CCD_RATE_THREADS) dst[i] = src[i];
+        for (int i = tid * 4; i < G.arm_blob_bytes; i += CCD_RATE_THREADS * 4)
+            *reinterpret_cast<uint32_t *>(arm + i) = *reinterpret_cast<const uint32_t *>(G.blob + i);
+        for (int i = tid * 4; i < Gg.ifce_blob_bytes; i += CCD_RATE_THREADS * 4)
+            *reinterpret_cast<uint32_t *>(ifce + i) = *reinterpret_cast<const uint32_t *>(G.blob + Gg.ifce_blob_off + i);
+        for (int i = tid; i < nk; i += CCD_RATE_THREADS) cand[i] = cand_g[i];
+    }
+    const int nr = min(CCD_RATE_TH, h - t.y0), nc = min(CCD_RATE_TW, w - t.x0);
+    for (int i = tid; i < (nr + 4) * CCD_ROW_COLS; i += CCD_RATE_THREADS) {
+        const int yy = t.y0 - 4 + (i >> 6), xx = t.x0 - 4 + (i & (CCD_ROW_COLS - 1));
+        int v = 0;
+        if (yy >= 0 && xx >= 0 && xx < w) v = lat[base + (long long)yy * w + xx];
+        sts_u8(rows + ((((uint32_t)yy & (CCD_RATE_ROWS - 1)) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))), v);
+    }
+    __syncthreads();
+    const uint32_t row_mask = CCD_RATE_ROWS - 1;
+    const int n = nr * nc;
+    const int n_ctx = G.n_ctx, cf = G.cf, nh = G.n_hidden, dim = n_ctx + cf;
+    const int n_in = g->ifce_in;
+    CandEval<MAXD, MAXH> E;
+    E.dim = dim;
+    E.nh = nh;
+    E.Wh = reinterpret_cast<const long long *>(arm);
+    E.Wl = E.Wh + (size_t)nh * dim * dim;
+    E.Ws = E.Wl + (size_t)dim * 2;
+    E.Bh = E.Ws + (size_t)dim * 2;
+    const long long *Bl = E.Bh + (size_t)nh * dim;
+    const long long *Bs = Bl + 2;
+    const long long *IW = reinterpret_cast<const long long *>(ifce);
+    const long long *IB = IW + (size_t)n_in * cf;
+    long long IA[31];  // IFCE pre-rounding sums
+    int IV[31];        // IFCE inputs
+    double acc[CCD_CAND_MAX + 1];
+    for (int k = 0; k < nk; k++) acc[k] = 0.0;
+    for (int p0 = 0; p0 < n; p0 += CCD_RATE_THREADS) {
+        const int s = p0 + tid;
+        if (s < n) {
+            const int ty = s / nc, tx = s - ty * nc;
+            const int y = t.y0 + ty, x = t.x0 + tx;
+            for (int c = 0; c < n_ctx; c++) {
+                const int yy = y + c_ctx_dy[c], xx = x + c_ctx_dx[c];
+                int v = 0;
+                if (yy >= 0 && xx >= 0 && xx < w)
+                    v = lds_s8(rows + ((((uint32_t)yy & row_mask) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))));
+                E.X[c] = (long long)v << 16;
+            }
+            // GenericArm::ifce
+            if (cf > 0) {
+                for (int f = 0; f < cf; f++) IA[f] = n_in > 0 ? IB[f] : 0;
+                for (int c = 0; c < n_in; c++) {
+                    const int sh = g->ch_sh[c];
+                    int v = 0;
+                    if (sh >= 0) v = lat[g->ch_off[c] + (long long)((y >> 1) >> sh) * g->ch_w[c] + ((x >> 1) >> sh)];
+                    IV[c] = v;
+                    for (int f = 0; f < cf; f++) IA[f] += IW[(size_t)c * cf + f] * ((long long)v << 16);
+                }
+                for (int f = 0; f < cf; f++)
+                    E.X[n_ctx + f] = n_in > 0 ? __float2ll_rz(__ll2float_rn(IA[f] >> 24)) << 16 : 0;
+            }
+            E.base(Bl, Bs);
+            const int sym = lds_s8(rows + (((uint32_t)y & row_mask) << 6 | ((uint32_t)x & (CCD_ROW_COLS - 1))));
+            const bool bad = sym < kSymMin || sym > kSymMax;
+            if (bad) atomicMin(J.bad, (unsigned long long)(base + (long long)y * w + x));
+            auto clamp_mu = [](long long o0) { long long v = o0 + 16384; return (int)(v < 0 ? 0 : (v > 32767 ? 32767 : v)); };
+            auto clamp_sc = [](long long o1) { long long v = o1 + 1280; return (int)(v < 0 ? 0 : (v > 2560 ? 2560 : v)); };
+            const int mu = clamp_mu((E.a0 + E.s0) >> 24), sc = clamp_sc((E.a1 + E.s1) >> 24);
+            // a bad symbol adds 0 bits, as in the rate kernel
+            const uint32_t f0 = bad ? (1u << 24) : coder_freq(sym, mu, sc, cdf, scale_tab);
+            fq[tid] = f0;
+            for (int k = 1; k < nk; k++) {
+                const CandDev c = cand[k];
+                long long r0 = 0, r1 = 0, q0 = 0, q1 = 0;  // changes of the output layer's / the stabiliser's sums
+                if (c.type == CCD_CAND_STAB) {
+                    const long long d = c.dv * (c.i < 0 ? 1 : E.X[c.i]);
+                    (c.o == 0 ? q0 : q1) = d;
+                } else if (c.type == CCD_CAND_ARM) {
+                    if (c.l == nh) {
+                        const long long d = c.dv * (c.i < 0 ? 1 : E.X[nh * MAXD + c.i]);
+                        (c.o == 0 ? r0 : r1) = d;
+                    } else {
+                        const long long yv = E.Y[c.l * MAXD + c.o] + c.dv * (c.i < 0 ? 1 : E.X[c.l * MAXD + c.i]);
+                        const long long dd = ((yv < 0 ? 0 : yv) >> 16) - E.X[(c.l + 1) * MAXD + c.o];
+                        if (dd != 0) E.propagate(c.l + 1, c.o, dd, r0, r1);
+                    }
+                } else if (c.type == CCD_CAND_IFCE && c.l == t.grid) {
+                    const long long av = IA[c.o] + c.dv * (c.i < 0 ? 1 : ((long long)IV[c.i] << 16));
+                    const int u = n_ctx + c.o;
+                    const long long dd = (__float2ll_rz(__ll2float_rn(av >> 24)) << 16) - E.X[u];
+                    if (dd != 0) {
+                        q0 = E.Ws[2 * u] * dd;
+                        q1 = E.Ws[2 * u + 1] * dd;
+                        E.propagate(0, u, dd, r0, r1);
+                    }
+                }
+                uint32_t f = f0;
+                if (!bad && (r0 | r1 | q0 | q1) != 0) {
+                    const int mu2 = clamp_mu((E.a0 + r0 + E.s0 + q0) >> 24);
+                    const int sc2 = clamp_sc((E.a1 + r1 + E.s1 + q1) >> 24);
+                    if (mu2 != mu || sc2 != sc) f = coder_freq(sym, mu2, sc2, cdf, scale_tab);
+                }
+                fq[k * CCD_RATE_THREADS + tid] = f;
+            }
+        }
+        __syncthreads();
+        for (int k = 0; k < nk; k++) {
+            const uint32_t *fk = fq + (size_t)k * CCD_RATE_THREADS;
+            if (!cand[k].quad_order) {
+                if (s < n) acc[k] += 24.0 - log2((double)fk[tid]);
+            } else if ((k & 3) == (tid >> 6)) {
+                const int v = tid & 63;
+#pragma unroll
+                for (int q = 0; q < 4; q++)
+                    if (p0 + v + 64 * q < n) acc[k] += 24.0 - log2((double)fk[v + 64 * q]);
+            }
+        }
+        __syncthreads();
+    }
+    // per candidate, the rate kernel's reduction on its own layout: lanes (butterfly), then the warps in order
+    for (int k = 0; k < nk; k++) {
+        const bool quad = cand[k].quad_order;
+        if (!quad) red[tid] = acc[k];
+        else if ((k & 3) == (tid >> 6)) red[tid & 63] = acc[k];
+        __syncthreads();
+        double a = quad ? ((tid & 3) == 0 ? red[tid >> 2] : 0.0) : red[tid];
+#pragma unroll
+        for (int d = 16; d > 0; d >>= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
+        if ((tid & 31) == 0) wsum[tid >> 5] = a;
+        __syncthreads();
+        if (tid == 0) {
+            double sum = 0.0;
+            for (int i = 0; i < CCD_RATE_THREADS / 32; i++) sum += wsum[i];
+            part[(size_t)blockIdx.x * nk + k] = sum;
+        }
+    }
+}
+
 }  // namespace
 
 unsigned long long g_ccd_launches = 0;
@@ -1791,6 +2038,22 @@ int ccd_rate_launch(const RateTile *d_tiles, int n_tiles, const RateJobDev *d_jo
 int ccd_rate_sweep_launch(const RateTile *d_tiles, int n_tiles, const SweepJobDev *d_jobs, const uint32_t *d_cdf,
                           const float *d_scale, double *d_part, cudaStream_t st) {
     k_rate_sweep<<<n_tiles, CCD_RATE_THREADS, 0, st>>>(d_tiles, d_jobs, d_cdf, d_scale, d_part);
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
+
+size_t ccd_rate_candidates_smem_bytes(int arm_blob_bytes, int ifce_blob_max, int n_cand) {
+    return ccd_rate_smem_bytes(arm_blob_bytes, ifce_blob_max) + (size_t)n_cand * sizeof(CandDev) +
+           (size_t)n_cand * CCD_RATE_THREADS * 4 + (size_t)CCD_RATE_THREADS * 8;
+}
+
+int ccd_rate_candidates_launch(const RateTile *d_tiles, int n_tiles, const CandJobDev *d_job, const CandDev *d_cand,
+                               bool wide, size_t smem, const uint32_t *d_cdf, const float *d_scale, double *d_part,
+                               cudaStream_t st) {
+    auto kern = wide ? k_rate_candidates<CCD_MAX_DIM, 7> : k_rate_candidates<32, 3>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    kern<<<n_tiles, CCD_RATE_THREADS, smem, st>>>(d_tiles, d_job, d_cand, d_cdf, d_scale, d_part);
     g_ccd_launches++;
     return (int)cudaGetLastError();
 }

@@ -162,6 +162,32 @@ struct SweepJobDev {
 int ccd_rate_sweep_launch(const RateTile *d_tiles, int n_tiles, const SweepJobDev *d_jobs, const uint32_t *d_cdf,
                           const float *d_scale, double *d_part, cudaStream_t st);
 
+// Candidate pricing (k_rate_candidates, DESIGN §4.11): the RateTile list of the rate pass for one job, one CTA per
+// tile.  Candidate 0 is the model itself; candidate k > 0 changes ONE fixed-point weight or bias of the ARM or of one
+// grid's IFCE by dv (the change build_arm makes of a change of one transmitted integer).  One f64 partial per
+// (tile, candidate) in part[n_cand * tile + k], summed in the order of the rate kernel the edited model takes.
+enum { CCD_CAND_BASE = 0, CCD_CAND_ARM = 1, CCD_CAND_STAB = 2, CCD_CAND_IFCE = 3 };
+struct CandDev {
+    int32_t type;        // CCD_CAND_*
+    int32_t l;           // ARM: layer (n_hidden = the output layer); IFCE: the decode-order grid
+    int32_t i;           // ARM: input, IFCE: channel of a weight; -1: a bias
+    int32_t o;           // ARM: unit, IFCE: feature
+    int64_t dv;          // change of the fixed-point weight / bias
+    int32_t quad_order;  // 1: the fast rate kernel's summation order (a quad of lanes per symbol), 0: the generic's
+    int32_t pad;
+};
+struct CandJobDev {
+    const EntStream *es;      // GENERIC (int64) ARM and IFCE blobs whatever the decoder's kernel
+    unsigned long long *bad;  // smallest decode-order index of a latent outside [-64, 63] (~0 if none)
+    int32_t n_cand;           // candidates + 1
+};
+// bytes of dynamic shared memory of k_rate_candidates for a job
+size_t ccd_rate_candidates_smem_bytes(int arm_blob_bytes, int ifce_blob_max, int n_cand);
+// wide: an ARM wider than 32 or deeper than 3 hidden layers (the kernel's per-thread arrays are sized for it)
+int ccd_rate_candidates_launch(const RateTile *d_tiles, int n_tiles, const CandJobDev *d_job, const CandDev *d_cand,
+                               bool wide, size_t smem, const uint32_t *d_cdf, const float *d_scale, double *d_part,
+                               cudaStream_t st);
+
 // --------------------------------------------------------------------------------------
 // Synthesis stage (ccd_synth.cu)
 // --------------------------------------------------------------------------------------

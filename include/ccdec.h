@@ -267,6 +267,22 @@ typedef struct CcdSweepJob {
 /* All jobs in ONE kernel launch; one copy each way; synchronous.  Returns CCD_OK or the first failing job's status. */
 int ccd_rate_sweep(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, void *cuda_stream);
 
+/* Candidate pricing for lossless model tuning (DESIGN §4.11): ccd_latent_rate's per-grid bits of one Cool-chic's decoded
+ * latents under its model and under k candidate models, each of which adds delta to ONE transmitted ARM or IFCE integer
+ * (nn_index into the ccd_decode_nn order: an ARM weight or bias, stabiliser included, or an IFCE weight or bias).
+ * bits_out[c * n_grids + g] (out, grid 0 = finest): c = 0 the model itself, c = 1 + j candidate j; each equals, bit for
+ * bit, ccd_latent_rate's grid_bits on the edited integers.  fast_out[c] (out, may be NULL): 1 if that model takes the
+ * fast entropy kernel by the decoder's rule (arm_fits_f64 and the IFCE bound), else 0.  One kernel launch, one copy each
+ * way, synchronous.  CCD_ERR_ARG, before any launch: k outside 1 .. CCD_CAND_MAX, an index outside the ARM and IFCE
+ * integers, a delta of 0; after the launch: a latent outside [-64, 63]. */
+#define CCD_CAND_MAX 64
+typedef struct CcdCandidate {
+    int32_t nn_index;
+    int32_t delta;
+} CcdCandidate;
+int ccd_rate_candidates(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints, const int8_t *d_latents,
+                        const CcdCandidate *cands, int k, double *bits_out, int32_t *fast_out, void *cuda_stream);
+
 /* Tail of decode_frame for every frame type (bitstream/decode.py:191-206 with
  * io/format/yuv.py:239-256,274-300): round to the 2^b-1 grid -> (444->420 2x2 average of
  * U,V) -> clamp [0,1] -> round again.  data_type: 0 rgb, 1 yuv420, 2 yuv444.

@@ -880,6 +880,13 @@ struct CoderProf {
     long long steady = 0, rare = 0, fail = 0, wait = 0, one = 0, single = 0;
     uint32_t n_steady = 0, n_one_ok = 0, n_fail = 0, n_pre = 0, n_move = 0, n_ref = 0, n_starve = 0, n_wait = 0, n_one = 0,
              n_single = 0;
+    // every failed round, [3 * where it ran + its decided prefix] (where: 0 steady round A on set p, 1 steady round B
+    // on set q, 2 the one-round path; `at` is where the next one would run), counted by selects so that the table stays
+    // in registers
+    uint32_t fails[9] = {}, at = 0;
+    // failed rounds followed by a window move in the same rare-path visit, failed rounds whose far symbol took the
+    // exact model, single-symbol steps that went to tier 2, and those of them that took the exact model
+    uint32_t n_fail_move = 0, n_fail_exact = 0, n_single_t2 = 0, n_single_exact = 0;
 };
 #endif
 
@@ -1035,6 +1042,8 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         c.n_redo++;                                                                                                   \
         pc.seg[3] += (N);                                                                                             \
         cp.n_pre += (N);                                                                                              \
+        _Pragma("unroll") for (uint32_t k_ = 0; k_ < 9u; k_++) cp.fails[k_] += 3u * cp.at + (N) == k_ ? 1u : 0u;        \
+        cp.n_fail_exact += (f_.flags & 2u) ? 1u : 0u; /* f_: the far decision of the CCD_FAIL expanding this */      \
     } while (0)
 #define PROF_ROUND(N)                                                                                                 \
     do {                                                                                                              \
@@ -1078,6 +1087,10 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
                     w0 = r_.w0;
                     wpos = r_.wpos;
                     if (__builtin_expect(r_.flags != 0u, 0)) note_flags(r_.flags);
+#ifdef CCD_PROFILE
+                    cp.n_single_t2++;
+                    cp.n_single_exact += (r_.flags & 2u) ? 1u : 0u;
+#endif
                 }
             }
             j++;
@@ -1095,6 +1108,9 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
         if ((int32_t)(limit - j) < (int32_t)(3u * NS)) {
             // fewer symbols ready than the steady loop wants: one round
             PROF_T(t1);
+#ifdef CCD_PROFILE
+            cp.at = 2;
+#endif
             {
                 CCD_ROUND(p, 0u)
             }
@@ -1126,6 +1142,7 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
                 const uint32_t rdy_ = lds_acq_u32(ready_a);
 #ifdef CCD_PROFILE
                 cp.n_ref++;
+                cp.at = 0;
 #endif
                 CCD_SLOAD(q, j + NS)
                 {
@@ -1134,6 +1151,9 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
                 }
                 PROF_ROUND(cp.n_steady);
                 if (__builtin_expect(__any_sync(0xffffffffu, rare_ != 0u), 0)) break;
+#ifdef CCD_PROFILE
+                cp.at = 1;
+#endif
                 CCD_SLOAD(p, j + NS)
                 {
                     CCD_ROUND(q, 2u * NS)
@@ -1149,14 +1169,21 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
                 move_window();
 #ifdef CCD_PROFILE
                 cp.n_move++;
+                cp.n_fail_move += miss_;
 #endif
             }
             if ((int32_t)(limit - j) < (int32_t)(2u * NS)) {
                 refresh();
                 if ((int32_t)(limit - j) < (int32_t)(2u * NS)) {
 #ifdef CCD_PROFILE
+                    // a failed round that leaves for want of ready symbols is timed (and counted in n_fail) here
+                    const long long dt = clock64() - tr;
                     cp.n_starve++;
-                    cp.rare += clock64() - tr;
+                    cp.rare += dt;
+                    if (miss_) {
+                        cp.fail += dt;
+                        cp.n_fail++;
+                    }
 #endif
                     break;
                 }
@@ -1189,13 +1216,20 @@ __device__ __forceinline__ void coder_grid_spec(const SLoc &S, const SmemLayout 
     // (the steady loop less its rare path), failed rounds of the steady loop timed from the loop's exit to the start of
     // the next round, the decided-prefix symbols of all failed rounds, the steady loop's window moves, its reads of
     // `ready` and its exits for want of ready symbols, waits of the outer loop, one-round steps (matched ones counted
-    // apart) and single-symbol steps, and the steady loop's rare path in all (from each exit to the next round or out)
+    // apart) and single-symbol steps, and the steady loop's rare path in all (from each exit to the next round or out);
+    // then the CTA (the stream's index in its launch), every failed round by where it ran (steady round A, round B,
+    // one-round path) and decided prefix 0 / 1 / 2, failed rounds followed by a window move, failed rounds that took
+    // the exact model, single-symbol steps through tier 2 and those that took the exact model.  Every symbol of the
+    // grid is in exactly one of: 3 per matched round, a failed round's prefix and its far symbol, a single step.
     if (lane == 0)
         printf("CCDPROF grid_begin %u n %u steady %lld %u fail %lld %u pre %u move %u ref %u starve %u wait %lld %u "
-               "one %lld %u %u single %lld %u rare %lld\n",
+               "one %lld %u %u single %lld %u rare %lld cta %u fail_a %u %u %u fail_b %u %u %u fail_one %u %u %u "
+               "fail_move %u fail_exact %u tier %u exact %u\n",
                ord_begin, ord_end - ord_begin, cp.steady - cp.rare, cp.n_steady, cp.fail, cp.n_fail, cp.n_pre,
                cp.n_move, cp.n_ref, cp.n_starve, cp.wait, cp.n_wait, cp.one, cp.n_one, cp.n_one_ok, cp.single,
-               cp.n_single, cp.rare);
+               cp.n_single, cp.rare, blockIdx.x, cp.fails[0], cp.fails[1], cp.fails[2], cp.fails[3], cp.fails[4],
+               cp.fails[5], cp.fails[6], cp.fails[7], cp.fails[8], cp.n_fail_move,
+               cp.n_fail_exact, cp.n_single_t2, cp.n_single_exact);
 #endif
     c.D = D;
     c.R = R;

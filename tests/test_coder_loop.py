@@ -13,9 +13,11 @@ symbols placed in coding order:
   move        sigma min and gaps 1 ... 4: every far symbol costs about a word, so the word window moves every few
               rounds, and the move coincides with a failed round;
   exact       far symbols outside the window: the exact model decides the first undecided symbol of a failed round.
-Each stream is decoded under the default, a one-warp and an all-warp producer mask (the one-warp mask lets `ready` lag
-the coder on the long grid, so that the loop leaves for want of ready symbols), and must equal the oracle bit for bit,
-status words included: [1] words consumed and [2] the symbols decided by the exact model."""
+Each stream is decoded under the default, a one-warp and an all-warp producer mask, and must equal the oracle bit for
+bit, status words included: [1] words consumed and [2] the symbols decided by the exact model.  Under the one-warp
+mask the producers fall so far behind that on `positions` and `move` the coder never enters the steady loop (one-round
+and single-symbol steps only); on `back2back` and `exact` the loop runs and leaves for want of ready symbols (about
+1 400 and 2 800 times on an H100).  tests/test_coder_paths.py counts these paths on the device."""
 import numpy as np
 import pytest
 from test_entropy_edges import (DB28, WIN_HALF, Model, _check_stream, _oracle_backend, build_stream, classes,  # noqa: F401

@@ -50,7 +50,8 @@ def prof_table(text):
         if line.startswith("CCDPROF"):
             v = [int(x) for x in re.findall(r"-?\d+", line)]
             rows.append(dict(zip(("ord", "n", "st_c", "st_n", "fa_c", "fa_n", "pre", "mv_n", "rf_n", "sv_n", "wt_c", "wt_n",
-                                  "one_c", "one_n", "one_ok", "sg_c", "sg_n", "rare_c"), v)))
+                                  "one_c", "one_n", "one_ok", "sg_c", "sg_n", "rare_c", "cta", "a0", "a1", "a2", "b0",
+                                  "b1", "b2", "o0", "o1", "o2", "fmove", "fexact", "tier", "sexact"), v)))
     if not rows:
         return
     print("coder warp per grid (decode order; kcyc = kilo-cycles; cyc/x = cycles per round / case):")
@@ -69,6 +70,14 @@ def prof_table(text):
     print("  matched: the steady loop less its rare path; fail: failed rounds of the steady loop, from the loop's exit "
           "to the next round; move: window moves; ready: reads of `ready` in the steady loop; starve: exits for want "
           "of ready symbols; rare: the steady loop's rare path in all")
+    print("failed rounds by path and decided prefix 0/1/2 (A, B: the steady loop's two rounds; one: the one-round path):")
+    print("%6s | %14s %14s %14s | %9s %10s | %7s %6s" % ("grid", "A", "B", "one", "fail+move", "fail exact", "tier 2",
+                                                       "exact"))
+    for name, r in [(str(i), r) for i, r in enumerate(rows)] + [("all", tot)]:
+        print("%6s | %4d %4d %4d %4d %4d %4d %4d %4d %4d | %9d %10d | %7d %6d"
+              % (name, r["a0"], r["a1"], r["a2"], r["b0"], r["b1"], r["b2"], r["o0"], r["o1"], r["o2"], r["fmove"],
+                 r["fexact"], r["tier"], r["sexact"]))
+    print("  tier 2 / exact: single-symbol steps through tier 2 / with the exact model")
 
 
 for it in range(3):

@@ -1,14 +1,15 @@
 """Quality analysis of a Cool-chic bitstream against its source: PSNR per plane and per frame, rate, and the
 prediction statistics of P / B frames, with the reference encoder's column names.
 
-    python cc_eval.py -i <bitstream.cool> --original <src.yuv|png|ppm> [--frame_offset N] [--ms_ssim] [--maps out.npz]
+    python cc_eval.py -i <bitstream.cool> --original <src.yuv|png|ppm> [--frame_offset N] [--ms_ssim] [--vif] [--maps out.npz]
                       [--grids] [--motion] [--device N]
 
 Display frame i is compared with source frame frame_offset + i.  ``--maps`` writes, per frame, the error map
 (sum over planes of the squared integer errors / (2^b - 1)^2, chroma at (y >> 1, x >> 1) for 4:2:0) and for P / B
 frames the alpha, beta and prediction maps.  ``--ms_ssim`` appends MS-SSIM columns (whole frame, in dB, per plane;
 ``n/a`` for a frame with a plane smaller than 176 x 176) and a mean line, and with ``--maps`` the scale-0 SSIM map of
-every plane.  ``--grids`` appends, per frame and per Cool-chic, a table of its latent grids: size, model bits and bpp,
+every plane.  ``--vif`` appends VIF columns (whole frame and per plane; ``n/a`` for a frame with a plane smaller than
+41 x 41 or a flat source plane) and a mean line.  ``--grids`` appends, per frame and per Cool-chic, a table of its latent grids: size, model bits and bpp,
 the frame PSNR with the grid alone read as zeros and its change from the decoded frame's, and for the residue the PSNR
 with only the synthesis grids from the coarsest down to that one kept (DESIGN §4.7).  The grid analysis decodes the
 bitstream a second time, after the quality table.
@@ -30,6 +31,7 @@ from coolchic_b200.bitstream.quality import video_quality
 COLUMNS = ["frame_idx", "frame_type", "psnr_db", "psnr_y_db", "psnr_u_db", "psnr_v_db", "rate_bpp", "alpha_mean",
            "beta_mean", "pred_psnr_db", "dummy_pred_psnr_db"]
 MS_SSIM_COLUMNS = ["ms_ssim", "ms_ssim_db", "ms_ssim_y", "ms_ssim_u", "ms_ssim_v"]
+VIF_COLUMNS = ["vif", "vif_y", "vif_u", "vif_v"]
 MOTION_COLUMNS = ["variant", "psnr_db", "psnr_y_db", "psnr_u_db", "psnr_v_db", "delta_db"]
 GRID_COLUMNS = ["grid", "size", "hyper", "bits", "bpp", "drop_psnr_db", "drop_delta_db", "coarse_psnr_db"]
 
@@ -45,6 +47,7 @@ if __name__ == "__main__":
     parser.add_argument("--frame_offset", type=int, default=0, help="Source frame of the first displayed frame.")
     parser.add_argument("--maps", type=str, default=None, help="Write the error / alpha / beta / prediction maps here (.npz).")
     parser.add_argument("--ms_ssim", action="store_true", help="Also report MS-SSIM.")
+    parser.add_argument("--vif", action="store_true", help="Also report VIF (visual information fidelity).")
     parser.add_argument("--grids", action="store_true", help="Also report what each latent grid costs and buys.")
     parser.add_argument("--motion", action="store_true", help="Also report what the motion, each reference and the "
                         "residue of every P / B frame buy.")
@@ -53,8 +56,9 @@ if __name__ == "__main__":
 
     with open(args.input, "rb") as f_in:
         frames = video_quality(f_in.read(), args.original, frame_offset=args.frame_offset, device=args.device,
-                               want_maps=args.maps is not None, ms_ssim=args.ms_ssim, motion=args.motion)
-    columns = COLUMNS + (MS_SSIM_COLUMNS if args.ms_ssim else [])
+                               want_maps=args.maps is not None, ms_ssim=args.ms_ssim, motion=args.motion,
+                               vif=args.vif)
+    columns = COLUMNS + (MS_SSIM_COLUMNS if args.ms_ssim else []) + (VIF_COLUMNS if args.vif else [])
     print(" ".join(f"{c:<18}" for c in columns))
     for key, q in frames.items():
         vals = [key, q.frame_type] + [_fmt(getattr(q, c)) for c in columns[2:]]
@@ -66,6 +70,9 @@ if __name__ == "__main__":
     if args.ms_ssim:
         have = [q.ms_ssim for q in frames.values() if q.ms_ssim is not None]
         print(f"mean ms_ssim {_fmt(sum(have) / len(have) if have else None)}  ({len(have)} of {len(frames)} frames)")
+    if args.vif:
+        have = [q.vif for q in frames.values() if q.vif is not None]
+        print(f"mean vif {_fmt(sum(have) / len(have) if have else None)}  ({len(have)} of {len(frames)} frames)")
     if args.maps:
         maps = {}
         for key, q in frames.items():

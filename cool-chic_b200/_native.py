@@ -28,7 +28,7 @@ EXPORTS = [
     "ccd_version", "ccd_sizeof_desc", "ccd_last_error", "ccd_create", "ccd_destroy", "ccd_nn_count",
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
     "ccd_encode_latents", "ccd_synthesize_many", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
-    "ccd_latent_rate", "ccd_latent_rate_edited", "ccd_rate_sweep", "ccd_rate_candidates", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_inter_stats", "ccd_inter_analysis",
+    "ccd_latent_rate", "ccd_latent_rate_edited", "ccd_rate_sweep", "ccd_rate_candidates", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_frame_vif", "ccd_inter_stats", "ccd_inter_analysis",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
     "ccd_debug_entropy_plan", "ccd_debug_cdf_table", "ccd_debug_detmath", "ccd_debug_sinc_coeffs", "ccd_debug_cr_noise",
 ]
@@ -162,6 +162,22 @@ class CcdSsimJob(ctypes.Structure):
     ]
 
 
+class CcdVifJob(ctypes.Structure):
+    _fields_ = [
+        ("d_planes", ctypes.c_void_p * 3),
+        ("d_src", ctypes.c_void_p),
+        ("h", ctypes.c_int32),
+        ("w", ctypes.c_int32),
+        ("chroma_shift", ctypes.c_int32),
+        ("bitdepth", ctypes.c_int32),
+        ("src_layout", ctypes.c_int32),
+        ("num", (ctypes.c_double * 4) * 3),
+        ("den", (ctypes.c_double * 4) * 3),
+        ("bad_index", ctypes.c_int64),
+        ("status", ctypes.c_int32),
+    ]
+
+
 class CcdInterFrame(ctypes.Structure):
     _fields_ = [
         ("d_residue", ctypes.c_void_p),
@@ -279,6 +295,8 @@ def load_library():
         L.ccd_frame_distortion.argtypes = [vp, ctypes.POINTER(CcdDistJob), ci, vp]
         L.ccd_frame_ssim.restype = ci
         L.ccd_frame_ssim.argtypes = [vp, ctypes.POINTER(CcdSsimJob), ci, vp]
+        L.ccd_frame_vif.restype = ci
+        L.ccd_frame_vif.argtypes = [vp, ctypes.POINTER(CcdVifJob), ci, vp]
         L.ccd_inter_stats.restype = ci
         L.ccd_inter_stats.argtypes = [vp, ctypes.POINTER(CcdInterFrame), ctypes.POINTER(CcdInterStats), vp]
         L.ccd_inter_analysis.restype = ci
@@ -755,7 +773,7 @@ class Context:
 
     def _frame_jobs(self, job_type, frames, sources, layouts):
         """The job array of a call that compares finished frames with their source samples (frame_distortion,
-        frame_ssim), the tensors it points into, and each frame's planes."""
+        frame_ssim, frame_vif), the tensors it points into, and each frame's planes."""
         n = len(frames)
         jobs = (job_type * n)()
         keep, planes = [], []
@@ -819,6 +837,17 @@ class Context:
             res[i]["cs"] = [list(jobs[i].cs[c]) for c in range(3)]
             res[i]["ssim"] = [list(jobs[i].ssim[c]) for c in range(3)]
         return res
+
+    def frame_vif(self, frames, sources: Sequence[torch.Tensor], layouts: Sequence[str]) -> List[dict]:
+        """VIF statistics of finished frames against their source samples (``ccd_frame_vif``), four launches for all
+        (one per scale).  Arguments as for frame_distortion; every plane needs both sides >= 41.  Per frame a dict with
+        ``num`` and ``den``: per plane, the four per-scale sums of the VIF numerator and denominator terms (f64, the
+        same on every run)."""
+        n = len(frames)
+        jobs, keep, _ = self._frame_jobs(CcdVifJob, frames, sources, layouts)
+        _check(self._lib.ccd_frame_vif(self._h, jobs, n, self._stream()), jobs)
+        return [{"num": [list(jobs[i].num[c]) for c in range(3)], "den": [list(jobs[i].den[c]) for c in range(3)]}
+                for i in range(n)]
 
     def inter_stats(self, residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow, warp_filter_size,
                     source: Optional[torch.Tensor] = None, layout: str = "planar", want_maps: bool = False) -> dict:

@@ -18,6 +18,11 @@ On request, the motion analysis of every P / B frame (``bitstream/motion.py``, D
 On request, MS-SSIM (Wang, Simoncelli and Bovik 2003; DESIGN §4.6) from the same integers: one ``ccd_frame_ssim`` call
 for every frame whose planes all have both sides of at least 176 samples (five scales of at least 11), formed per plane
 on the host from the per-scale means, and per frame the pixel-weighted mean over the planes.  Smaller frames get None.
+
+On request, VIF (Sheikh and Bovik 2006, the multi-scale pixel-domain vifp_mscale; DESIGN §4.12) from the same
+integers in 8-bit units: one ``ccd_frame_vif`` call for every frame whose planes all have both sides of at least 41
+samples (a valid output at the fourth scale), per plane sum_s num_s / sum_s den_s, and per frame the pixel-weighted
+mean over the planes.  Smaller frames, and frames with a flat source plane (no VIF), get None.
 """
 import math
 from dataclasses import dataclass, field
@@ -57,6 +62,21 @@ def ms_ssim_from_scales(cs: List[float], ssim: List[float]) -> float:
     return v * max(ssim[4], 0.0) ** w[4]
 
 
+VIF_MIN_SIDE = 41  # scales 0..3: 41 -> 17 -> 7 -> 3 samples, and 3 taps at the last
+
+
+def vif_from_scales(num: List[float], den: List[float]) -> Optional[float]:
+    """VIF of one plane from its four per-scale sums: sum num / sum den; None for a flat source plane (sum den = 0)."""
+    d = sum(den)
+    return None if d == 0 else sum(num) / d
+
+
+def vif_applies(img_size, frame_data_type: str) -> bool:
+    """Whether every plane of an (h, w) frame has both sides >= 41 (4:2:0 chroma: (h / 2, w / 2))."""
+    cs = 1 if frame_data_type == "yuv420" else 0
+    return min(img_size) >> cs >= VIF_MIN_SIDE
+
+
 def ms_ssim_applies(img_size, frame_data_type: str) -> bool:
     """Whether every plane of an (h, w) frame has both sides >= 176 (4:2:0 chroma: (h / 2, w / 2))."""
     cs = 1 if frame_data_type == "yuv420" else 0
@@ -85,6 +105,7 @@ class FrameQuality:
     pred_map: Optional[torch.Tensor] = None    # [3, H, W] (P / B)
     ms_ssim_planes: Optional[List[float]] = None        # per plane; None: not asked for, or a plane below 176
     ssim_maps: Optional[List[torch.Tensor]] = None      # per plane, [h_c - 10, w_c - 10] scale-0 SSIM map
+    vif_planes: Optional[List[Optional[float]]] = None  # per plane (None: flat source); None: not asked for, or below 41
     motion: Optional["MotionAnalysis"] = None  # noqa: F821  (bitstream/motion.py; P / B frames with motion=True)
     plane_mse: List[float] = field(init=False)
 
@@ -125,6 +146,17 @@ class FrameQuality:
     ms_ssim_y = property(lambda self: None if self.ms_ssim_planes is None else self.ms_ssim_planes[0])
     ms_ssim_u = property(lambda self: None if self.ms_ssim_planes is None else self.ms_ssim_planes[1])
     ms_ssim_v = property(lambda self: None if self.ms_ssim_planes is None else self.ms_ssim_planes[2])
+
+    @property
+    def vif(self) -> Optional[float]:
+        """Pixel-weighted mean of the planes' VIF (the rule of ms_ssim); None if a plane has none."""
+        if self.vif_planes is None or any(v is None for v in self.vif_planes):
+            return None
+        return sum(n * v for n, v in zip(self.n_samples, self.vif_planes)) / sum(self.n_samples)
+
+    vif_y = property(lambda self: None if self.vif_planes is None else self.vif_planes[0])
+    vif_u = property(lambda self: None if self.vif_planes is None else self.vif_planes[1])
+    vif_v = property(lambda self: None if self.vif_planes is None else self.vif_planes[2])
 
 
 def _frame_layout(buf, max_decoding_order: int):
@@ -183,12 +215,13 @@ def _upload_sources(ctx, by_display):
 @torch.no_grad()
 def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int = 0, max_decoding_order: int = -1,
                   device: int = 0, want_maps: bool = False, ms_ssim: bool = False,
-                  motion: bool = False) -> Dict[str, FrameQuality]:
+                  motion: bool = False, vif: bool = False) -> Dict[str, FrameQuality]:
     """Quality of every frame of an image / video bitstream against its source file (.yuv / .png / .ppm):
     ``{str(display_idx): FrameQuality}`` in display order.  ``ms_ssim`` adds MS-SSIM for every frame whose planes
     all have both sides >= 176 (``ms_ssim_planes`` stays None for the others), with the SSIM maps if ``want_maps``.
     ``motion`` fills ``FrameQuality.motion`` of every P / B frame (a MotionAnalysis, with the flow maps if
-    ``want_maps``); I frames keep None.  A source whose format, bitdepth or size differs from the
+    ``want_maps``); I frames keep None.  ``vif`` adds VIF for every frame whose planes all have both sides >= 41
+    (``vif_planes`` stays None for the others).  A source whose format, bitdepth or size differs from the
     decoded frames, or that has too few frames, raises ValueError before anything runs on the device."""
     frames = _frame_layout(memoryview(bytes(bitstream_bytes)), max_decoding_order)
     by_display = _read_sources(frames, original_path, frame_offset)
@@ -234,6 +267,13 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
             res = ctx.frame_ssim([decoded[str(d)] for d in big], [sources[d] for d in big],
                                  [by_display[d][3].layout for d in big], want_maps=want_maps)
             ssim = dict(zip(big, res))
+    vifs = {}
+    if vif:
+        big = [d for d in order if vif_applies(by_display[d][3].img_size, by_display[d][3].frame_data_type)]
+        if big:
+            res = ctx.frame_vif([decoded[str(d)] for d in big], [sources[d] for d in big],
+                                [by_display[d][3].layout for d in big])
+            vifs = dict(zip(big, res))
     out = {}
     for d, r in zip(order, dist):
         _, fh, n_bytes, s = by_display[d]
@@ -254,5 +294,7 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
         if d in ssim:
             q.ms_ssim_planes = [ms_ssim_from_scales(c, s_) for c, s_ in zip(ssim[d]["cs"], ssim[d]["ssim"])]
             q.ssim_maps = ssim[d].get("maps")
+        if d in vifs:
+            q.vif_planes = [vif_from_scales(n_, d_) for n_, d_ in zip(vifs[d]["num"], vifs[d]["den"])]
         out[str(d)] = q
     return out

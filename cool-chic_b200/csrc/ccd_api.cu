@@ -430,7 +430,7 @@ struct CcdContext {
     float *d_scale = nullptr;
     uint32_t *d_cdf = nullptr;
     DeviceBuf upload;   // words / blobs / stream structs / statuses / synthesis weights
-    DeviceBuf scratch;  // synthesis intermediates, latents when the caller does not want them, MS-SSIM pyramid levels
+    DeviceBuf scratch;  // synthesis intermediates, latents when the caller does not want them, MS-SSIM and VIF pyramid levels
     DeviceBuf zeros;    // all zero: the latents of the grids a synthesis job masks
     unsigned char *h_pin = nullptr;
     size_t h_pin_cap = 0;
@@ -2066,7 +2066,7 @@ int ccd_rate_sweep(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, void *cuda_st
     return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return rate_sweep_body(ctx, jobs, n_jobs, st); });
 }
 
-// The checks of a job that compares a finished frame with its source samples (CcdDistJob, CcdSsimJob)
+// The checks of a job that compares a finished frame with its source samples (CcdDistJob, CcdSsimJob, CcdVifJob)
 extern "C++" template <class Job>
 int check_frame_job(Job &J, int i) {
     J.bad_index = -1;
@@ -2226,6 +2226,97 @@ static int frame_ssim_body(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, cudaSt
 
 int ccd_frame_ssim(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, void *cuda_stream) {
     return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return frame_ssim_body(ctx, jobs, n_jobs, st); });
+}
+
+static int frame_vif_body(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, cudaStream_t st) {
+    constexpr int S = CCD_VIF_SCALES;
+    const size_t n = (size_t)n_jobs;
+    auto side = [&](int i, int c, int s, bool width) {  // plane c of job i at scale s
+        const CcdVifJob &J = jobs[i];
+        return ccd_vif_side((width ? J.w : J.h) >> (c ? J.chroma_shift : 0), s);
+    };
+    auto tiles = [&](int i, int c, int s) { return ccd_ssim_tiles(side(i, c, s, false), side(i, c, s, true)); };
+    // the job's partials at scale s start at part_at[i * S + s] (pairs, planes in order); scales 1..3 of every plane of
+    // every job, one after the other, in the context's scratch
+    std::vector<size_t> part_at(n * S);
+    size_t n_part = 0, pyr_bytes = 0;
+    int max_tiles[S] = {0, 0, 0, 0};
+    for (int i = 0; i < n_jobs; i++) {
+        if (int rc = check_frame_job(jobs[i], i)) return rc;
+        for (int c = 0; c < 3; c++)  // a valid output at the last scale: both sides >= 41
+            if (std::min(side(i, c, S - 1, false), side(i, c, S - 1, true)) < ccd_vif_taps(S - 1))
+                return jobs[i].status = fail(CCD_ERR_ARG, "job %d: plane %d is %dx%d, VIF needs both sides >= 41", i, c,
+                                             side(i, c, 0, true), side(i, c, 0, false));
+        for (int s = 0; s < S; s++) {
+            part_at[(size_t)i * S + s] = n_part;
+            const int t = tiles(i, 0, s) + tiles(i, 1, s) + tiles(i, 2, s);
+            max_tiles[s] = std::max(max_tiles[s], t);
+            n_part += (size_t)t;
+            for (int c = 0; s > 0 && c < 3; c++) pyr_bytes += al(sizeof(double2) * (size_t)side(i, c, s, false) * side(i, c, s, true));
+        }
+    }
+    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
+    // the job array, then the results: bad[n] ~0, then the partials, which are not uploaded
+    Arena A;
+    const size_t off_jobs = A.take(sizeof(VifJobDev) * n), off_bad = A.take(8 * n, 8);
+    const size_t off_part = A.take(2 * sizeof(double) * n_part, 8);
+    if (int rc = stage(ctx, A)) return rc;
+    if (int rc = ensure_dev(ctx->scratch, pyr_bytes)) return rc;
+    memset(A.h + off_bad, 0xff, 8 * n);
+    double *d_part = reinterpret_cast<double *>(A.dv + off_part);
+    unsigned char *pyr = ctx->scratch.p;
+    for (int i = 0; i < n_jobs; i++) {
+        const CcdVifJob &J = jobs[i];
+        VifJobDev D;
+        memset(&D, 0, sizeof(D));
+        for (int c = 0; c < 3; c++) D.p[c] = J.d_planes[c];
+        for (int s = 0; s < S; s++) {
+            D.part[s] = d_part + 2 * part_at[(size_t)i * S + s];
+            for (int c = 0; s > 0 && c < 3; c++) {
+                D.lvl[c][s] = reinterpret_cast<double2 *>(pyr);
+                pyr += al(sizeof(double2) * (size_t)side(i, c, s, false) * side(i, c, s, true));
+            }
+        }
+        D.src = J.d_src;
+        D.h = J.h;
+        D.w = J.w;
+        D.cs = J.chroma_shift;
+        D.hwc = J.src_layout;
+        D.wide = J.bitdepth > 8;
+        D.Md = (double)((1 << J.bitdepth) - 1);
+        D.M = (float)D.Md;
+        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
+        memcpy(A.h + off_jobs + sizeof(VifJobDev) * (size_t)i, &D, sizeof(D));
+    }
+    double g[S][17] = {};  // scale s: N_s taps of a Gaussian with sigma N_s / 5, normalised to sum 1
+    for (int s = 0; s < S; s++) {
+        const int N = ccd_vif_taps(s);
+        const double sigma = N / 5.0;
+        double gs = 0.0;
+        for (int k = 0; k < N; k++) gs += (g[s][k] = std::exp(-(double)((2 * k - (N - 1)) * (2 * k - (N - 1))) / (8.0 * sigma * sigma)));
+        for (int k = 0; k < N; k++) g[s][k] /= gs;
+    }
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
+    int e = ccd_vif_launch(reinterpret_cast<const VifJobDev *>(A.dv + off_jobs), n_jobs, max_tiles, g, st);
+    if (e != 0) return fail(CCD_ERR_CUDA, "VIF launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    if (int rc = download(A, off_bad, st, "VIF")) return rc;
+    const double *part = reinterpret_cast<const double *>(A.h + off_part);
+    for (int i = 0; i < n_jobs; i++) {
+        for (int s = 0; s < S; s++) {
+            const double *p = part + 2 * part_at[(size_t)i * S + s];  // the planes' tiles in order
+            for (int c = 0; c < 3; c++) {
+                const size_t t = (size_t)tiles(i, c, s);
+                jobs[i].num[c][s] = ordered_sum(p, t, 2);
+                jobs[i].den[c][s] = ordered_sum(p + 1, t, 2);
+                p += 2 * t;
+            }
+        }
+    }
+    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) { return off_grid_error(jobs[i], i); });
+}
+
+int ccd_frame_vif(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, void *cuda_stream) {
+    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return frame_vif_body(ctx, jobs, n_jobs, st); });
 }
 
 int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitdepth, int data_type, float *d_out_a,

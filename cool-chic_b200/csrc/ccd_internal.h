@@ -317,6 +317,30 @@ static __host__ __device__ __forceinline__ int ccd_ssim_tiles(int h, int w) {
 int ccd_ssim_launch(const SsimJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_SSIM_SCALES], const double g[11],
                     cudaStream_t st);
 
+// VIF (DESIGN §4.12): one k_frame_vif<s> launch per scale, tiles as for MS-SSIM (ccd_ssim_tiles over the plane at scale
+// s); a tile stages CCD_SSIM_T + N_s - 1 rows and columns of both images and writes its share of scale s + 1.
+#define CCD_VIF_SCALES 4
+struct VifJobDev {
+    const float *p[3];          // finished planes (FrameData layout), read at scale 0
+    const void *src;            // source samples as for DistJobDev
+    double2 *lvl[3][CCD_VIF_SCALES];  // scales 1..3 per plane: (decoded, source) in 8-bit units
+    double *part[CCD_VIF_SCALES];     // per scale: (sum num, sum den) of each of the job's tiles, in tile order
+    int32_t h, w, cs, hwc, wide;
+    float M;
+    double Md;                  // M in f64: a sample k is v = k * 255 / M
+    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
+};
+// the window of scale s: N_s = 2^(4 - s) + 1 taps
+static __host__ __device__ __forceinline__ constexpr int ccd_vif_taps(int s) { return (1 << (4 - s)) + 1; }
+// a side of n samples at scale 0 is this many at scale s: filtered "valid" with N_s taps, then every other sample
+static __host__ __device__ __forceinline__ int ccd_vif_side(int n, int s) {
+    for (int t = 1; t <= s; t++) n = (n - ccd_vif_taps(t) + 2) >> 1;
+    return n;
+}
+// four launches; max_tiles[s]: the most tiles of one job at scale s; g[s]: the N_s taps of scale s
+int ccd_vif_launch(const VifJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_VIF_SCALES], const double g[CCD_VIF_SCALES][17],
+                   cudaStream_t st);
+
 // P/B reconstruction (ccd_inter.cu); returns -1 for an unsupported filter size
 struct InterLaunch {
     const float *residue, *motion;  // [4|5][h][w], [2|4][h][w]

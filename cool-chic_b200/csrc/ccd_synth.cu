@@ -1601,27 +1601,111 @@ int ccd_dist_launch(const DistJobDev *d_jobs, int n_jobs, int64_t max_pixels, in
     return (int)cudaGetLastError();
 }
 
-// ---- MS-SSIM against the source (DESIGN §4.6), one scale per launch.  x = the decoded image, y = the source, both as
-// the integer sums S_j of the 4^j samples a level-j sample covers: below 65535 * 256 < 2^24, so staged exactly in fp32
-// (68 KB of shared memory: three CTAs per SM); every moment is formed in f64 on S_j and scaled by 4^-j or 16^-j
-// afterwards, which is exact.  Per tile: stage (T + 10)^2 samples of both images, write the next level's T/2 x T/2
-// samples, filter the five moments horizontally then vertically (11 taps, valid positions only), and add cs and
-// l * cs of the tile's valid positions in a fixed order into one f64 partial each.
+// ---- Tiled local statistics against the source: MS-SSIM (DESIGN §4.6) and VIF (§4.12), one scale per launch.  A CTA
+// of kTileWarps warps takes one CCD_SSIM_T x CCD_SSIM_T tile of one plane at one scale, stages it with its halo, forms
+// the five local moments x, y, x^2, y^2, x y with a separable window, and reduces two per-pixel terms to one f64
+// partial each, in a fixed order.
+namespace {
+constexpr int kTileWarps = 8;
+constexpr int kTileK = 4;  // consecutive outputs per thread in either moment pass
+static_assert(CCD_SSIM_T == 32 && CCD_SSIM_T / kTileK == kTileWarps, "vertical pass: lane = column, warp = K rows");
+static_assert((CCD_SSIM_T / 2) * (CCD_SSIM_T / 2) == 32 * kTileWarps, "one next-level sample per thread");
+}  // namespace
+
+static __device__ __forceinline__ void report_bad(unsigned long long bad, unsigned long long *out, int tid) {
+    for (int o = 16; o > 0; o >>= 1) bad = min(bad, __shfl_down_sync(0xffffffffu, bad, o));
+    if ((tid & 31) == 0 && bad != ~0ull) atomicMin(out, bad);
+}
+
+// Horizontal pass: rows [0, In) of the staged [In][In] images sx, sy, filtered with the NT taps g at T positions per
+// row, into sh[5][In][T].  A thread takes K consecutive outputs of one row at a time.
+template <int NT, int In, class S>
+static __device__ __forceinline__ void moments_h(const S *sx, const S *sy, const double *g, double *sh, int tid) {
+    constexpr int T = CCD_SSIM_T, K = kTileK;
+    for (int task = tid; task < In * (T / K); task += 32 * kTileWarps) {
+        const int r = task / (T / K), q0 = task % (T / K) * K;
+        const S *rx = sx + r * In + q0, *ry = sy + r * In + q0;
+        double m[5][K];
+#pragma unroll
+        for (int k = 0; k < K; k++)
+#pragma unroll
+            for (int e = 0; e < 5; e++) m[e][k] = 0.0;
+#pragma unroll
+        for (int i = 0; i < K + NT - 1; i++) {
+            const double x = rx[i], y = ry[i], v[5] = {x, y, x * x, y * y, x * y};
+#pragma unroll
+            for (int k = 0; k < K; k++) {
+                if (i - k < 0 || i - k > NT - 1) continue;
+#pragma unroll
+                for (int e = 0; e < 5; e++) m[e][k] = fma(g[i - k], v[e], m[e][k]);
+            }
+        }
+#pragma unroll
+        for (int e = 0; e < 5; e++)
+#pragma unroll
+            for (int k = 0; k < K; k++) sh[(e * In + r) * T + q0 + k] = m[e][k];
+    }
+}
+
+// Vertical pass: the five moments of column q at rows r0 .. r0 + K - 1, from sh[5][In][T].
+template <int NT, int In>
+static __device__ __forceinline__ void moments_v(const double *sh, const double *g, int q, int r0, double (&m)[5][kTileK]) {
+    constexpr int T = CCD_SSIM_T, K = kTileK;
+#pragma unroll
+    for (int k = 0; k < K; k++)
+#pragma unroll
+        for (int e = 0; e < 5; e++) m[e][k] = 0.0;
+#pragma unroll
+    for (int i = 0; i < K + NT - 1; i++) {
+#pragma unroll
+        for (int e = 0; e < 5; e++) {
+            const double v = sh[(e * In + r0 + i) * T + q];
+#pragma unroll
+            for (int k = 0; k < K; k++)
+                if (i - k >= 0 && i - k <= NT - 1) m[e][k] = fma(g[i - k], v, m[e][k]);
+        }
+    }
+}
+
+// The CTA's two sums a, b, handed to thread 0's store(a, b): a lane butterfly, then the warps in order (sred: [warps][2])
+template <class Store>
+static __device__ __forceinline__ void tile_sums(double &a, double &b, double *sred, int tid, Store store) {
+    for (int o = 16; o > 0; o >>= 1) {
+        a += __shfl_xor_sync(0xffffffffu, a, o);
+        b += __shfl_xor_sync(0xffffffffu, b, o);
+    }
+    if ((tid & 31) == 0) {
+        sred[2 * (tid >> 5)] = a;
+        sred[2 * (tid >> 5) + 1] = b;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        double pa = 0.0, pb = 0.0;
+        for (int wi = 0; wi < kTileWarps; wi++) {
+            pa += sred[2 * wi];
+            pb += sred[2 * wi + 1];
+        }
+        store(pa, pb);
+    }
+}
+
+// ---- MS-SSIM.  x = the decoded image, y = the source, both as the integer sums S_j of the 4^j samples a level-j
+// sample covers: below 65535 * 256 < 2^24, so staged exactly in fp32 (68 KB of shared memory: three CTAs per SM);
+// every moment is formed in f64 on S_j and scaled by 4^-j or 16^-j afterwards, which is exact.  Per tile: stage
+// (T + 10)^2 samples of both images, write the next level's T/2 x T/2 samples, filter the five moments horizontally
+// then vertically (11 taps, valid positions only), and add cs and l * cs of the tile's valid positions in a fixed
+// order into one f64 partial each.
 namespace {
 constexpr int kSsimIn = CCD_SSIM_T + CCD_SSIM_HALO;  // staged rows and columns
-constexpr int kSsimK = 4;                            // consecutive outputs per thread in either pass
-constexpr int kSsimWarps = 8;
-constexpr size_t kSsimSmem = sizeof(float) * 2 * kSsimIn * kSsimIn + sizeof(double) * (5 * kSsimIn * CCD_SSIM_T + 2 * kSsimWarps);
-static_assert(CCD_SSIM_T == 32 && CCD_SSIM_T / kSsimK == kSsimWarps, "vertical pass: lane = column, warp = K rows");
-static_assert((CCD_SSIM_T / 2) * (CCD_SSIM_T / 2) == 32 * kSsimWarps, "one next-level sample per thread");
+constexpr size_t kSsimSmem = sizeof(float) * 2 * kSsimIn * kSsimIn + sizeof(double) * (5 * kSsimIn * CCD_SSIM_T + 2 * kTileWarps);
 struct SsimArgs {
     double g[11];
     int scale;
 };
 }  // namespace
 
-__global__ void __launch_bounds__(32 * kSsimWarps, 3) k_frame_ssim(const SsimJobDev *__restrict__ jobs, const SsimArgs a) {
-    constexpr int T = CCD_SSIM_T, K = kSsimK;
+__global__ void __launch_bounds__(32 * kTileWarps, 3) k_frame_ssim(const SsimJobDev *__restrict__ jobs, const SsimArgs a) {
+    constexpr int T = CCD_SSIM_T, K = kTileK;
     extern __shared__ double ssim_sm[];
     double *sh = ssim_sm;                                 // [5][kSsimIn][T]: the horizontal pass
     float *sx = reinterpret_cast<float *>(sh + 5 * kSsimIn * T), *sy = sx + kSsimIn * kSsimIn;  // [kSsimIn][kSsimIn]
@@ -1641,7 +1725,7 @@ __global__ void __launch_bounds__(32 * kSsimWarps, 3) k_frame_ssim(const SsimJob
 
     unsigned long long bad = ~0ull;
     const unsigned n0 = (unsigned)J.h * J.w, n1 = (unsigned)(J.h >> J.cs) * (unsigned)(J.w >> J.cs);
-    for (int i = tid; i < kSsimIn * kSsimIn; i += 32 * kSsimWarps) {
+    for (int i = tid; i < kSsimIn * kSsimIn; i += 32 * kTileWarps) {
         const int r = i / kSsimIn, q = i - r * kSsimIn, y = y0 + r, x = x0 + q;
         float vx = 0.0f, vy = 0.0f;  // integers below 2^24: exact
         if (y < h && x < w) {
@@ -1661,10 +1745,7 @@ __global__ void __launch_bounds__(32 * kSsimWarps, 3) k_frame_ssim(const SsimJob
         sx[i] = vx;
         sy[i] = vy;
     }
-    if (j == 0) {
-        for (int o = 16; o > 0; o >>= 1) bad = min(bad, __shfl_down_sync(0xffffffffu, bad, o));
-        if ((tid & 31) == 0 && bad != ~0ull) atomicMin(J.bad, bad);
-    }
+    if (j == 0) report_bad(bad, J.bad, tid);
     __syncthreads();
 
     if (j + 1 < CCD_SSIM_SCALES) {  // the next level: floor sizes, an odd last row or column is dropped
@@ -1677,51 +1758,15 @@ __global__ void __launch_bounds__(32 * kSsimWarps, 3) k_frame_ssim(const SsimJob
         }
     }
 
-    // horizontal pass: x, y, x^2, y^2, x y (the f64 products are exact: S_j < 2^24) over 11 columns
-    for (int task = tid; task < kSsimIn * (T / K); task += 32 * kSsimWarps) {
-        const int r = task / (T / K), q0 = task % (T / K) * K;
-        const float *rx = sx + r * kSsimIn + q0, *ry = sy + r * kSsimIn + q0;
-        double m[5][K];
-#pragma unroll
-        for (int k = 0; k < K; k++)
-#pragma unroll
-            for (int e = 0; e < 5; e++) m[e][k] = 0.0;
-#pragma unroll
-        for (int i = 0; i < K + 10; i++) {
-            const double x = rx[i], y = ry[i], v[5] = {x, y, x * x, y * y, x * y};
-#pragma unroll
-            for (int k = 0; k < K; k++) {
-                if (i - k < 0 || i - k > 10) continue;
-#pragma unroll
-                for (int e = 0; e < 5; e++) m[e][k] = fma(a.g[i - k], v[e], m[e][k]);
-            }
-        }
-#pragma unroll
-        for (int e = 0; e < 5; e++)
-#pragma unroll
-            for (int k = 0; k < K; k++) sh[(e * kSsimIn + r) * T + q0 + k] = m[e][k];
-    }
+    // the f64 products of the horizontal pass are exact: S_j < 2^24
+    moments_h<11, kSsimIn>(sx, sy, a.g, sh, tid);
     __syncthreads();
 
-    // vertical pass: lane = column, warp = K consecutive output rows
     double s_cs = 0.0, s_ssim = 0.0;
     {
         const int q = tid & 31, r0 = (tid >> 5) * K;
         double m[5][K];
-#pragma unroll
-        for (int k = 0; k < K; k++)
-#pragma unroll
-            for (int e = 0; e < 5; e++) m[e][k] = 0.0;
-#pragma unroll
-        for (int i = 0; i < K + 10; i++) {
-#pragma unroll
-            for (int e = 0; e < 5; e++) {
-                const double v = sh[(e * kSsimIn + r0 + i) * T + q];
-#pragma unroll
-                for (int k = 0; k < K; k++)
-                    if (i - k >= 0 && i - k <= 10) m[e][k] = fma(a.g[i - k], v, m[e][k]);
-            }
-        }
+        moments_v<11, kSsimIn>(sh, a.g, q, r0, m);
         const double s1 = ldexp(1.0, -2 * j), s2 = __dmul_rn(s1, s1);
         const int x = x0 + q, wo = w - CCD_SSIM_HALO, ho = h - CCD_SSIM_HALO;
 #pragma unroll
@@ -1741,24 +1786,10 @@ __global__ void __launch_bounds__(32 * kSsimWarps, 3) k_frame_ssim(const SsimJob
             if (j == 0 && J.map[c]) J.map[c][(size_t)y * wo + x] = __double2float_rn(ls);
         }
     }
-    for (int o = 16; o > 0; o >>= 1) {  // lane butterfly, then the warps in order
-        s_cs += __shfl_xor_sync(0xffffffffu, s_cs, o);
-        s_ssim += __shfl_xor_sync(0xffffffffu, s_ssim, o);
-    }
-    if ((tid & 31) == 0) {
-        sred[2 * (tid >> 5)] = s_cs;
-        sred[2 * (tid >> 5) + 1] = s_ssim;
-    }
-    __syncthreads();
-    if (tid == 0) {
-        double pc = 0.0, ps = 0.0;
-        for (int wi = 0; wi < kSsimWarps; wi++) {
-            pc += sred[2 * wi];
-            ps += sred[2 * wi + 1];
-        }
+    tile_sums(s_cs, s_ssim, sred, tid, [&](double pc, double ps) {
         J.part[j][2 * blockIdx.x] = pc;
         J.part[j][2 * blockIdx.x + 1] = ps;
-    }
+    });
 }
 
 int ccd_ssim_launch(const SsimJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_SSIM_SCALES], const double g[11],
@@ -1769,11 +1800,162 @@ int ccd_ssim_launch(const SsimJobDev *d_jobs, int n_jobs, const int max_tiles[CC
     memcpy(a.g, g, sizeof(a.g));
     for (int j = 0; j < CCD_SSIM_SCALES; j++) {  // scale j + 1 reads the level scale j wrote: stream order
         a.scale = j;
-        k_frame_ssim<<<dim3((unsigned)max_tiles[j], (unsigned)n_jobs, 1), 32 * kSsimWarps, kSsimSmem, st>>>(d_jobs, a);
+        k_frame_ssim<<<dim3((unsigned)max_tiles[j], (unsigned)n_jobs, 1), 32 * kTileWarps, kSsimSmem, st>>>(d_jobs, a);
         g_ccd_launches++;
         if ((e = cudaGetLastError()) != cudaSuccess) return (int)e;
     }
     return 0;
+}
+
+// ---- VIF.  x = the decoded image (distorted), y = the source (reference), both in 8-bit units and f64 from the start:
+// v = k * 255 / M at scale 0, the filtered and decimated values at scales 1..3.  Per tile of scale S: stage
+// (T + N_S - 1)^2 samples of both images (61 to 98 KB of shared memory: at least two CTAs per SM), write the next scale's
+// T/2 x T/2 samples (N_{S+1} taps each way, then the even rows and columns), filter the five moments horizontally then
+// vertically (N_S taps, valid positions only), and add the per-pixel num and den terms of the tile's valid positions in
+// a fixed order into one f64 partial each.
+namespace {
+template <int S>
+constexpr int kVifIn = CCD_SSIM_T + ccd_vif_taps(S) - 1;  // staged rows and columns
+template <int S>
+constexpr size_t kVifSmem = sizeof(double) * (2 * kVifIn<S> * kVifIn<S> + 5 * kVifIn<S> * CCD_SSIM_T + 2 * kTileWarps);
+struct VifArgs {
+    double g[17];   // this scale's N_S taps
+    double gn[9];   // the next scale's taps
+};
+}  // namespace
+
+template <int S>
+__global__ void __launch_bounds__(32 * kTileWarps, 2) k_frame_vif(const VifJobDev *__restrict__ jobs, const VifArgs a) {
+    constexpr int T = CCD_SSIM_T, K = kTileK, N = ccd_vif_taps(S), In = kVifIn<S>;
+    extern __shared__ double vif_sm[];
+    double *sh = vif_sm;                             // [5][In][T]: the horizontal pass
+    double *sx = sh + 5 * In * T, *sy = sx + In * In;  // [In][In]
+    double *sred = sy + In * In;                     // [warps][2]
+    const VifJobDev &J = jobs[blockIdx.y];
+    const int tid = (int)threadIdx.x;
+    int c = 0, t = (int)blockIdx.x, h = 0, w = 0;
+    for (;; c++) {  // the plane and tile of this CTA
+        if (c == 3) return;
+        h = ccd_vif_side(c ? J.h >> J.cs : J.h, S);
+        w = ccd_vif_side(c ? J.w >> J.cs : J.w, S);
+        const int n = ccd_ssim_tiles(h, w);
+        if (t < n) break;
+        t -= n;
+    }
+    const int tw = (w + T - 1) / T, y0 = t / tw * T, x0 = t % tw * T;
+
+    unsigned long long bad = ~0ull;
+    const unsigned n0 = (unsigned)J.h * J.w, n1 = (unsigned)(J.h >> J.cs) * (unsigned)(J.w >> J.cs);
+    for (int i = tid; i < In * In; i += 32 * kTileWarps) {
+        const int r = i / In, q = i - r * In, y = y0 + r, x = x0 + q;
+        double vx = 0.0, vy = 0.0;
+        if (y < h && x < w) {
+            const unsigned s = (unsigned)y * (unsigned)w + (unsigned)x;
+            if constexpr (S == 0) {
+                const DecodedSample D = read_decoded(J.p[c], s, J.M);
+                const unsigned pidx = c == 0 ? s : n0 + (unsigned)(c - 1) * n1 + s;  // as k_frame_dist reports it
+                vx = __ddiv_rn(__dmul_rn((double)D.kd, 255.0), J.Md);
+                vy = __ddiv_rn(__dmul_rn((double)source_sample(J.src, J.wide, J.hwc ? (size_t)s * 3 + c : (size_t)pidx), 255.0), J.Md);
+                if (r < T && q < T && CCD_OFF_GRID(D)) bad = min(bad, (unsigned long long)pidx);
+            } else {
+                const double2 v = J.lvl[c][S][s];
+                vx = v.x;
+                vy = v.y;
+            }
+        }
+        sx[i] = vx;
+        sy[i] = vy;
+    }
+    if constexpr (S == 0) report_bad(bad, J.bad, tid);
+    __syncthreads();
+
+    if constexpr (S + 1 < CCD_VIF_SCALES) {  // the next scale: N_{S+1} taps "valid" each way, the even rows and columns
+        constexpr int NN = ccd_vif_taps(S + 1);
+        const int r = tid / (T / 2), q = tid % (T / 2), Y = (y0 >> 1) + r, X = (x0 >> 1) + q;
+        const int hn = (h - NN + 2) >> 1, wn = (w - NN + 2) >> 1;
+        if (Y < hn && X < wn) {
+            const double *px = sx + 2 * r * In + 2 * q, *py = sy + 2 * r * In + 2 * q;
+            double ox = 0.0, oy = 0.0;
+#pragma unroll
+            for (int u = 0; u < NN; u++) {  // rows first, then the column: the order of the separable restatement
+                double hx = 0.0, hy = 0.0;
+#pragma unroll
+                for (int v = 0; v < NN; v++) {
+                    hx = fma(a.gn[v], px[u * In + v], hx);
+                    hy = fma(a.gn[v], py[u * In + v], hy);
+                }
+                ox = fma(a.gn[u], hx, ox);
+                oy = fma(a.gn[u], hy, oy);
+            }
+            J.lvl[c][S + 1][(size_t)Y * wn + X] = make_double2(ox, oy);
+        }
+    }
+
+    moments_h<N, In>(sx, sy, a.g, sh, tid);
+    __syncthreads();
+
+    double s_num = 0.0, s_den = 0.0;
+    {
+        const int q = tid & 31, r0 = (tid >> 5) * K;
+        double m[5][K];
+        moments_v<N, In>(sh, a.g, q, r0, m);
+        const int x = x0 + q, wo = w - N + 1, ho = h - N + 1;
+#pragma unroll
+        for (int k = 0; k < K; k++) {
+            const int y = y0 + r0 + k;
+            if (x >= wo || y >= ho) continue;
+            // no contraction: identical images give sigma_ref^2 = sigma_dist^2 = sigma_12 exactly, as in the checker
+            const double mu1 = m[1][k], mu2 = m[0][k];  // reference (source), distorted (decoded)
+            double s1 = fmax(__dsub_rn(m[3][k], __dmul_rn(mu1, mu1)), 0.0);
+            const double s2 = fmax(__dsub_rn(m[2][k], __dmul_rn(mu2, mu2)), 0.0);
+            const double s12 = __dsub_rn(m[4][k], __dmul_rn(mu1, mu2));
+            double g = __ddiv_rn(s12, __dadd_rn(s1, 1e-10));
+            double sv = __dsub_rn(s2, __dmul_rn(g, s12));
+            if (s1 < 1e-10) {
+                g = 0.0;
+                sv = s2;
+                s1 = 0.0;
+            }
+            if (s2 < 1e-10) {
+                g = 0.0;
+                sv = 0.0;
+            }
+            if (g < 0.0) {
+                sv = s2;
+                g = 0.0;
+            }
+            sv = fmax(sv, 1e-10);
+            s_num = __dadd_rn(s_num, log10(__dadd_rn(1.0, __ddiv_rn(__dmul_rn(__dmul_rn(g, g), s1), __dadd_rn(sv, 2.0)))));
+            s_den = __dadd_rn(s_den, log10(__dadd_rn(1.0, __ddiv_rn(s1, 2.0))));
+        }
+    }
+    tile_sums(s_num, s_den, sred, tid, [&](double pn, double pd) {
+        J.part[S][2 * blockIdx.x] = pn;
+        J.part[S][2 * blockIdx.x + 1] = pd;
+    });
+}
+
+template <int S>
+static int vif_launch_scale(const VifJobDev *d_jobs, int n_jobs, int tiles, const double *g, const double *gn,
+                            cudaStream_t st) {
+    cudaError_t e = cudaFuncSetAttribute(k_frame_vif<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVifSmem<S>);
+    if (e != cudaSuccess) return (int)e;
+    VifArgs a;
+    memset(&a, 0, sizeof(a));
+    memcpy(a.g, g, sizeof(double) * ccd_vif_taps(S));
+    if (gn) memcpy(a.gn, gn, sizeof(double) * ccd_vif_taps(S + 1));
+    k_frame_vif<S><<<dim3((unsigned)tiles, (unsigned)n_jobs, 1), 32 * kTileWarps, kVifSmem<S>, st>>>(d_jobs, a);
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
+
+int ccd_vif_launch(const VifJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_VIF_SCALES], const double g[CCD_VIF_SCALES][17],
+                   cudaStream_t st) {
+    // scale s + 1 reads the samples scale s wrote: stream order
+    if (int e = vif_launch_scale<0>(d_jobs, n_jobs, max_tiles[0], g[0], g[1], st)) return e;
+    if (int e = vif_launch_scale<1>(d_jobs, n_jobs, max_tiles[1], g[1], g[2], st)) return e;
+    if (int e = vif_launch_scale<2>(d_jobs, n_jobs, max_tiles[2], g[2], g[3], st)) return e;
+    return vif_launch_scale<3>(d_jobs, n_jobs, max_tiles[3], g[3], nullptr, st);
 }
 
 int ccd_finish(const float *d_in, int h, int w, int bitdepth, int data_type, float *a, float *b, float *c,

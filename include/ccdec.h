@@ -374,6 +374,28 @@ typedef struct CcdSsimJob {
 /* All jobs in five kernel launches, one per scale; synchronous.  Returns CCD_OK or the first failing job's status. */
 int ccd_frame_ssim(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, void *cuda_stream);
 
+/* Multi-scale pixel-domain VIF of finished frames against their source (Sheikh and Bovik 2006, the LIVE vifp_mscale;
+ * DESIGN §4.12).  Inputs as for CcdDistJob; the source is the reference image, the decoded frame the distorted one,
+ * both in 8-bit units v = k * 255 / M (f64), so the model's noise variance 2 means the same at every bit depth.  Each
+ * plane at its own resolution.  Scale s = 0..3 uses an N_s = 2^(4 - s) + 1 tap Gaussian window (sigma N_s / 5),
+ * "valid"; scale s >= 1 is scale s - 1 filtered with scale s's window and decimated to its even rows and columns.
+ * Every plane needs both sides >= 41 (a valid output at scale 3), else CCD_ERR_ARG before any launch.
+ * Outputs: num[c][s], den[c][s] = the sums over plane c at scale s of log10(1 + g^2 sigma_ref^2 / (sv^2 + 2)) and of
+ * log10(1 + sigma_ref^2 / 2) (f64 partials per tile added in tile order: the same on every run); the plane's VIF is
+ * sum_s num / sum_s den.  An off-grid decoded value is reported as by ccd_frame_distortion. */
+typedef struct CcdVifJob {
+    const float *d_planes[3];
+    const void *d_src;
+    int32_t h, w, chroma_shift, bitdepth, src_layout;
+    double num[3][4];
+    double den[3][4];
+    int64_t bad_index;
+    int32_t status;
+} CcdVifJob;
+
+/* All jobs in four kernel launches, one per scale; synchronous.  Returns CCD_OK or the first failing job's status. */
+int ccd_frame_vif(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, void *cuda_stream);
+
 /* Statistics of a P/B frame's prediction (training/test.py:169-199), with the fp32 operations of the reconstruction
  * (bitdepth >= 1: the source scale): pred (beta * p0 + (1 - beta) * p1 for B), alpha, beta.  d_src (optional): source
  * samples as for ccd_frame_distortion (src_layout 1 not for yuv420); orig = ks / M, 4:2:0 chroma read at >> 1,

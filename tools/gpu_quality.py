@@ -1,14 +1,14 @@
-"""Development tool: time the quality kernels (k_frame_dist, k_frame_ssim, k_inter_stats) with CUDA events, median of
+"""Development tool: time the quality kernels (k_frame_dist, k_frame_ssim, k_frame_vif, k_inter_stats) with CUDA events, median of
 --steps calls.
 
 Workloads:
-  * k_frame_dist and k_frame_ssim on the 32 decoded frames of bench.py's gop32_1080p_yuv420 stream (8-bit planar sources);
-  * k_frame_dist and k_frame_ssim on 1176 Kodak-size (768x512) rgb frames in one call (8-bit HWC sources);
+  * k_frame_dist, k_frame_ssim and k_frame_vif on the 32 decoded frames of bench.py's gop32_1080p_yuv420 stream (8-bit planar sources);
+  * k_frame_dist, k_frame_ssim and k_frame_vif on 1176 Kodak-size (768x512) rgb frames in one call (8-bit HWC sources);
   * k_inter_stats on one 1080p B frame of that stream, with its source.
 Reports, per workload, the whole call (CUDA events around the C-ABI call: staging, kernel, result copy), the kernel
-alone (torch.profiler; for MS-SSIM the sum of its five launches), the bytes the kernel must move and that over kernel
+alone (torch.profiler; for MS-SSIM and VIF the sum of the five or four launches), the bytes the kernel must move and that over kernel
 time against the H100 SXM's 3.35 TB/s, with the card's name, power limit and max SM clock read in the same run.  For
-MS-SSIM also the f64 FLOPs the algorithm needs over kernel time against the card's FP64 rate at its max SM clock
+MS-SSIM and VIF also the f64 FLOPs the algorithm needs over kernel time against the card's FP64 rate at its max SM clock
 (64 FP64 FMA per SM per cycle on an H100).
 
     python tools/gpu_quality.py [--steps 20]
@@ -55,6 +55,29 @@ def ssim_work(shapes):
     return n_bytes, flops
 
 
+def vif_work(shapes):
+    """(bytes, f64 FLOPs) the VIF of planes of the given (h, w) shapes needs.  Bytes: scale 0 reads 4 (fp32 decoded) + 1
+    (8-bit source) bytes per sample, scales 1..3 read 16 bytes per sample (the two f64 values), and every scale but the
+    last writes 16 bytes per sample of the next.  FLOPs: per scale of N taps, 3 products per sample, 5 moments x N taps
+    of FMA (2 FLOPs) per horizontal output (h x (w - N + 1)) and per vertical output ((h - N + 1) x (w - N + 1)), 40
+    for the per-pixel epilogue (a division or a log10 counted as one), and (N' + 1) N' FMA per next-scale sample and
+    image (N' taps)."""
+    taps = [2 ** (4 - s) + 1 for s in range(4)]
+    n_bytes = flops = 0
+    for h, w in shapes:
+        for s, n in enumerate(taps):
+            if s > 0:
+                h, w = (h - n + 2) // 2, (w - n + 2) // 2
+            n_bytes += h * w * (5 if s == 0 else 16)
+            flops += 3 * h * w + 10 * n * h * (w - n + 1) + (10 * n + 40) * (h - n + 1) * (w - n + 1)
+            if s < 3:
+                nn = taps[s + 1]
+                hn, wn = (h - nn + 2) // 2, (w - nn + 2) // 2
+                n_bytes += 16 * hn * wn
+                flops += 2 * 2 * (nn + 1) * nn * hn * wn
+    return n_bytes, flops
+
+
 def fp64_flops_per_s(card_csv):
     """The card's FP64 FMA rate at its max SM clock (nvidia-smi's clocks.max.sm), 2 FLOPs per FMA."""
     mhz = float(card_csv.split(",")[-1].strip().split()[0])
@@ -81,7 +104,7 @@ def measure(fn, kernel, steps, n_bytes, flops=None, fp64=None):
     for ev in prof.events():
         if kernel in ev.name:
             kern.append(ev.device_time_total / 1e3 if hasattr(ev, "device_time_total") else ev.cuda_time_total / 1e3)
-    per_call = len(kern) // steps if kern else 1  # MS-SSIM: five launches per call, summed in launch order
+    per_call = len(kern) // steps if kern else 1  # MS-SSIM, VIF: five or four launches per call, summed in launch order
     kern = [sum(kern[i:i + per_call]) for i in range(0, len(kern), per_call)]
     k_ms = float(np.median(kern)) if kern else float("nan")
     out = {"call_ms_median": float(np.median(call)), "kernel_ms_median": k_ms, "kernel_bytes": int(n_bytes),
@@ -119,6 +142,8 @@ def main():
     shapes = [(1080, 1920), (540, 960), (540, 960)] * len(frames)
     out["ssim_gop32_1080p_yuv420"] = measure(lambda: ctx.frame_ssim(frames, srcs, ["planar"] * len(frames)),
                                              "k_frame_ssim", args.steps, *ssim_work(shapes), fp64)
+    out["vif_gop32_1080p_yuv420"] = measure(lambda: ctx.frame_vif(frames, srcs, ["planar"] * len(frames)),
+                                            "k_frame_vif", args.steps, *vif_work(shapes), fp64)
 
     fh, cc, refs = kept["fh"], kept["cc"], kept["refs"]
     src = srcs[0]  # any 1080p 4:2:0 source: the timing does not depend on the values
@@ -143,6 +168,11 @@ def main():
                                      args.steps, 5 * 3 * h * w * n)
     out["ssim_kodak_x1176_rgb"] = measure(lambda: ctx.frame_ssim(kframes, ksrcs, ["hwc"] * n), "k_frame_ssim",
                                           args.steps, *ssim_work([(h, w)] * 3 * n), fp64)
+    out["vif_kodak_x1176_rgb"] = measure(lambda: ctx.frame_vif(kframes, ksrcs, ["hwc"] * n), "k_frame_vif",
+                                         args.steps, *vif_work([(h, w)] * 3 * n), fp64)
+    for k in ("vif_gop32_1080p_yuv420", "vif_kodak_x1176_rgb"):  # which roofline is nearer
+        v = out[k]
+        v["bound"] = "fp64" if v["share_of_fp64_rate"] > v["share_of_3.35TB_per_s"] else "hbm"
     print(json.dumps(out))
 
 

@@ -1,7 +1,8 @@
 """Quality analysis of a Cool-chic bitstream against its source: PSNR per plane and per frame, rate, and the
 prediction statistics of P / B frames, with the reference encoder's column names.
 
-    python cc_eval.py -i <bitstream.cool> --original <src.yuv|png|ppm> [--frame_offset N] [--ms_ssim] [--vif] [--maps out.npz]
+    python cc_eval.py -i <bitstream.cool> --original <src.yuv|png|ppm> [--frame_offset N] [--ms_ssim] [--vif] [--psnr_hvs]
+                      [--maps out.npz]
                       [--grids] [--motion] [--device N]
 
 Display frame i is compared with source frame frame_offset + i.  ``--maps`` writes, per frame, the error map
@@ -9,7 +10,9 @@ Display frame i is compared with source frame frame_offset + i.  ``--maps`` writ
 frames the alpha, beta and prediction maps.  ``--ms_ssim`` appends MS-SSIM columns (whole frame, in dB, per plane;
 ``n/a`` for a frame with a plane smaller than 176 x 176) and a mean line, and with ``--maps`` the scale-0 SSIM map of
 every plane.  ``--vif`` appends VIF columns (whole frame and per plane; ``n/a`` for a frame with a plane smaller than
-41 x 41 or a flat source plane) and a mean line.  ``--grids`` appends, per frame and per Cool-chic, a table of its latent grids: size, model bits and bpp,
+41 x 41 or a flat source plane) and a mean line.  ``--psnr_hvs`` appends PSNR-HVS and PSNR-HVS-M columns (whole
+frame, and PSNR-HVS-M per plane; ``n/a`` for a frame with a plane smaller than 8 x 8) and a mean line, and with
+``--maps`` each plane's block map of S_hvs_m / 64 / 255^2.  ``--grids`` appends, per frame and per Cool-chic, a table of its latent grids: size, model bits and bpp,
 the frame PSNR with the grid alone read as zeros and its change from the decoded frame's, and for the residue the PSNR
 with only the synthesis grids from the coarsest down to that one kept (DESIGN §4.7).  The grid analysis decodes the
 bitstream a second time, after the quality table.
@@ -32,6 +35,7 @@ COLUMNS = ["frame_idx", "frame_type", "psnr_db", "psnr_y_db", "psnr_u_db", "psnr
            "beta_mean", "pred_psnr_db", "dummy_pred_psnr_db"]
 MS_SSIM_COLUMNS = ["ms_ssim", "ms_ssim_db", "ms_ssim_y", "ms_ssim_u", "ms_ssim_v"]
 VIF_COLUMNS = ["vif", "vif_y", "vif_u", "vif_v"]
+HVS_COLUMNS = ["psnr_hvs_db", "psnr_hvs_m_db", "psnr_hvs_m_y_db", "psnr_hvs_m_u_db", "psnr_hvs_m_v_db"]
 MOTION_COLUMNS = ["variant", "psnr_db", "psnr_y_db", "psnr_u_db", "psnr_v_db", "delta_db"]
 GRID_COLUMNS = ["grid", "size", "hyper", "bits", "bpp", "drop_psnr_db", "drop_delta_db", "coarse_psnr_db"]
 
@@ -48,6 +52,7 @@ if __name__ == "__main__":
     parser.add_argument("--maps", type=str, default=None, help="Write the error / alpha / beta / prediction maps here (.npz).")
     parser.add_argument("--ms_ssim", action="store_true", help="Also report MS-SSIM.")
     parser.add_argument("--vif", action="store_true", help="Also report VIF (visual information fidelity).")
+    parser.add_argument("--psnr_hvs", action="store_true", help="Also report PSNR-HVS and PSNR-HVS-M.")
     parser.add_argument("--grids", action="store_true", help="Also report what each latent grid costs and buys.")
     parser.add_argument("--motion", action="store_true", help="Also report what the motion, each reference and the "
                         "residue of every P / B frame buy.")
@@ -57,8 +62,9 @@ if __name__ == "__main__":
     with open(args.input, "rb") as f_in:
         frames = video_quality(f_in.read(), args.original, frame_offset=args.frame_offset, device=args.device,
                                want_maps=args.maps is not None, ms_ssim=args.ms_ssim, motion=args.motion,
-                               vif=args.vif)
-    columns = COLUMNS + (MS_SSIM_COLUMNS if args.ms_ssim else []) + (VIF_COLUMNS if args.vif else [])
+                               vif=args.vif, psnr_hvs=args.psnr_hvs)
+    columns = (COLUMNS + (MS_SSIM_COLUMNS if args.ms_ssim else []) + (VIF_COLUMNS if args.vif else [])
+               + (HVS_COLUMNS if args.psnr_hvs else []))
     print(" ".join(f"{c:<18}" for c in columns))
     for key, q in frames.items():
         vals = [key, q.frame_type] + [_fmt(getattr(q, c)) for c in columns[2:]]
@@ -73,6 +79,11 @@ if __name__ == "__main__":
     if args.vif:
         have = [q.vif for q in frames.values() if q.vif is not None]
         print(f"mean vif {_fmt(sum(have) / len(have) if have else None)}  ({len(have)} of {len(frames)} frames)")
+    if args.psnr_hvs:
+        have = [q for q in frames.values() if q.hvs_planes is not None]
+        mean = {c: _fmt(sum(getattr(q, c) for q in have) / len(have) if have else None) for c in HVS_COLUMNS[:2]}
+        print(f"mean psnr_hvs_db {mean['psnr_hvs_db']}  psnr_hvs_m_db {mean['psnr_hvs_m_db']}  ({len(have)} of "
+              f"{len(frames)} frames)")
     if args.maps:
         maps = {}
         for key, q in frames.items():
@@ -83,6 +94,8 @@ if __name__ == "__main__":
                     maps[f"frame{key}_{name}"] = t.cpu().numpy()
             for plane, t in zip("yuv", q.ssim_maps or []):
                 maps[f"frame{key}_ssim_{plane}"] = t.cpu().numpy()
+            for plane, t in zip("yuv", q.hvs_maps or []):
+                maps[f"frame{key}_hvs_{plane}"] = t.cpu().numpy()
             for r, ref in enumerate(q.motion.refs if q.motion is not None else []):
                 maps[f"frame{key}_flow{r}"] = ref.flow_map.cpu().numpy()
         np.savez_compressed(args.maps, **maps)

@@ -28,7 +28,7 @@ EXPORTS = [
     "ccd_version", "ccd_sizeof_desc", "ccd_last_error", "ccd_create", "ccd_destroy", "ccd_nn_count",
     "ccd_latent_count", "ccd_decode_nn", "ccd_decode_many", "ccd_decode_coolchic", "ccd_decode_latents",
     "ccd_encode_latents", "ccd_synthesize_many", "ccd_finish_frame", "ccd_reconstruct_frame", "ccd_pack_frame", "ccd_pack_samples",
-    "ccd_latent_rate", "ccd_latent_rate_edited", "ccd_rate_sweep", "ccd_rate_candidates", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_frame_vif", "ccd_inter_stats", "ccd_inter_analysis",
+    "ccd_latent_rate", "ccd_latent_rate_edited", "ccd_rate_sweep", "ccd_rate_candidates", "ccd_frame_distortion", "ccd_frame_ssim", "ccd_frame_vif", "ccd_frame_hvs", "ccd_inter_stats", "ccd_inter_analysis",
     "ccd_debug_laplace_domain", "ccd_debug_last_status", "ccd_debug_launch_count", "ccd_debug_set_producer_mask", "ccd_last_timing",
     "ccd_debug_entropy_plan", "ccd_debug_cdf_table", "ccd_debug_detmath", "ccd_debug_sinc_coeffs", "ccd_debug_cr_noise",
 ]
@@ -178,6 +178,23 @@ class CcdVifJob(ctypes.Structure):
     ]
 
 
+class CcdHvsJob(ctypes.Structure):
+    _fields_ = [
+        ("d_planes", ctypes.c_void_p * 3),
+        ("d_src", ctypes.c_void_p),
+        ("h", ctypes.c_int32),
+        ("w", ctypes.c_int32),
+        ("chroma_shift", ctypes.c_int32),
+        ("bitdepth", ctypes.c_int32),
+        ("src_layout", ctypes.c_int32),
+        ("d_map", ctypes.c_void_p * 3),
+        ("s_hvs_m", ctypes.c_double * 3),
+        ("s_hvs", ctypes.c_double * 3),
+        ("bad_index", ctypes.c_int64),
+        ("status", ctypes.c_int32),
+    ]
+
+
 class CcdInterFrame(ctypes.Structure):
     _fields_ = [
         ("d_residue", ctypes.c_void_p),
@@ -297,6 +314,8 @@ def load_library():
         L.ccd_frame_ssim.argtypes = [vp, ctypes.POINTER(CcdSsimJob), ci, vp]
         L.ccd_frame_vif.restype = ci
         L.ccd_frame_vif.argtypes = [vp, ctypes.POINTER(CcdVifJob), ci, vp]
+        L.ccd_frame_hvs.restype = ci
+        L.ccd_frame_hvs.argtypes = [vp, ctypes.POINTER(CcdHvsJob), ci, vp]
         L.ccd_inter_stats.restype = ci
         L.ccd_inter_stats.argtypes = [vp, ctypes.POINTER(CcdInterFrame), ctypes.POINTER(CcdInterStats), vp]
         L.ccd_inter_analysis.restype = ci
@@ -773,7 +792,7 @@ class Context:
 
     def _frame_jobs(self, job_type, frames, sources, layouts):
         """The job array of a call that compares finished frames with their source samples (frame_distortion,
-        frame_ssim, frame_vif), the tensors it points into, and each frame's planes."""
+        frame_ssim, frame_vif, frame_hvs), the tensors it points into, and each frame's planes."""
         n = len(frames)
         jobs = (job_type * n)()
         keep, planes = [], []
@@ -848,6 +867,29 @@ class Context:
         _check(self._lib.ccd_frame_vif(self._h, jobs, n, self._stream()), jobs)
         return [{"num": [list(jobs[i].num[c]) for c in range(3)], "den": [list(jobs[i].den[c]) for c in range(3)]}
                 for i in range(n)]
+
+    def frame_hvs(self, frames, sources: Sequence[torch.Tensor], layouts: Sequence[str],
+                  want_maps: bool = False) -> List[dict]:
+        """PSNR-HVS-M sums of finished frames against their source samples (``ccd_frame_hvs``), one launch for all.
+        Arguments as for frame_distortion; every plane needs both sides >= 8.  Per frame a dict with ``s_hvs_m`` and
+        ``s_hvs`` (per plane, the sums over its 8 x 8 blocks of the masked and unmasked CSF-weighted squared DCT
+        errors, f64, the same on every run), ``n_coeffs`` (per plane, 64 per block) and on request ``maps``: per plane
+        each block's S_hvs_m / 64 / 255^2 ([h_c >> 3, w_c >> 3] float32 CUDA)."""
+        n = len(frames)
+        jobs, keep, planes = self._frame_jobs(CcdHvsJob, frames, sources, layouts)
+        res = []
+        for i in range(n):
+            r = {"n_coeffs": [64 * (t.shape[-2] >> 3) * (t.shape[-1] >> 3) for t in planes[i]]}
+            if want_maps:
+                r["maps"] = [torch.empty((t.shape[-2] >> 3, t.shape[-1] >> 3), dtype=torch.float32,
+                                         device=self.torch_device) for t in planes[i]]
+                jobs[i].d_map[:] = [m.data_ptr() for m in r["maps"]]
+            res.append(r)
+        _check(self._lib.ccd_frame_hvs(self._h, jobs, n, self._stream()), jobs)
+        for i in range(n):
+            res[i]["s_hvs_m"] = list(jobs[i].s_hvs_m)
+            res[i]["s_hvs"] = list(jobs[i].s_hvs)
+        return res
 
     def inter_stats(self, residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow, warp_filter_size,
                     source: Optional[torch.Tensor] = None, layout: str = "planar", want_maps: bool = False) -> dict:

@@ -23,6 +23,11 @@ On request, VIF (Sheikh and Bovik 2006, the multi-scale pixel-domain vifp_mscale
 integers in 8-bit units: one ``ccd_frame_vif`` call for every frame whose planes all have both sides of at least 41
 samples (a valid output at the fourth scale), per plane sum_s num_s / sum_s den_s, and per frame the pixel-weighted
 mean over the planes.  Smaller frames, and frames with a flat source plane (no VIF), get None.
+
+On request, PSNR-HVS-M and PSNR-HVS (Ponomarenko et al. 2007; DESIGN §4.13) from the same integers in 8-bit units:
+one ``ccd_frame_hvs`` call for every frame whose planes all have both sides of at least 8 samples (one 8 x 8 block),
+per plane the masked and unmasked sums of CSF-weighted squared DCT errors over its blocks, and per frame the
+coefficient-weighted mean over the planes.  Smaller frames get None.
 """
 import math
 from dataclasses import dataclass, field
@@ -77,6 +82,21 @@ def vif_applies(img_size, frame_data_type: str) -> bool:
     return min(img_size) >> cs >= VIF_MIN_SIDE
 
 
+HVS_MIN_SIDE = 8  # one 8 x 8 block
+
+
+def hvs_from_sums(sums: List[float], n_coeffs: List[int]) -> float:
+    """PSNR-HVS(-M) in dB of one or more planes from their sums of weighted squared DCT errors and their coefficient
+    counts: dist_to_db(sum S / sum N / 255^2), the rule psnr_db applies to the pixel-weighted MSE."""
+    return dist_to_db(sum(sums) / sum(n_coeffs) / 255.0**2)
+
+
+def hvs_applies(img_size, frame_data_type: str) -> bool:
+    """Whether every plane of an (h, w) frame has both sides >= 8 (4:2:0 chroma: (h / 2, w / 2))."""
+    cs = 1 if frame_data_type == "yuv420" else 0
+    return min(img_size) >> cs >= HVS_MIN_SIDE
+
+
 def ms_ssim_applies(img_size, frame_data_type: str) -> bool:
     """Whether every plane of an (h, w) frame has both sides >= 176 (4:2:0 chroma: (h / 2, w / 2))."""
     cs = 1 if frame_data_type == "yuv420" else 0
@@ -106,6 +126,8 @@ class FrameQuality:
     ms_ssim_planes: Optional[List[float]] = None        # per plane; None: not asked for, or a plane below 176
     ssim_maps: Optional[List[torch.Tensor]] = None      # per plane, [h_c - 10, w_c - 10] scale-0 SSIM map
     vif_planes: Optional[List[Optional[float]]] = None  # per plane (None: flat source); None: not asked for, or below 41
+    hvs_planes: Optional[List[tuple]] = None            # per plane (S_hvs_m, S_hvs, N_c); None: not asked for, or below 8
+    hvs_maps: Optional[List[torch.Tensor]] = None       # per plane, [h_c >> 3, w_c >> 3]: S_hvs_m / 64 / 255^2 per block
     motion: Optional["MotionAnalysis"] = None  # noqa: F821  (bitstream/motion.py; P / B frames with motion=True)
     plane_mse: List[float] = field(init=False)
 
@@ -157,6 +179,17 @@ class FrameQuality:
     vif_y = property(lambda self: None if self.vif_planes is None else self.vif_planes[0])
     vif_u = property(lambda self: None if self.vif_planes is None else self.vif_planes[1])
     vif_v = property(lambda self: None if self.vif_planes is None else self.vif_planes[2])
+
+    def _hvs_db(self, k: int, planes) -> Optional[float]:
+        if self.hvs_planes is None:
+            return None
+        return hvs_from_sums([self.hvs_planes[c][k] for c in planes], [self.hvs_planes[c][2] for c in planes])
+
+    psnr_hvs_m_db = property(lambda self: self._hvs_db(0, (0, 1, 2)))
+    psnr_hvs_db = property(lambda self: self._hvs_db(1, (0, 1, 2)))
+    psnr_hvs_m_y_db = property(lambda self: self._hvs_db(0, (0,)))
+    psnr_hvs_m_u_db = property(lambda self: self._hvs_db(0, (1,)))
+    psnr_hvs_m_v_db = property(lambda self: self._hvs_db(0, (2,)))
 
 
 def _frame_layout(buf, max_decoding_order: int):
@@ -215,13 +248,15 @@ def _upload_sources(ctx, by_display):
 @torch.no_grad()
 def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int = 0, max_decoding_order: int = -1,
                   device: int = 0, want_maps: bool = False, ms_ssim: bool = False,
-                  motion: bool = False, vif: bool = False) -> Dict[str, FrameQuality]:
+                  motion: bool = False, vif: bool = False, psnr_hvs: bool = False) -> Dict[str, FrameQuality]:
     """Quality of every frame of an image / video bitstream against its source file (.yuv / .png / .ppm):
     ``{str(display_idx): FrameQuality}`` in display order.  ``ms_ssim`` adds MS-SSIM for every frame whose planes
     all have both sides >= 176 (``ms_ssim_planes`` stays None for the others), with the SSIM maps if ``want_maps``.
     ``motion`` fills ``FrameQuality.motion`` of every P / B frame (a MotionAnalysis, with the flow maps if
     ``want_maps``); I frames keep None.  ``vif`` adds VIF for every frame whose planes all have both sides >= 41
-    (``vif_planes`` stays None for the others).  A source whose format, bitdepth or size differs from the
+    (``vif_planes`` stays None for the others).  ``psnr_hvs`` adds PSNR-HVS-M and PSNR-HVS for every frame whose
+    planes all have both sides >= 8 (``hvs_planes`` stays None for the others), with the block maps if ``want_maps``.
+    A source whose format, bitdepth or size differs from the
     decoded frames, or that has too few frames, raises ValueError before anything runs on the device."""
     frames = _frame_layout(memoryview(bytes(bitstream_bytes)), max_decoding_order)
     by_display = _read_sources(frames, original_path, frame_offset)
@@ -274,6 +309,13 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
             res = ctx.frame_vif([decoded[str(d)] for d in big], [sources[d] for d in big],
                                 [by_display[d][3].layout for d in big])
             vifs = dict(zip(big, res))
+    hvs = {}
+    if psnr_hvs:
+        big = [d for d in order if hvs_applies(by_display[d][3].img_size, by_display[d][3].frame_data_type)]
+        if big:
+            res = ctx.frame_hvs([decoded[str(d)] for d in big], [sources[d] for d in big],
+                                [by_display[d][3].layout for d in big], want_maps=want_maps)
+            hvs = dict(zip(big, res))
     out = {}
     for d, r in zip(order, dist):
         _, fh, n_bytes, s = by_display[d]
@@ -296,5 +338,8 @@ def video_quality(bitstream_bytes: bytes, original_path: str, frame_offset: int 
             q.ssim_maps = ssim[d].get("maps")
         if d in vifs:
             q.vif_planes = [vif_from_scales(n_, d_) for n_, d_ in zip(vifs[d]["num"], vifs[d]["den"])]
+        if d in hvs:
+            q.hvs_planes = list(zip(hvs[d]["s_hvs_m"], hvs[d]["s_hvs"], hvs[d]["n_coeffs"]))
+            q.hvs_maps = hvs[d].get("maps")
         out[str(d)] = q
     return out

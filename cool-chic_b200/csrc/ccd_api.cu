@@ -2066,7 +2066,8 @@ int ccd_rate_sweep(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, void *cuda_st
     return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return rate_sweep_body(ctx, jobs, n_jobs, st); });
 }
 
-// The checks of a job that compares a finished frame with its source samples (CcdDistJob, CcdSsimJob, CcdVifJob)
+// The checks of a job that compares a finished frame with its source samples (CcdDistJob, CcdSsimJob, CcdVifJob,
+// CcdHvsJob)
 extern "C++" template <class Job>
 int check_frame_job(Job &J, int i) {
     J.bad_index = -1;
@@ -2317,6 +2318,81 @@ static int frame_vif_body(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, cudaStre
 
 int ccd_frame_vif(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, void *cuda_stream) {
     return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return frame_vif_body(ctx, jobs, n_jobs, st); });
+}
+
+static int frame_hvs_body(CcdContext *ctx, CcdHvsJob *jobs, int n_jobs, cudaStream_t st) {
+    const size_t n = (size_t)n_jobs;
+    auto side = [&](int i, int c, bool width) {  // plane c of job i
+        const CcdHvsJob &J = jobs[i];
+        return (width ? J.w : J.h) >> (c ? J.chroma_shift : 0);
+    };
+    auto tiles = [&](int i, int c) { return ccd_hvs_tiles(side(i, c, false), side(i, c, true)); };
+    // the job's partials start at part_at[i] (pairs, planes in order)
+    std::vector<size_t> part_at(n);
+    size_t n_part = 0;
+    int max_tiles = 0;
+    for (int i = 0; i < n_jobs; i++) {
+        if (int rc = check_frame_job(jobs[i], i)) return rc;
+        for (int c = 0; c < 3; c++)  // one 8 x 8 block at least
+            if (std::min(side(i, c, false), side(i, c, true)) < 8)
+                return jobs[i].status = fail(CCD_ERR_ARG, "job %d: plane %d is %dx%d, PSNR-HVS-M needs both sides >= 8", i, c,
+                                             side(i, c, true), side(i, c, false));
+        part_at[(size_t)i] = n_part;
+        const int t = tiles(i, 0) + tiles(i, 1) + tiles(i, 2);
+        max_tiles = std::max(max_tiles, t);
+        n_part += (size_t)t;
+    }
+    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
+    // the job array, then the results: bad[n] ~0, then the partials, which are not uploaded
+    Arena A;
+    const size_t off_jobs = A.take(sizeof(HvsJobDev) * n), off_bad = A.take(8 * n, 8);
+    const size_t off_part = A.take(2 * sizeof(double) * n_part, 8);
+    if (int rc = stage(ctx, A)) return rc;
+    memset(A.h + off_bad, 0xff, 8 * n);
+    double *d_part = reinterpret_cast<double *>(A.dv + off_part);
+    for (int i = 0; i < n_jobs; i++) {
+        const CcdHvsJob &J = jobs[i];
+        HvsJobDev D;
+        memset(&D, 0, sizeof(D));
+        for (int c = 0; c < 3; c++) {
+            D.p[c] = J.d_planes[c];
+            D.map[c] = J.d_map[c];
+        }
+        D.part = d_part + 2 * part_at[(size_t)i];
+        D.src = J.d_src;
+        D.h = J.h;
+        D.w = J.w;
+        D.cs = J.chroma_shift;
+        D.hwc = J.src_layout;
+        D.wide = J.bitdepth > 8;
+        D.Md = (double)((1 << J.bitdepth) - 1);
+        D.M = (float)D.Md;
+        D.s2 = (255.0 / D.Md) * (255.0 / D.Md);
+        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
+        memcpy(A.h + off_jobs + sizeof(HvsJobDev) * (size_t)i, &D, sizeof(D));
+    }
+    double dct[8][8];  // the orthonormal DCT-II: dct[k][n] = a_k cos(pi (2n + 1) k / 16), a_0 = sqrt(1/8), a_k = 1/2
+    for (int k = 0; k < 8; k++)
+        for (int m = 0; m < 8; m++) dct[k][m] = (k ? 0.5 : std::sqrt(0.125)) * std::cos(std::acos(-1.0) * (2 * m + 1) * k / 16.0);
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
+    int e = ccd_hvs_launch(reinterpret_cast<const HvsJobDev *>(A.dv + off_jobs), n_jobs, max_tiles, dct, st);
+    if (e != 0) return fail(CCD_ERR_CUDA, "PSNR-HVS-M launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    if (int rc = download(A, off_bad, st, "PSNR-HVS-M")) return rc;
+    const double *part = reinterpret_cast<const double *>(A.h + off_part);
+    for (int i = 0; i < n_jobs; i++) {
+        const double *p = part + 2 * part_at[(size_t)i];  // the planes' tiles in order
+        for (int c = 0; c < 3; c++) {
+            const size_t t = (size_t)tiles(i, c);
+            jobs[i].s_hvs_m[c] = ordered_sum(p, t, 2);
+            jobs[i].s_hvs[c] = ordered_sum(p + 1, t, 2);
+            p += 2 * t;
+        }
+    }
+    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) { return off_grid_error(jobs[i], i); });
+}
+
+int ccd_frame_hvs(CcdContext *ctx, CcdHvsJob *jobs, int n_jobs, void *cuda_stream) {
+    return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return frame_hvs_body(ctx, jobs, n_jobs, st); });
 }
 
 int ccd_finish_frame(CcdContext *ctx, const float *d_in, int h, int w, int bitdepth, int data_type, float *d_out_a,

@@ -341,6 +341,30 @@ static __host__ __device__ __forceinline__ int ccd_vif_side(int n, int s) {
 int ccd_vif_launch(const VifJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_VIF_SCALES], const double g[CCD_VIF_SCALES][17],
                    cudaStream_t st);
 
+// PSNR-HVS-M (DESIGN §4.13): one k_frame_hvs launch for every plane of every job of a call, blockIdx.y = job,
+// blockIdx.x = tile over the job's planes (plane 0's tiles, then plane 1's, then plane 2's, each row-major).  A tile is
+// a strip of CCD_HVS_ROWS rows and CCD_HVS_COLS columns of its plane; the tiles cover every sample (each is read once,
+// for the off-grid check), and only the 8 x 8 blocks that lie wholly inside the plane are measured.
+#define CCD_HVS_ROWS 8
+#define CCD_HVS_COLS 256
+struct HvsJobDev {
+    const float *p[3];          // finished planes (FrameData layout)
+    const void *src;            // source samples as for DistJobDev
+    float *map[3];              // optional [h_c >> 3][w_c >> 3]: each block's S_hvs_m / 64 / 255^2
+    double *part;               // (sum S_hvs_m, sum S_hvs) of each of the job's tiles, in tile order
+    int32_t h, w, cs, hwc, wide;
+    float M;
+    double Md;                  // M in f64: a sample k is v = k * 255 / M
+    double s2;                  // (255 / M)^2: integer variances to 8-bit units
+    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
+};
+// tiles of one plane of h x w samples
+static __host__ __device__ __forceinline__ int ccd_hvs_tiles(int h, int w) {
+    return ((h + CCD_HVS_ROWS - 1) / CCD_HVS_ROWS) * ((w + CCD_HVS_COLS - 1) / CCD_HVS_COLS);
+}
+// one launch; max_tiles: the most tiles of one job; dct[k][n]: the orthonormal 8-point DCT-II basis
+int ccd_hvs_launch(const HvsJobDev *d_jobs, int n_jobs, int max_tiles, const double dct[8][8], cudaStream_t st);
+
 // P/B reconstruction (ccd_inter.cu); returns -1 for an unsupported filter size
 struct InterLaunch {
     const float *residue, *motion;  // [4|5][h][w], [2|4][h][w]

@@ -1958,6 +1958,202 @@ int ccd_vif_launch(const VifJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_
     return vif_launch_scale<3>(d_jobs, n_jobs, max_tiles[3], g[3], nullptr, st);
 }
 
+// ---- PSNR-HVS-M.  A = the source, B = the decoded image, both in 8-bit units v = k * 255 / M (f64).  Per tile: stage
+// the integers of a strip of CCD_HVS_ROWS x CCD_HVS_COLS samples of both images (32 blocks side by side); then one
+// thread per (block, row) forms the row's integer sums and its 8-point DCT, and after that one thread per (block,
+// column) the column's DCT, masking sum and error sums.  The 8 lanes of a block reduce by a butterfly, which leaves
+// the same bits in every lane, and the tile adds its blocks in a fixed order into one f64 partial per sum.
+namespace {
+constexpr int kHvsLd = CCD_HVS_COLS + 1;  // staged row stride: the 8 rows of a block fall in distinct banks
+static_assert(CCD_HVS_ROWS == 8 && CCD_HVS_COLS / 8 * 8 == 32 * kTileWarps, "one thread per (block, row), then per (block, column)");
+struct HvsArgs {
+    double dct[8][8];  // dct[k][n]: the orthonormal 8-point DCT-II basis, computed on the host
+};
+// Ponomarenko et al. (2007), rows k = 0..7, columns l = 0..7: CSF = round(25.735088 / Q, 6), Mask = round((10 / Q)^2,
+// 6), Q the JPEG luminance quantisation table.  Read through the read-only path: the 8 columns of a warp's lanes share
+// one cache line.
+__device__ const double kHvsCsf[64] = {
+    1.608443, 2.339554, 2.573509, 1.608443, 1.072295, 0.643377, 0.504610, 0.421887,
+    2.144591, 2.144591, 1.838221, 1.354478, 0.989811, 0.443708, 0.428918, 0.467911,
+    1.838221, 1.979622, 1.608443, 1.072295, 0.643377, 0.451493, 0.372972, 0.459555,
+    1.838221, 1.513829, 1.169777, 0.887417, 0.504610, 0.295806, 0.321689, 0.415082,
+    1.429727, 1.169777, 0.695543, 0.459555, 0.378457, 0.236102, 0.249855, 0.334222,
+    1.072295, 0.735288, 0.467911, 0.402111, 0.317717, 0.247453, 0.227744, 0.279729,
+    0.525206, 0.402111, 0.329937, 0.295806, 0.249855, 0.212687, 0.214459, 0.254803,
+    0.357432, 0.279729, 0.270896, 0.262603, 0.229778, 0.257351, 0.249855, 0.259950};
+__device__ const double kHvsMask[64] = {
+    0.390625, 0.826446, 1.000000, 0.390625, 0.173611, 0.062500, 0.038447, 0.026874,
+    0.694444, 0.694444, 0.510204, 0.277008, 0.147929, 0.029727, 0.027778, 0.033058,
+    0.510204, 0.591716, 0.390625, 0.173611, 0.062500, 0.030779, 0.021004, 0.031888,
+    0.510204, 0.346021, 0.206612, 0.118906, 0.038447, 0.013212, 0.015625, 0.026015,
+    0.308642, 0.206612, 0.073046, 0.031888, 0.021626, 0.008417, 0.009426, 0.016866,
+    0.173611, 0.081633, 0.033058, 0.024414, 0.015242, 0.009246, 0.007831, 0.011815,
+    0.041649, 0.024414, 0.016437, 0.013212, 0.009426, 0.006830, 0.006944, 0.009803,
+    0.019290, 0.011815, 0.011080, 0.010412, 0.007972, 0.010000, 0.009426, 0.010203};
+}  // namespace
+
+// y[k] = sum_n dct[k][n] x[n]: 8 FMAs per output, n in order
+static __device__ __forceinline__ void hvs_dct8(const double (&x)[8], const double (&dct)[8][8], double (&y)[8]) {
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        double acc = 0.0;
+#pragma unroll
+        for (int n = 0; n < 8; n++) acc = fma(dct[k][n], x[n], acc);
+        y[k] = acc;
+    }
+}
+
+// vari(Z) = (n sum z^2 - (sum z)^2) / (n - 1) from the exact integer sums s, q of the block's k, in 8-bit units
+static __device__ __forceinline__ double hvs_vari(long long s, long long q, int n, double s2) {
+    return __dmul_rn(__ddiv_rn((double)(n * q - s * s), (double)(n - 1)), s2);
+}
+
+// The masking ratio pop of a block, from row e of its integers k in lane e of the block's 8 lanes: 0 for a flat block,
+// else the quadrants' vari (top-left, top-right, bottom-right, bottom-left, added in that order) over the block's.
+// Every lane of the 8 gets the same value.
+static __device__ __forceinline__ double hvs_pop(const int (&k)[8], int e, double s2) {
+    long long v[4] = {0, 0, 0, 0};  // sum k and sum k^2 of the row's left half, then of its right half
+#pragma unroll
+    for (int n = 0; n < 8; n++) {
+        v[(n >> 2) * 2] += k[n];
+        v[(n >> 2) * 2 + 1] += (long long)k[n] * k[n];
+    }
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1)  // rows 0..3, or rows 4..7
+#pragma unroll
+        for (int j = 0; j < 4; j++) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
+    long long u[4];  // the other four rows
+#pragma unroll
+    for (int j = 0; j < 4; j++) u[j] = __shfl_xor_sync(0xffffffffu, v[j], 4);
+    const long long s = v[0] + v[2] + u[0] + u[2], q = v[1] + v[3] + u[1] + u[3];
+    if (64 * q - s * s == 0) return 0.0;
+    const bool top = e < 4;
+    const double q00 = hvs_vari(top ? v[0] : u[0], top ? v[1] : u[1], 16, s2);
+    const double q01 = hvs_vari(top ? v[2] : u[2], top ? v[3] : u[3], 16, s2);
+    const double q10 = hvs_vari(top ? u[0] : v[0], top ? u[1] : v[1], 16, s2);
+    const double q11 = hvs_vari(top ? u[2] : v[2], top ? u[3] : v[3], 16, s2);
+    return __ddiv_rn(__dadd_rn(__dadd_rn(__dadd_rn(q00, q01), q11), q10), hvs_vari(s, q, 64, s2));
+}
+
+static __device__ __forceinline__ double hvs_group_sum(double x) {  // the 8 lanes of a block, xor butterfly
+#pragma unroll
+    for (int o = 1; o < 8; o <<= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    return x;
+}
+
+__global__ void __launch_bounds__(32 * kTileWarps) k_frame_hvs(const HvsJobDev *__restrict__ jobs, const HvsArgs a) {
+    constexpr int R = CCD_HVS_ROWS, W = CCD_HVS_COLS;
+    __shared__ double hvs_sm[2 * R * kHvsLd];  // [2][R][kHvsLd]: the staged integers (int), then the row pass (f64)
+    __shared__ double sred[2 * kTileWarps];
+    int *si = reinterpret_cast<int *>(hvs_sm);
+    const HvsJobDev &J = jobs[blockIdx.y];
+    const int tid = (int)threadIdx.x;
+    int c = 0, t = (int)blockIdx.x, h = 0, w = 0;
+    for (;; c++) {  // the plane and tile of this CTA
+        if (c == 3) return;
+        h = c ? J.h >> J.cs : J.h;
+        w = c ? J.w >> J.cs : J.w;
+        const int n = ccd_hvs_tiles(h, w);
+        if (t < n) break;
+        t -= n;
+    }
+    const int tw = (w + W - 1) / W, y0 = t / tw * R, x0 = t % tw * W;
+
+    // every sample of the strip, for the off-grid check; rows [0, R) of A (source), then of B (decoded)
+    unsigned long long bad = ~0ull;
+    const unsigned n0 = (unsigned)J.h * J.w, n1 = (unsigned)(J.h >> J.cs) * (unsigned)(J.w >> J.cs);
+    for (int i = tid; i < R * W; i += 32 * kTileWarps) {
+        const int r = i / W, q = i % W, y = y0 + r, x = x0 + q;
+        int ka = 0, kb = 0;
+        if (y < h && x < w) {
+            const unsigned s = (unsigned)y * (unsigned)w + (unsigned)x;
+            const DecodedSample D = read_decoded(J.p[c], s, J.M);
+            const unsigned pidx = c == 0 ? s : n0 + (unsigned)(c - 1) * n1 + s;  // as k_frame_dist reports it
+            kb = (int)D.kd;
+            ka = source_sample(J.src, J.wide, J.hwc ? (size_t)s * 3 + c : (size_t)pidx);
+            if (CCD_OFF_GRID(D)) bad = min(bad, (unsigned long long)pidx);
+        }
+        si[r * kHvsLd + q] = ka;
+        si[(R + r) * kHvsLd + q] = kb;
+    }
+    report_bad(bad, J.bad, tid);
+    __syncthreads();
+
+    const int b = tid >> 3, e = tid & 7;  // this thread's block of the strip, and its row, then its column
+    double xa[8], xb[8], ya[8], yb[8];
+    double pop_a, pop_b;
+    {
+        int ka[8], kb[8];
+#pragma unroll
+        for (int n = 0; n < 8; n++) {
+            ka[n] = si[e * kHvsLd + 8 * b + n];
+            kb[n] = si[(R + e) * kHvsLd + 8 * b + n];
+        }
+        __syncthreads();  // the row pass overwrites the staged integers
+        pop_a = hvs_pop(ka, e, J.s2);
+        pop_b = hvs_pop(kb, e, J.s2);
+#pragma unroll
+        for (int n = 0; n < 8; n++) {
+            xa[n] = __ddiv_rn(__dmul_rn((double)ka[n], 255.0), J.Md);
+            xb[n] = __ddiv_rn(__dmul_rn((double)kb[n], 255.0), J.Md);
+        }
+    }
+    hvs_dct8(xa, a.dct, ya);
+    hvs_dct8(xb, a.dct, yb);
+#pragma unroll
+    for (int l = 0; l < 8; l++) {
+        hvs_sm[e * kHvsLd + 8 * b + l] = ya[l];
+        hvs_sm[(R + e) * kHvsLd + 8 * b + l] = yb[l];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        xa[r] = hvs_sm[r * kHvsLd + 8 * b + e];
+        xb[r] = hvs_sm[(R + r) * kHvsLd + 8 * b + e];
+    }
+    hvs_dct8(xa, a.dct, ya);  // ya[k] = A_dct[k][e], yb[k] = B_dct[k][e]
+    hvs_dct8(xb, a.dct, yb);
+
+    double m_a = 0.0, m_b = 0.0;  // sum of A_dct^2 Mask over the block but (0, 0)
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        const double wm = k == 0 && e == 0 ? 0.0 : __ldg(kHvsMask + 8 * k + e);
+        m_a = fma(__dmul_rn(ya[k], ya[k]), wm, m_a);
+        m_b = fma(__dmul_rn(yb[k], yb[k]), wm, m_b);
+    }
+    m_a = hvs_group_sum(m_a);
+    m_b = hvs_group_sum(m_b);
+    const double T = fmax(__dmul_rn(__dsqrt_rn(__dmul_rn(m_a, pop_a)), 1.0 / 32), __dmul_rn(__dsqrt_rn(__dmul_rn(m_b, pop_b)), 1.0 / 32));
+    double s_hvs = 0.0, s_hvs_m = 0.0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        const double csf = __ldg(kHvsCsf + 8 * k + e);
+        const double u = fabs(__dsub_rn(ya[k], yb[k])), d = __dmul_rn(u, csf);
+        s_hvs = fma(d, d, s_hvs);
+        const double um = k == 0 && e == 0 ? u : fmax(__dsub_rn(u, __ddiv_rn(T, __ldg(kHvsMask + 8 * k + e))), 0.0);
+        const double dm = __dmul_rn(um, csf);
+        s_hvs_m = fma(dm, dm, s_hvs_m);
+    }
+    s_hvs = hvs_group_sum(s_hvs);
+    s_hvs_m = hvs_group_sum(s_hvs_m);
+    const bool own = e == 0 && y0 + 8 <= h && x0 + 8 * b + 8 <= w;  // lane 0 of a block wholly inside the plane
+    if (own && J.map[c]) J.map[c][(size_t)(y0 >> 3) * (w >> 3) + (x0 >> 3) + b] = __double2float_rn(__ddiv_rn(s_hvs_m, 64.0 * 255 * 255));
+    s_hvs_m = own ? s_hvs_m : 0.0;
+    s_hvs = own ? s_hvs : 0.0;
+    tile_sums(s_hvs_m, s_hvs, sred, tid, [&](double pm, double p) {
+        J.part[2 * blockIdx.x] = pm;
+        J.part[2 * blockIdx.x + 1] = p;
+    });
+}
+
+int ccd_hvs_launch(const HvsJobDev *d_jobs, int n_jobs, int max_tiles, const double dct[8][8], cudaStream_t st) {
+    HvsArgs a;
+    memcpy(a.dct, dct, sizeof(a.dct));
+    k_frame_hvs<<<dim3((unsigned)max_tiles, (unsigned)n_jobs, 1), 32 * kTileWarps, 0, st>>>(d_jobs, a);
+    g_ccd_launches++;
+    return (int)cudaGetLastError();
+}
+
 int ccd_finish(const float *d_in, int h, int w, int bitdepth, int data_type, float *a, float *b, float *c,
                cudaStream_t st) {
     const float M = (float)((1 << bitdepth) - 1);

@@ -396,6 +396,30 @@ typedef struct CcdVifJob {
 /* All jobs in four kernel launches, one per scale; synchronous.  Returns CCD_OK or the first failing job's status. */
 int ccd_frame_vif(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, void *cuda_stream);
 
+/* PSNR-HVS-M and PSNR-HVS of finished frames against their source (Ponomarenko et al. 2007; DESIGN §4.13).  Inputs as
+ * for CcdDistJob; both images in 8-bit units v = k * 255 / M (f64).  Each plane at its own resolution, cut into the
+ * non-overlapping 8 x 8 blocks that lie wholly inside it (the other samples are read only for the off-grid check);
+ * per block the orthonormal 2-D DCT-II of both images, the contrast masking of the larger of the two blocks' masks,
+ * and the CSF-weighted squared coefficient errors.  Every plane needs both sides >= 8, else CCD_ERR_ARG before any
+ * launch.
+ * d_map[c] (optional): float32 [h_c >> 3][w_c >> 3], each block's S_hvs_m / 64 / 255^2.
+ * Outputs: s_hvs_m[c], s_hvs[c] = the sums over plane c's blocks of the masked and unmasked weighted squared errors
+ * (f64 partials per tile added in tile order: the same on every run); with N_c = 64 blocks, the plane's PSNR-HVS-M is
+ * -10 log10(s_hvs_m / N_c / 255^2).  An off-grid decoded value is reported as by ccd_frame_distortion. */
+typedef struct CcdHvsJob {
+    const float *d_planes[3];
+    const void *d_src;
+    int32_t h, w, chroma_shift, bitdepth, src_layout;
+    float *d_map[3];
+    double s_hvs_m[3];
+    double s_hvs[3];
+    int64_t bad_index;
+    int32_t status;
+} CcdHvsJob;
+
+/* All jobs in ONE kernel launch; synchronous.  Returns CCD_OK or the first failing job's status. */
+int ccd_frame_hvs(CcdContext *ctx, CcdHvsJob *jobs, int n_jobs, void *cuda_stream);
+
 /* Statistics of a P/B frame's prediction (training/test.py:169-199), with the fp32 operations of the reconstruction
  * (bitdepth >= 1: the source scale): pred (beta * p0 + (1 - beta) * p1 for B), alpha, beta.  d_src (optional): source
  * samples as for ccd_frame_distortion (src_layout 1 not for yuv420); orig = ks / M, 4:2:0 chroma read at >> 1,

@@ -1,15 +1,18 @@
-"""Development tool: time the quality kernels (k_frame_dist, k_frame_ssim, k_frame_vif, k_inter_stats) with CUDA events, median of
---steps calls.
+"""Development tool: time the quality kernels (k_frame_dist, k_frame_ssim, k_frame_vif, k_frame_hvs, k_inter_stats) with CUDA
+events, median of --steps calls.
 
 Workloads:
-  * k_frame_dist, k_frame_ssim and k_frame_vif on the 32 decoded frames of bench.py's gop32_1080p_yuv420 stream (8-bit planar sources);
-  * k_frame_dist, k_frame_ssim and k_frame_vif on 1176 Kodak-size (768x512) rgb frames in one call (8-bit HWC sources);
+  * k_frame_dist, k_frame_ssim, k_frame_vif and k_frame_hvs on the 32 decoded frames of bench.py's gop32_1080p_yuv420
+    stream (8-bit planar sources);
+  * k_frame_dist, k_frame_ssim, k_frame_vif and k_frame_hvs on 1176 Kodak-size (768x512) rgb frames in one call (8-bit
+    HWC sources);
   * k_inter_stats on one 1080p B frame of that stream, with its source.
 Reports, per workload, the whole call (CUDA events around the C-ABI call: staging, kernel, result copy), the kernel
 alone (torch.profiler; for MS-SSIM and VIF the sum of the five or four launches), the bytes the kernel must move and that over kernel
 time against the H100 SXM's 3.35 TB/s, with the card's name, power limit and max SM clock read in the same run.  For
-MS-SSIM and VIF also the f64 FLOPs the algorithm needs over kernel time against the card's FP64 rate at its max SM clock
-(64 FP64 FMA per SM per cycle on an H100).
+MS-SSIM, VIF and PSNR-HVS-M also the f64 FLOPs the algorithm needs over kernel time against the card's FP64 rate at its
+max SM clock (64 FP64 FMA per SM per cycle on an H100), and for VIF and PSNR-HVS-M which of the two rooflines is
+nearer.
 
     python tools/gpu_quality.py [--steps 20]
 """
@@ -75,6 +78,19 @@ def vif_work(shapes):
                 hn, wn = (h - nn + 2) // 2, (w - nn + 2) // 2
                 n_bytes += 16 * hn * wn
                 flops += 2 * 2 * (nn + 1) * nn * hn * wn
+    return n_bytes, flops
+
+
+def hvs_work(shapes):
+    """(bytes, f64 FLOPs) the PSNR-HVS-M of planes of the given (h, w) shapes needs.  Bytes: 4 (fp32 decoded) + 1
+    (8-bit source) per sample, every sample read once.  FLOPs per 8 x 8 block wholly inside the plane: per image, the
+    8-bit units (a multiply and a division per sample), the 2-D DCT (1024 FMA) and the 63-term mask sum (a square and
+    an FMA per term); per coefficient 11 (difference, absolute value, two weighted squares, the mask's division,
+    subtraction and clamp, a division counted as one)."""
+    n_bytes = flops = 0
+    for h, w in shapes:
+        n_bytes += 5 * h * w
+        flops += (h // 8) * (w // 8) * (2 * (2 * 64 + 2 * 1024 + 3 * 63) + 11 * 64)
     return n_bytes, flops
 
 
@@ -144,6 +160,8 @@ def main():
                                              "k_frame_ssim", args.steps, *ssim_work(shapes), fp64)
     out["vif_gop32_1080p_yuv420"] = measure(lambda: ctx.frame_vif(frames, srcs, ["planar"] * len(frames)),
                                             "k_frame_vif", args.steps, *vif_work(shapes), fp64)
+    out["hvs_gop32_1080p_yuv420"] = measure(lambda: ctx.frame_hvs(frames, srcs, ["planar"] * len(frames)),
+                                            "k_frame_hvs", args.steps, *hvs_work(shapes), fp64)
 
     fh, cc, refs = kept["fh"], kept["cc"], kept["refs"]
     src = srcs[0]  # any 1080p 4:2:0 source: the timing does not depend on the values
@@ -170,7 +188,10 @@ def main():
                                           args.steps, *ssim_work([(h, w)] * 3 * n), fp64)
     out["vif_kodak_x1176_rgb"] = measure(lambda: ctx.frame_vif(kframes, ksrcs, ["hwc"] * n), "k_frame_vif",
                                          args.steps, *vif_work([(h, w)] * 3 * n), fp64)
-    for k in ("vif_gop32_1080p_yuv420", "vif_kodak_x1176_rgb"):  # which roofline is nearer
+    out["hvs_kodak_x1176_rgb"] = measure(lambda: ctx.frame_hvs(kframes, ksrcs, ["hwc"] * n), "k_frame_hvs",
+                                         args.steps, *hvs_work([(h, w)] * 3 * n), fp64)
+    for k in ("vif_gop32_1080p_yuv420", "vif_kodak_x1176_rgb", "hvs_gop32_1080p_yuv420", "hvs_kodak_x1176_rgb"):
+        # which roofline is nearer
         v = out[k]
         v["bound"] = "fp64" if v["share_of_fp64_rate"] > v["share_of_3.35TB_per_s"] else "hbm"
     print(json.dumps(out))

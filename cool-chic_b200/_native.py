@@ -128,71 +128,43 @@ class CcdSweepJob(ctypes.Structure):
     ]
 
 
+# The frame jobs (CcdDistJob, CcdSsimJob, CcdVifJob, CcdHvsJob): the same inputs, their own results, the same tail
+_FRAME_JOB_INPUTS = [
+    ("d_planes", ctypes.c_void_p * 3),
+    ("d_src", ctypes.c_void_p),
+    ("h", ctypes.c_int32),
+    ("w", ctypes.c_int32),
+    ("chroma_shift", ctypes.c_int32),
+    ("bitdepth", ctypes.c_int32),
+    ("src_layout", ctypes.c_int32),
+]
+_FRAME_JOB_TAIL = [("bad_index", ctypes.c_int64), ("status", ctypes.c_int32)]
+
+
 class CcdDistJob(ctypes.Structure):
-    _fields_ = [
-        ("d_planes", ctypes.c_void_p * 3),
-        ("d_src", ctypes.c_void_p),
-        ("h", ctypes.c_int32),
-        ("w", ctypes.c_int32),
-        ("chroma_shift", ctypes.c_int32),
-        ("bitdepth", ctypes.c_int32),
-        ("src_layout", ctypes.c_int32),
-        ("d_map", ctypes.c_void_p),
-        ("sse", ctypes.c_uint64 * 3),
-        ("max_abs", ctypes.c_uint32 * 3),
-        ("bad_index", ctypes.c_int64),
-        ("status", ctypes.c_int32),
-    ]
+    _fields_ = _FRAME_JOB_INPUTS + [("d_map", ctypes.c_void_p), ("sse", ctypes.c_uint64 * 3),
+                                    ("max_abs", ctypes.c_uint32 * 3)] + _FRAME_JOB_TAIL
 
 
 class CcdSsimJob(ctypes.Structure):
-    _fields_ = [
-        ("d_planes", ctypes.c_void_p * 3),
-        ("d_src", ctypes.c_void_p),
-        ("h", ctypes.c_int32),
-        ("w", ctypes.c_int32),
-        ("chroma_shift", ctypes.c_int32),
-        ("bitdepth", ctypes.c_int32),
-        ("src_layout", ctypes.c_int32),
-        ("d_map", ctypes.c_void_p * 3),
-        ("cs", (ctypes.c_double * 5) * 3),
-        ("ssim", (ctypes.c_double * 5) * 3),
-        ("bad_index", ctypes.c_int64),
-        ("status", ctypes.c_int32),
-    ]
+    _fields_ = _FRAME_JOB_INPUTS + [("d_map", ctypes.c_void_p * 3), ("cs", (ctypes.c_double * 5) * 3),
+                                    ("ssim", (ctypes.c_double * 5) * 3)] + _FRAME_JOB_TAIL
 
 
 class CcdVifJob(ctypes.Structure):
-    _fields_ = [
-        ("d_planes", ctypes.c_void_p * 3),
-        ("d_src", ctypes.c_void_p),
-        ("h", ctypes.c_int32),
-        ("w", ctypes.c_int32),
-        ("chroma_shift", ctypes.c_int32),
-        ("bitdepth", ctypes.c_int32),
-        ("src_layout", ctypes.c_int32),
-        ("num", (ctypes.c_double * 4) * 3),
-        ("den", (ctypes.c_double * 4) * 3),
-        ("bad_index", ctypes.c_int64),
-        ("status", ctypes.c_int32),
-    ]
+    _fields_ = _FRAME_JOB_INPUTS + [("num", (ctypes.c_double * 4) * 3), ("den", (ctypes.c_double * 4) * 3)] + _FRAME_JOB_TAIL
 
 
 class CcdHvsJob(ctypes.Structure):
-    _fields_ = [
-        ("d_planes", ctypes.c_void_p * 3),
-        ("d_src", ctypes.c_void_p),
-        ("h", ctypes.c_int32),
-        ("w", ctypes.c_int32),
-        ("chroma_shift", ctypes.c_int32),
-        ("bitdepth", ctypes.c_int32),
-        ("src_layout", ctypes.c_int32),
-        ("d_map", ctypes.c_void_p * 3),
-        ("s_hvs_m", ctypes.c_double * 3),
-        ("s_hvs", ctypes.c_double * 3),
-        ("bad_index", ctypes.c_int64),
-        ("status", ctypes.c_int32),
-    ]
+    _fields_ = _FRAME_JOB_INPUTS + [("d_map", ctypes.c_void_p * 3), ("s_hvs_m", ctypes.c_double * 3),
+                                    ("s_hvs", ctypes.c_double * 3)] + _FRAME_JOB_TAIL
+
+
+def _source_fits(src, h, w, cs, bitdepth):
+    """(dtype ok, expected sample count) of source samples for an h x w frame with chroma shift cs: a contiguous CUDA
+    tensor, uint8 up to 8 bits and int16 (holding uint16) above, of h w + 2 (h >> cs)(w >> cs) samples"""
+    dtype_ok = src.is_cuda and src.is_contiguous() and src.dtype == (torch.uint8 if bitdepth <= 8 else torch.int16)
+    return dtype_ok, h * w + 2 * (h >> cs) * (w >> cs)
 
 
 class CcdInterFrame(ctypes.Structure):
@@ -799,11 +771,11 @@ class Context:
         for i, (fd, src, lay) in enumerate(zip(frames, sources, layouts)):
             ts, cs = _planes(fd.data, fd.frame_data_type)
             h, w = ts[0].shape[-2:]
-            if not (src.is_cuda and src.is_contiguous() and src.dtype == (torch.uint8 if fd.bitdepth <= 8 else torch.int16)):
+            dtype_ok, n = _source_fits(src, h, w, cs, fd.bitdepth)
+            if not dtype_ok:
                 raise ValueError(f"sources[{i}] must be a contiguous {'uint8' if fd.bitdepth <= 8 else 'int16'} CUDA tensor")
-            if src.numel() != h * w + 2 * (h >> cs) * (w >> cs):
-                raise ValueError(f"sources[{i}] holds {src.numel()} samples, a {h}x{w} {fd.frame_data_type} frame has "
-                                 f"{h * w + 2 * (h >> cs) * (w >> cs)}")
+            if src.numel() != n:
+                raise ValueError(f"sources[{i}] holds {src.numel()} samples, a {h}x{w} {fd.frame_data_type} frame has {n}")
             keep += [ts, src]
             planes.append(ts)
             for c in range(3):
@@ -812,6 +784,12 @@ class Context:
             jobs[i].h, jobs[i].w, jobs[i].chroma_shift, jobs[i].bitdepth = h, w, cs, int(fd.bitdepth)
             jobs[i].src_layout = SOURCE_LAYOUTS[lay]
         return jobs, keep, planes
+
+    def _plane_maps(self, jobs, res, planes, shape):
+        """Per frame one float32 CUDA map per plane, of shape(h_c, w_c), in res[i]["maps"] and jobs[i].d_map"""
+        for job, r, ts in zip(jobs, res, planes):
+            r["maps"] = [torch.empty(shape(*t.shape[-2:]), dtype=torch.float32, device=self.torch_device) for t in ts]
+            job.d_map[:] = [m.data_ptr() for m in r["maps"]]
 
     def frame_distortion(self, frames, sources: Sequence[torch.Tensor], layouts: Sequence[str],
                          want_maps: bool = False) -> List[dict]:
@@ -843,14 +821,9 @@ class Context:
         and on request ``maps``: per plane the scale-0 SSIM map ([h_c - 10, w_c - 10] float32 CUDA)."""
         n = len(frames)
         jobs, keep, planes = self._frame_jobs(CcdSsimJob, frames, sources, layouts)
-        res = []
-        for i in range(n):
-            r = {}
-            if want_maps:
-                r["maps"] = [torch.empty((max(t.shape[-2] - 10, 0), max(t.shape[-1] - 10, 0)), dtype=torch.float32,
-                                         device=self.torch_device) for t in planes[i]]
-                jobs[i].d_map[:] = [m.data_ptr() for m in r["maps"]]
-            res.append(r)
+        res = [{} for _ in range(n)]
+        if want_maps:
+            self._plane_maps(jobs, res, planes, lambda h, w: (max(h - 10, 0), max(w - 10, 0)))
         _check(self._lib.ccd_frame_ssim(self._h, jobs, n, self._stream()), jobs)
         for i in range(n):
             res[i]["cs"] = [list(jobs[i].cs[c]) for c in range(3)]
@@ -877,19 +850,20 @@ class Context:
         each block's S_hvs_m / 64 / 255^2 ([h_c >> 3, w_c >> 3] float32 CUDA)."""
         n = len(frames)
         jobs, keep, planes = self._frame_jobs(CcdHvsJob, frames, sources, layouts)
-        res = []
-        for i in range(n):
-            r = {"n_coeffs": [64 * (t.shape[-2] >> 3) * (t.shape[-1] >> 3) for t in planes[i]]}
-            if want_maps:
-                r["maps"] = [torch.empty((t.shape[-2] >> 3, t.shape[-1] >> 3), dtype=torch.float32,
-                                         device=self.torch_device) for t in planes[i]]
-                jobs[i].d_map[:] = [m.data_ptr() for m in r["maps"]]
-            res.append(r)
+        res = [{"n_coeffs": [64 * (t.shape[-2] >> 3) * (t.shape[-1] >> 3) for t in planes[i]]} for i in range(n)]
+        if want_maps:
+            self._plane_maps(jobs, res, planes, lambda h, w: (h >> 3, w >> 3))
         _check(self._lib.ccd_frame_hvs(self._h, jobs, n, self._stream()), jobs)
         for i in range(n):
             res[i]["s_hvs_m"] = list(jobs[i].s_hvs_m)
             res[i]["s_hvs"] = list(jobs[i].s_hvs)
         return res
+
+    @staticmethod
+    def _check_inter_source(source, h, w, frame_data_type, bitdepth):
+        dtype_ok, n = _source_fits(source, h, w, 1 if frame_data_type == "yuv420" else 0, bitdepth)
+        if not (dtype_ok and source.numel() == n):
+            raise ValueError(f"source must hold the {h}x{w} {frame_data_type} frame's samples, contiguous on the device")
 
     def inter_stats(self, residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow, warp_filter_size,
                     source: Optional[torch.Tensor] = None, layout: str = "planar", want_maps: bool = False) -> dict:
@@ -900,10 +874,7 @@ class Context:
         f, keep, h, w = self._inter_frame(residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow,
                                           warp_filter_size)
         if source is not None:
-            cs = 1 if frame_data_type == "yuv420" else 0
-            if not (source.is_cuda and source.is_contiguous() and source.dtype == (torch.uint8 if bitdepth <= 8 else torch.int16)
-                    and source.numel() == h * w + 2 * (h >> cs) * (w >> cs)):
-                raise ValueError(f"source must hold the {h}x{w} {frame_data_type} frame's samples, contiguous on the device")
+            self._check_inter_source(source, h, w, frame_data_type, bitdepth)
         dev = self.torch_device
         out = {}
         if want_maps:
@@ -928,10 +899,7 @@ class Context:
         ``flow`` ([2, H, W] float32 CUDA, the total displacement)."""
         f, keep, h, w = self._inter_frame(residue, motion, refs, is_b, frame_data_type, bitdepth, global_flow,
                                           warp_filter_size)
-        cs = 1 if frame_data_type == "yuv420" else 0
-        if not (source.is_cuda and source.is_contiguous() and source.dtype == (torch.uint8 if bitdepth <= 8 else torch.int16)
-                and source.numel() == h * w + 2 * (h >> cs) * (w >> cs)):
-            raise ValueError(f"source must hold the {h}x{w} {frame_data_type} frame's samples, contiguous on the device")
+        self._check_inter_source(source, h, w, frame_data_type, bitdepth)
         n_ref = 2 if is_b else 1
         flows = [torch.empty((2, h, w), dtype=torch.float32, device=self.torch_device) for _ in range(n_ref)] if want_maps else []
         an = CcdInterAnalysis(d_src=source.data_ptr(), src_layout=SOURCE_LAYOUTS[layout])

@@ -2082,12 +2082,114 @@ int check_frame_job(Job &J, int i) {
     return CCD_OK;
 }
 
-// The message of a job whose decoded frame has a sample off the k / M grid (report(), after the kernel)
-extern "C++" template <class Job>
-int off_grid_error(const Job &J, int i) {
-    return fail(CCD_ERR_ARG, "job %d: decoded sample %lld is off the k / (2^%d - 1) grid", i, (long long)J.bad_index,
-                J.bitdepth);
+extern "C++" {
+// Plane c of a frame job: its height, or its width when width
+template <class Job>
+int plane_side(const Job &J, int c, bool width) {
+    return (width ? J.w : J.h) >> (c ? J.chroma_shift : 0);
 }
+
+// The tiles of a call of MS-SSIM, VIF or PSNR-HVS-M (one scale) in the order locate_tile (ccd_synth.cu) walks them:
+// per job and scale, plane 0's tiles, then plane 1's, then plane 2's, each tile one pair of f64 partials.
+struct TilePlan {
+    int S = 1;
+    std::vector<int> tiles;       // [job][scale][plane]
+    std::vector<size_t> part_at;  // [job][scale]: the first partial pair
+    std::vector<size_t> lvl_at;   // [job][scale][plane]: scales 1.. of the plane in the context's scratch
+    size_t n_part = 0, lvl_bytes = 0;
+    int max_tiles[CCD_SSIM_SCALES] = {};  // the most tiles of one job at each scale
+    // f(i, c, s, a, b): the two sums of plane c of job i at scale s, its tiles' partial pairs added in tile order
+    template <class F>
+    void sums(const double *part, int n_jobs, F &&f) const {
+        for (int i = 0; i < n_jobs; i++)
+            for (int s = 0; s < S; s++) {
+                const double *p = part + 2 * part_at[(size_t)i * S + s];
+                for (int c = 0; c < 3; c++) {
+                    const size_t t = (size_t)tiles[((size_t)i * S + s) * 3 + c];
+                    f(i, c, s, ordered_sum(p, t, 2), ordered_sum(p + 1, t, 2));
+                    p += 2 * t;
+                }
+            }
+    }
+};
+
+// Checks the jobs and plans their tiles: side(n, s) is a side of n samples at scale s and tiles(h, w) the tiles of an
+// h x w plane, as the kernels locate them; scales 1.. take sample_bytes per sample of scratch (0: none); every plane
+// needs both sides >= min_side.
+template <class Job, class Side, class Tiles>
+int plan_tiles(TilePlan &P, Job *jobs, int n_jobs, int S, Side side, Tiles tiles, size_t sample_bytes, const char *metric,
+               int min_side) {
+    const size_t n = (size_t)n_jobs;
+    P.S = S;
+    P.tiles.resize(n * S * 3);
+    P.part_at.resize(n * S);
+    P.lvl_at.resize(n * S * 3);
+    for (int i = 0; i < n_jobs; i++) {
+        if (int rc = check_frame_job(jobs[i], i)) return rc;
+        for (int c = 0; c < 3; c++)
+            if (std::min(plane_side(jobs[i], c, false), plane_side(jobs[i], c, true)) < min_side)
+                return jobs[i].status = fail(CCD_ERR_ARG, "job %d: plane %d is %dx%d, %s needs both sides >= %d", i, c,
+                                             plane_side(jobs[i], c, true), plane_side(jobs[i], c, false), metric, min_side);
+        for (int s = 0; s < S; s++) {
+            const size_t is = (size_t)i * S + s;
+            P.part_at[is] = P.n_part;
+            int t = 0;
+            for (int c = 0; c < 3; c++) {
+                const int h = side(plane_side(jobs[i], c, false), s), w = side(plane_side(jobs[i], c, true), s);
+                t += P.tiles[is * 3 + c] = tiles(h, w);
+                P.lvl_at[is * 3 + c] = P.lvl_bytes;
+                if (s > 0) P.lvl_bytes += al(sample_bytes * (size_t)h * w);
+            }
+            P.max_tiles[s] = std::max(P.max_tiles[s], t);
+            P.n_part += (size_t)t;
+        }
+    }
+    return CCD_OK;
+}
+
+// The call path of a metric against the source (ccd_frame_distortion, _ssim, _vif, _hvs), after the jobs' checks: one
+// arena of the device jobs, the bad words (~0) and the metric's results region of res_bytes, the first res_up of which
+// go up zeroed with the jobs (the kernels write the rest), and scratch_bytes of the context's scratch.  fill(i, D, res)
+// sets the metric's own fields of job i (res: the results region on the device), launch(d_jobs) runs its kernels and
+// read(res) takes the downloaded results.
+template <class Dev, class Job, class Fill, class Launch, class Read>
+int frame_pair_call(CcdContext *ctx, Job *jobs, int n_jobs, const char *what, size_t res_bytes, size_t res_up,
+                    size_t scratch_bytes, cudaStream_t st, Fill &&fill, Launch &&launch, Read &&read) {
+    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
+    Arena A;
+    const size_t n = (size_t)n_jobs, off_jobs = A.take(sizeof(Dev) * n), off_bad = A.take(8 * n, 8);
+    const size_t off_res = A.take(res_bytes, 8);
+    if (int rc = stage(ctx, A)) return rc;
+    if (int rc = ensure_dev(ctx->scratch, scratch_bytes)) return rc;
+    memset(A.h + off_bad, 0xff, 8 * n);
+    memset(A.h + off_res, 0, res_up);
+    for (int i = 0; i < n_jobs; i++) {
+        const Job &J = jobs[i];
+        Dev D;
+        memset(&D, 0, sizeof(D));
+        for (int c = 0; c < 3; c++) D.p[c] = J.d_planes[c];
+        D.src = J.d_src;
+        D.h = J.h;
+        D.w = J.w;
+        D.cs = J.chroma_shift;
+        D.hwc = J.src_layout;
+        D.wide = J.bitdepth > 8;
+        D.M = (float)((1 << J.bitdepth) - 1);  // exact
+        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
+        fill(i, D, A.dv + off_res);
+        memcpy(A.h + off_jobs + sizeof(Dev) * (size_t)i, &D, sizeof(D));
+    }
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_res + res_up, cudaMemcpyHostToDevice, st));
+    if (int e = launch(reinterpret_cast<const Dev *>(A.dv + off_jobs)))
+        return fail(CCD_ERR_CUDA, "%s launch failed: %s", what, cudaGetErrorString((cudaError_t)e));
+    if (int rc = download(A, off_bad, st, what)) return rc;
+    read(A.h + off_res);
+    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {
+        return fail(CCD_ERR_ARG, "job %d: decoded sample %lld is off the k / (2^%d - 1) grid", i,
+                    (long long)jobs[i].bad_index, jobs[i].bitdepth);
+    });
+}
+}  // extern "C++"
 
 static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, cudaStream_t st) {
     int64_t max_pixels = 1;
@@ -2095,42 +2197,22 @@ static int frame_distortion_body(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, 
         if (int rc = check_frame_job(jobs[i], i)) return rc;
         max_pixels = std::max(max_pixels, (int64_t)jobs[i].h * jobs[i].w);
     }
-    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
-    // the job array, then the results: sse[n][3] and max_abs[n][3] zeroed, bad[n] ~0
-    Arena A;
-    const size_t n = (size_t)n_jobs, off_jobs = A.take(sizeof(DistJobDev) * n), off_sse = A.take(24 * n);
-    const size_t off_bad = A.take(8 * n, 8), off_max = A.take(12 * n, 4);
-    if (int rc = stage(ctx, A)) return rc;
-    memset(A.h + off_sse, 0, A.end - off_sse);
-    memset(A.h + off_bad, 0xff, 8 * n);
-    for (int i = 0; i < n_jobs; i++) {
-        const CcdDistJob &J = jobs[i];
-        DistJobDev D;
-        for (int c = 0; c < 3; c++) D.p[c] = J.d_planes[c];
-        D.src = J.d_src;
-        D.map = J.d_map;
-        D.h = J.h;
-        D.w = J.w;
-        D.cs = J.chroma_shift;
-        D.hwc = J.src_layout;
-        const double M = (double)((1 << J.bitdepth) - 1);
-        D.M = (float)M;
-        D.M2 = (float)(M * M);
-        D.wide = J.bitdepth > 8;
-        D.sse = reinterpret_cast<unsigned long long *>(A.dv + off_sse) + 3 * i;
-        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
-        D.max_abs = reinterpret_cast<unsigned int *>(A.dv + off_max) + 3 * i;
-        memcpy(A.h + off_jobs + sizeof(DistJobDev) * (size_t)i, &D, sizeof(D));
-    }
-    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, A.end, cudaMemcpyHostToDevice, st));
-    int e = ccd_dist_launch(reinterpret_cast<const DistJobDev *>(A.dv + off_jobs), n_jobs, max_pixels, ctx->n_sm, st);
-    if (e != 0) return fail(CCD_ERR_CUDA, "frame distortion launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    if (int rc = download(A, off_sse, st, "frame distortion")) return rc;
-    for (int i = 0; i < n_jobs; i++) {
-        memcpy(jobs[i].sse, A.h + off_sse + 24 * (size_t)i, 24);
-        memcpy(jobs[i].max_abs, A.h + off_max + 12 * (size_t)i, 12);
-    }
-    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) { return off_grid_error(jobs[i], i); });
+    const size_t n = (size_t)n_jobs;  // the results: sse[n][3], then max_abs[n][3], zeroed
+    return frame_pair_call<DistJobDev>(
+        ctx, jobs, n_jobs, "frame distortion", 36 * n, 36 * n, 0, st,
+        [&](int i, DistJobDev &D, unsigned char *res) {
+            D.map = jobs[i].d_map;
+            D.M2 = (float)((double)D.M * D.M);
+            D.sse = reinterpret_cast<unsigned long long *>(res) + 3 * i;
+            D.max_abs = reinterpret_cast<unsigned int *>(res + 24 * n) + 3 * i;
+        },
+        [&](const DistJobDev *d) { return ccd_dist_launch(d, n_jobs, max_pixels, ctx->n_sm, st); },
+        [&](const unsigned char *res) {
+            for (int i = 0; i < n_jobs; i++) {
+                memcpy(jobs[i].sse, res + 24 * (size_t)i, 24);
+                memcpy(jobs[i].max_abs, res + 24 * n + 12 * (size_t)i, 12);
+            }
+        });
 }
 
 int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cuda_stream) {
@@ -2139,90 +2221,33 @@ int ccd_frame_distortion(CcdContext *ctx, CcdDistJob *jobs, int n_jobs, void *cu
 
 static int frame_ssim_body(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, cudaStream_t st) {
     constexpr int S = CCD_SSIM_SCALES;
-    const size_t n = (size_t)n_jobs;
-    auto side = [&](int i, int c, int j, bool width) {  // plane c of job i at scale j
-        const CcdSsimJob &J = jobs[i];
-        return ((width ? J.w : J.h) >> (c ? J.chroma_shift : 0)) >> j;
-    };
-    auto tiles = [&](int i, int c, int j) { return ccd_ssim_tiles(side(i, c, j, false), side(i, c, j, true)); };
-    // the job's partials at scale j start at part_at[i * S + j] (pairs, planes in order); the pyramid levels 1..4 of
-    // every plane of every job, one after the other, in the context's scratch
-    std::vector<size_t> part_at(n * S);
-    size_t n_part = 0, pyr_bytes = 0;
-    int max_tiles[S] = {0, 0, 0, 0, 0};
-    for (int i = 0; i < n_jobs; i++) {
-        if (int rc = check_frame_job(jobs[i], i)) return rc;
-        for (int c = 0; c < 3; c++)
-            if (std::min(side(i, c, 0, false), side(i, c, 0, true)) < 176)
-                return jobs[i].status = fail(CCD_ERR_ARG, "job %d: plane %d is %dx%d, MS-SSIM needs both sides >= 176", i, c,
-                                             side(i, c, 0, true), side(i, c, 0, false));
-        for (int j = 0; j < S; j++) {
-            part_at[(size_t)i * S + j] = n_part;
-            const int t = tiles(i, 0, j) + tiles(i, 1, j) + tiles(i, 2, j);
-            max_tiles[j] = std::max(max_tiles[j], t);
-            n_part += (size_t)t;
-            for (int c = 0; j > 0 && c < 3; c++) pyr_bytes += al(sizeof(uint2) * (size_t)side(i, c, j, false) * side(i, c, j, true));
-        }
-    }
-    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
-    // the job array, then the results: bad[n] ~0, then the partials, which are not uploaded
-    Arena A;
-    const size_t off_jobs = A.take(sizeof(SsimJobDev) * n), off_bad = A.take(8 * n, 8);
-    const size_t off_part = A.take(2 * sizeof(double) * n_part, 8);
-    if (int rc = stage(ctx, A)) return rc;
-    if (int rc = ensure_dev(ctx->scratch, pyr_bytes)) return rc;
-    memset(A.h + off_bad, 0xff, 8 * n);
-    double *d_part = reinterpret_cast<double *>(A.dv + off_part);
-    unsigned char *pyr = ctx->scratch.p;
-    for (int i = 0; i < n_jobs; i++) {
-        const CcdSsimJob &J = jobs[i];
-        SsimJobDev D;
-        memset(&D, 0, sizeof(D));
-        for (int c = 0; c < 3; c++) {
-            D.p[c] = J.d_planes[c];
-            D.map[c] = J.d_map[c];
-        }
-        for (int j = 0; j < S; j++) {
-            D.part[j] = d_part + 2 * part_at[(size_t)i * S + j];
-            for (int c = 0; j > 0 && c < 3; c++) {
-                D.lvl[c][j] = reinterpret_cast<uint2 *>(pyr);
-                pyr += al(sizeof(uint2) * (size_t)side(i, c, j, false) * side(i, c, j, true));
-            }
-        }
-        D.src = J.d_src;
-        D.h = J.h;
-        D.w = J.w;
-        D.cs = J.chroma_shift;
-        D.hwc = J.src_layout;
-        D.wide = J.bitdepth > 8;
-        const double M = (double)((1 << J.bitdepth) - 1);
-        D.M = (float)M;
-        D.C1 = (0.01 * M) * (0.01 * M);
-        D.C2 = (0.03 * M) * (0.03 * M);
-        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
-        memcpy(A.h + off_jobs + sizeof(SsimJobDev) * (size_t)i, &D, sizeof(D));
-    }
+    auto side = [](int n, int j) { return n >> j; };
+    TilePlan P;
+    if (int rc = plan_tiles(P, jobs, n_jobs, S, side, ccd_ssim_tiles, sizeof(uint2), "MS-SSIM", 176)) return rc;
     double g[11], gs = 0.0;  // the Gaussian window, sigma 1.5, normalised to sum 1
     for (int k = 0; k < 11; k++) gs += (g[k] = std::exp(-(double)((k - 5) * (k - 5)) / (2.0 * 1.5 * 1.5)));
     for (int k = 0; k < 11; k++) g[k] /= gs;
-    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
-    int e = ccd_ssim_launch(reinterpret_cast<const SsimJobDev *>(A.dv + off_jobs), n_jobs, max_tiles, g, st);
-    if (e != 0) return fail(CCD_ERR_CUDA, "MS-SSIM launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    if (int rc = download(A, off_bad, st, "MS-SSIM")) return rc;
-    const double *part = reinterpret_cast<const double *>(A.h + off_part);
-    for (int i = 0; i < n_jobs; i++) {
-        for (int j = 0; j < S; j++) {
-            const double *p = part + 2 * part_at[(size_t)i * S + j];  // the planes' tiles in order
-            for (int c = 0; c < 3; c++) {
-                const size_t t = (size_t)tiles(i, c, j);
-                const double n_pos = (double)(side(i, c, j, false) - CCD_SSIM_HALO) * (side(i, c, j, true) - CCD_SSIM_HALO);
-                jobs[i].cs[c][j] = ordered_sum(p, t, 2) / n_pos;
-                jobs[i].ssim[c][j] = ordered_sum(p + 1, t, 2) / n_pos;
-                p += 2 * t;
+    return frame_pair_call<SsimJobDev>(
+        ctx, jobs, n_jobs, "MS-SSIM", 16 * P.n_part, 0, P.lvl_bytes, st,
+        [&](int i, SsimJobDev &D, unsigned char *res) {
+            for (int c = 0; c < 3; c++) D.map[c] = jobs[i].d_map[c];
+            for (int j = 0; j < S; j++) {
+                D.part[j] = reinterpret_cast<double *>(res) + 2 * P.part_at[(size_t)i * S + j];
+                for (int c = 0; j > 0 && c < 3; c++)
+                    D.lvl[c][j] = reinterpret_cast<uint2 *>(ctx->scratch.p + P.lvl_at[((size_t)i * S + j) * 3 + c]);
             }
-        }
-    }
-    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) { return off_grid_error(jobs[i], i); });
+            D.C1 = (0.01 * D.M) * (0.01 * D.M);
+            D.C2 = (0.03 * D.M) * (0.03 * D.M);
+        },
+        [&](const SsimJobDev *d) { return ccd_ssim_launch(d, n_jobs, P.max_tiles, g, st); },
+        [&](const unsigned char *res) {
+            P.sums(reinterpret_cast<const double *>(res), n_jobs, [&](int i, int c, int j, double a, double b) {
+                const double n_pos = (double)(side(plane_side(jobs[i], c, false), j) - CCD_SSIM_HALO) *
+                                     (side(plane_side(jobs[i], c, true), j) - CCD_SSIM_HALO);
+                jobs[i].cs[c][j] = a / n_pos;
+                jobs[i].ssim[c][j] = b / n_pos;
+            });
+        });
 }
 
 int ccd_frame_ssim(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, void *cuda_stream) {
@@ -2231,64 +2256,8 @@ int ccd_frame_ssim(CcdContext *ctx, CcdSsimJob *jobs, int n_jobs, void *cuda_str
 
 static int frame_vif_body(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, cudaStream_t st) {
     constexpr int S = CCD_VIF_SCALES;
-    const size_t n = (size_t)n_jobs;
-    auto side = [&](int i, int c, int s, bool width) {  // plane c of job i at scale s
-        const CcdVifJob &J = jobs[i];
-        return ccd_vif_side((width ? J.w : J.h) >> (c ? J.chroma_shift : 0), s);
-    };
-    auto tiles = [&](int i, int c, int s) { return ccd_ssim_tiles(side(i, c, s, false), side(i, c, s, true)); };
-    // the job's partials at scale s start at part_at[i * S + s] (pairs, planes in order); scales 1..3 of every plane of
-    // every job, one after the other, in the context's scratch
-    std::vector<size_t> part_at(n * S);
-    size_t n_part = 0, pyr_bytes = 0;
-    int max_tiles[S] = {0, 0, 0, 0};
-    for (int i = 0; i < n_jobs; i++) {
-        if (int rc = check_frame_job(jobs[i], i)) return rc;
-        for (int c = 0; c < 3; c++)  // a valid output at the last scale: both sides >= 41
-            if (std::min(side(i, c, S - 1, false), side(i, c, S - 1, true)) < ccd_vif_taps(S - 1))
-                return jobs[i].status = fail(CCD_ERR_ARG, "job %d: plane %d is %dx%d, VIF needs both sides >= 41", i, c,
-                                             side(i, c, 0, true), side(i, c, 0, false));
-        for (int s = 0; s < S; s++) {
-            part_at[(size_t)i * S + s] = n_part;
-            const int t = tiles(i, 0, s) + tiles(i, 1, s) + tiles(i, 2, s);
-            max_tiles[s] = std::max(max_tiles[s], t);
-            n_part += (size_t)t;
-            for (int c = 0; s > 0 && c < 3; c++) pyr_bytes += al(sizeof(double2) * (size_t)side(i, c, s, false) * side(i, c, s, true));
-        }
-    }
-    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
-    // the job array, then the results: bad[n] ~0, then the partials, which are not uploaded
-    Arena A;
-    const size_t off_jobs = A.take(sizeof(VifJobDev) * n), off_bad = A.take(8 * n, 8);
-    const size_t off_part = A.take(2 * sizeof(double) * n_part, 8);
-    if (int rc = stage(ctx, A)) return rc;
-    if (int rc = ensure_dev(ctx->scratch, pyr_bytes)) return rc;
-    memset(A.h + off_bad, 0xff, 8 * n);
-    double *d_part = reinterpret_cast<double *>(A.dv + off_part);
-    unsigned char *pyr = ctx->scratch.p;
-    for (int i = 0; i < n_jobs; i++) {
-        const CcdVifJob &J = jobs[i];
-        VifJobDev D;
-        memset(&D, 0, sizeof(D));
-        for (int c = 0; c < 3; c++) D.p[c] = J.d_planes[c];
-        for (int s = 0; s < S; s++) {
-            D.part[s] = d_part + 2 * part_at[(size_t)i * S + s];
-            for (int c = 0; s > 0 && c < 3; c++) {
-                D.lvl[c][s] = reinterpret_cast<double2 *>(pyr);
-                pyr += al(sizeof(double2) * (size_t)side(i, c, s, false) * side(i, c, s, true));
-            }
-        }
-        D.src = J.d_src;
-        D.h = J.h;
-        D.w = J.w;
-        D.cs = J.chroma_shift;
-        D.hwc = J.src_layout;
-        D.wide = J.bitdepth > 8;
-        D.Md = (double)((1 << J.bitdepth) - 1);
-        D.M = (float)D.Md;
-        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
-        memcpy(A.h + off_jobs + sizeof(VifJobDev) * (size_t)i, &D, sizeof(D));
-    }
+    TilePlan P;  // 41: the least side with a valid output at the last scale, ccd_vif_side(41, 3) = ccd_vif_taps(3)
+    if (int rc = plan_tiles(P, jobs, n_jobs, S, ccd_vif_side, ccd_ssim_tiles, sizeof(double2), "VIF", 41)) return rc;
     double g[S][17] = {};  // scale s: N_s taps of a Gaussian with sigma N_s / 5, normalised to sum 1
     for (int s = 0; s < S; s++) {
         const int N = ccd_vif_taps(s);
@@ -2297,23 +2266,23 @@ static int frame_vif_body(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, cudaStre
         for (int k = 0; k < N; k++) gs += (g[s][k] = std::exp(-(double)((2 * k - (N - 1)) * (2 * k - (N - 1))) / (8.0 * sigma * sigma)));
         for (int k = 0; k < N; k++) g[s][k] /= gs;
     }
-    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
-    int e = ccd_vif_launch(reinterpret_cast<const VifJobDev *>(A.dv + off_jobs), n_jobs, max_tiles, g, st);
-    if (e != 0) return fail(CCD_ERR_CUDA, "VIF launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    if (int rc = download(A, off_bad, st, "VIF")) return rc;
-    const double *part = reinterpret_cast<const double *>(A.h + off_part);
-    for (int i = 0; i < n_jobs; i++) {
-        for (int s = 0; s < S; s++) {
-            const double *p = part + 2 * part_at[(size_t)i * S + s];  // the planes' tiles in order
-            for (int c = 0; c < 3; c++) {
-                const size_t t = (size_t)tiles(i, c, s);
-                jobs[i].num[c][s] = ordered_sum(p, t, 2);
-                jobs[i].den[c][s] = ordered_sum(p + 1, t, 2);
-                p += 2 * t;
+    return frame_pair_call<VifJobDev>(
+        ctx, jobs, n_jobs, "VIF", 16 * P.n_part, 0, P.lvl_bytes, st,
+        [&](int i, VifJobDev &D, unsigned char *res) {
+            for (int s = 0; s < S; s++) {
+                D.part[s] = reinterpret_cast<double *>(res) + 2 * P.part_at[(size_t)i * S + s];
+                for (int c = 0; s > 0 && c < 3; c++)
+                    D.lvl[c][s] = reinterpret_cast<double2 *>(ctx->scratch.p + P.lvl_at[((size_t)i * S + s) * 3 + c]);
             }
-        }
-    }
-    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) { return off_grid_error(jobs[i], i); });
+            D.Md = D.M;
+        },
+        [&](const VifJobDev *d) { return ccd_vif_launch(d, n_jobs, P.max_tiles, g, st); },
+        [&](const unsigned char *res) {
+            P.sums(reinterpret_cast<const double *>(res), n_jobs, [&](int i, int c, int s, double a, double b) {
+                jobs[i].num[c][s] = a;
+                jobs[i].den[c][s] = b;
+            });
+        });
 }
 
 int ccd_frame_vif(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, void *cuda_stream) {
@@ -2321,74 +2290,26 @@ int ccd_frame_vif(CcdContext *ctx, CcdVifJob *jobs, int n_jobs, void *cuda_strea
 }
 
 static int frame_hvs_body(CcdContext *ctx, CcdHvsJob *jobs, int n_jobs, cudaStream_t st) {
-    const size_t n = (size_t)n_jobs;
-    auto side = [&](int i, int c, bool width) {  // plane c of job i
-        const CcdHvsJob &J = jobs[i];
-        return (width ? J.w : J.h) >> (c ? J.chroma_shift : 0);
-    };
-    auto tiles = [&](int i, int c) { return ccd_hvs_tiles(side(i, c, false), side(i, c, true)); };
-    // the job's partials start at part_at[i] (pairs, planes in order)
-    std::vector<size_t> part_at(n);
-    size_t n_part = 0;
-    int max_tiles = 0;
-    for (int i = 0; i < n_jobs; i++) {
-        if (int rc = check_frame_job(jobs[i], i)) return rc;
-        for (int c = 0; c < 3; c++)  // one 8 x 8 block at least
-            if (std::min(side(i, c, false), side(i, c, true)) < 8)
-                return jobs[i].status = fail(CCD_ERR_ARG, "job %d: plane %d is %dx%d, PSNR-HVS-M needs both sides >= 8", i, c,
-                                             side(i, c, true), side(i, c, false));
-        part_at[(size_t)i] = n_part;
-        const int t = tiles(i, 0) + tiles(i, 1) + tiles(i, 2);
-        max_tiles = std::max(max_tiles, t);
-        n_part += (size_t)t;
-    }
-    if (n_jobs > 65535) return fail(CCD_ERR_UNSUPPORTED, "%d frames in one call (at most 65535)", n_jobs);
-    // the job array, then the results: bad[n] ~0, then the partials, which are not uploaded
-    Arena A;
-    const size_t off_jobs = A.take(sizeof(HvsJobDev) * n), off_bad = A.take(8 * n, 8);
-    const size_t off_part = A.take(2 * sizeof(double) * n_part, 8);
-    if (int rc = stage(ctx, A)) return rc;
-    memset(A.h + off_bad, 0xff, 8 * n);
-    double *d_part = reinterpret_cast<double *>(A.dv + off_part);
-    for (int i = 0; i < n_jobs; i++) {
-        const CcdHvsJob &J = jobs[i];
-        HvsJobDev D;
-        memset(&D, 0, sizeof(D));
-        for (int c = 0; c < 3; c++) {
-            D.p[c] = J.d_planes[c];
-            D.map[c] = J.d_map[c];
-        }
-        D.part = d_part + 2 * part_at[(size_t)i];
-        D.src = J.d_src;
-        D.h = J.h;
-        D.w = J.w;
-        D.cs = J.chroma_shift;
-        D.hwc = J.src_layout;
-        D.wide = J.bitdepth > 8;
-        D.Md = (double)((1 << J.bitdepth) - 1);
-        D.M = (float)D.Md;
-        D.s2 = (255.0 / D.Md) * (255.0 / D.Md);
-        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
-        memcpy(A.h + off_jobs + sizeof(HvsJobDev) * (size_t)i, &D, sizeof(D));
-    }
+    TilePlan P;  // one 8 x 8 block at least
+    if (int rc = plan_tiles(P, jobs, n_jobs, 1, [](int n, int) { return n; }, ccd_hvs_tiles, 0, "PSNR-HVS-M", 8)) return rc;
     double dct[8][8];  // the orthonormal DCT-II: dct[k][n] = a_k cos(pi (2n + 1) k / 16), a_0 = sqrt(1/8), a_k = 1/2
     for (int k = 0; k < 8; k++)
         for (int m = 0; m < 8; m++) dct[k][m] = (k ? 0.5 : std::sqrt(0.125)) * std::cos(std::acos(-1.0) * (2 * m + 1) * k / 16.0);
-    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
-    int e = ccd_hvs_launch(reinterpret_cast<const HvsJobDev *>(A.dv + off_jobs), n_jobs, max_tiles, dct, st);
-    if (e != 0) return fail(CCD_ERR_CUDA, "PSNR-HVS-M launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    if (int rc = download(A, off_bad, st, "PSNR-HVS-M")) return rc;
-    const double *part = reinterpret_cast<const double *>(A.h + off_part);
-    for (int i = 0; i < n_jobs; i++) {
-        const double *p = part + 2 * part_at[(size_t)i];  // the planes' tiles in order
-        for (int c = 0; c < 3; c++) {
-            const size_t t = (size_t)tiles(i, c);
-            jobs[i].s_hvs_m[c] = ordered_sum(p, t, 2);
-            jobs[i].s_hvs[c] = ordered_sum(p + 1, t, 2);
-            p += 2 * t;
-        }
-    }
-    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) { return off_grid_error(jobs[i], i); });
+    return frame_pair_call<HvsJobDev>(
+        ctx, jobs, n_jobs, "PSNR-HVS-M", 16 * P.n_part, 0, 0, st,
+        [&](int i, HvsJobDev &D, unsigned char *res) {
+            for (int c = 0; c < 3; c++) D.map[c] = jobs[i].d_map[c];
+            D.part = reinterpret_cast<double *>(res) + 2 * P.part_at[(size_t)i];
+            D.Md = D.M;
+            D.s2 = (255.0 / D.Md) * (255.0 / D.Md);
+        },
+        [&](const HvsJobDev *d) { return ccd_hvs_launch(d, n_jobs, P.max_tiles[0], dct, st); },
+        [&](const unsigned char *res) {
+            P.sums(reinterpret_cast<const double *>(res), n_jobs, [&](int i, int c, int, double a, double b) {
+                jobs[i].s_hvs_m[c] = a;
+                jobs[i].s_hvs[c] = b;
+            });
+        });
 }
 
 int ccd_frame_hvs(CcdContext *ctx, CcdHvsJob *jobs, int n_jobs, void *cuda_stream) {

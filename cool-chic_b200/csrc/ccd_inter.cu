@@ -276,8 +276,7 @@ __global__ void __launch_bounds__(128)
             for (int c = 0; c < 3; c++) {
                 const size_t k = o.src_hwc ? 3 * i + c
                                            : (c == 0 ? i : plane + (c - 1) * nc + (size_t)(y >> ref_cs) * wc + (x >> ref_cs));
-                const int ks = o.src_wide ? (int)__ldg(static_cast<const uint16_t *>(o.src) + k)
-                                          : (int)__ldg(static_cast<const uint8_t *>(o.src) + k);
+                const int ks = source_sample(o.src, o.src_wide, k);
                 const float orig = __fdiv_rn((float)ks, o.src_M);
                 float dummy = __fadd_rn(0.0f, ref_at(ref0, c, ref_cs, w, y, x));
                 if (is_b) dummy = __fadd_rn(dummy, ref_at(ref1, c, ref_cs, w, y, x));
@@ -378,8 +377,7 @@ __global__ void __launch_bounds__(128)
         for (int c = 0; c < 3; c++) {
             const size_t k = o.src_hwc ? 3 * i + c
                                        : (c == 0 ? i : plane + (c - 1) * nc + (size_t)(y >> ref_cs) * wc + (x >> ref_cs));
-            ks[c] = o.src_wide ? (int)__ldg(static_cast<const uint16_t *>(o.src) + k)
-                               : (int)__ldg(static_cast<const uint8_t *>(o.src) + k);
+            ks[c] = source_sample(o.src, o.src_wide, k);
         }
     }
     float res[3];

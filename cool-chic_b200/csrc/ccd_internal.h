@@ -265,22 +265,27 @@ int ccd_pack(const float *const planes[3], int h, int w, int cs, int bitdepth, i
              void *d_out, cudaStream_t st);
 int ccd_pack_flat(const float *d_in, size_t n, int bitdepth, int sample_bytes, void *d_out, cudaStream_t st);
 
-// Distortion of finished frames against their source samples (ccd_synth.cu, next to the packing kernels): one launch
-// for every job of a call, blockIdx.y = job.
-struct DistJobDev {
+// A finished frame and its source samples, as every metric against the source reads them (ccd_synth.cu, next to the
+// packing kernels): the first part of DistJobDev, SsimJobDev, VifJobDev and HvsJobDev.
+struct FramePairDev {
     const float *p[3];          // finished planes (FrameData layout); planes 1, 2 are [h >> cs][w >> cs]
     const void *src;            // source samples, uint8 (bitdepth <= 8) or uint16: planar, or [h][w][3] when hwc
-    float *map;                 // optional [h][w] error map
     int32_t h, w, cs, hwc;
-    float M, M2;                // 2^b - 1 and fp32(M^2)
     int32_t wide;               // 2-byte source samples
+    float M;                    // 2^b - 1
+    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
+};
+
+// Distortion: one launch for every job of a call, blockIdx.y = job.
+struct DistJobDev : FramePairDev {
+    float *map;                 // optional [h][w] error map
+    float M2;                   // fp32(M^2)
     unsigned long long *sse;    // [3], zeroed by the host
     unsigned int *max_abs;      // [3], zeroed by the host
-    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
 };
 int ccd_dist_launch(const DistJobDev *d_jobs, int n_jobs, int64_t max_pixels, int n_sm, cudaStream_t st);
 
-// A decoded sample read back to its integer kd = rint(v * M) (k_frame_dist, k_frame_ssim)
+// A decoded sample read back to its integer kd = rint(v * M) (read_pair in ccd_synth.cu)
 struct DecodedSample {
     float v, vm, kd;  // the decoded value, fp32(v * M), rint(v * M)
 };
@@ -292,22 +297,22 @@ static __device__ __forceinline__ DecodedSample read_decoded(const float *p, uns
 // the condition of its if, it compiles to the same branches as k_frame_dist had before it was shared.
 #define CCD_OFF_GRID(D) (!((D).v >= 0.0f && (D).v <= 1.0f) || fabsf(__fsub_rn((D).vm, (D).kd)) > 0.0625f)
 
+// Source sample k as uploaded (uint8, or uint16 when wide), never widened on the host
+static __device__ __forceinline__ int source_sample(const void *src, bool wide, size_t k) {
+    return wide ? (int)__ldg(static_cast<const uint16_t *>(src) + k) : (int)__ldg(static_cast<const uint8_t *>(src) + k);
+}
+
 // MS-SSIM (DESIGN §4.6): one k_frame_ssim launch per scale for every plane of every job of a call, blockIdx.y = job,
 // blockIdx.x = tile over the job's planes (plane 0's tiles, then plane 1's, then plane 2's, each row-major).  A tile owns
 // CCD_SSIM_T x CCD_SSIM_T samples of its plane's level (even origin) and reads a CCD_SSIM_HALO halo below and right.
 #define CCD_SSIM_T 32
 #define CCD_SSIM_HALO 10
 #define CCD_SSIM_SCALES 5
-struct SsimJobDev {
-    const float *p[3];          // finished planes (FrameData layout), read at scale 0
-    const void *src;            // source samples as for DistJobDev
+struct SsimJobDev : FramePairDev {
     float *map[3];              // optional scale-0 SSIM maps, [h_c - 10][w_c - 10]
     uint2 *lvl[3][CCD_SSIM_SCALES];  // pyramid levels 1..4 per plane: (decoded, source) 2 x 2 sums of the level above
     double *part[CCD_SSIM_SCALES];   // per scale: (sum cs, sum l cs) of each of the job's tiles, in tile order
-    int32_t h, w, cs, hwc, wide;
-    float M;
     double C1, C2;              // (0.01 M)^2, (0.03 M)^2
-    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
 };
 // tiles of one plane of h x w samples at some level
 static __host__ __device__ __forceinline__ int ccd_ssim_tiles(int h, int w) {
@@ -320,15 +325,10 @@ int ccd_ssim_launch(const SsimJobDev *d_jobs, int n_jobs, const int max_tiles[CC
 // VIF (DESIGN §4.12): one k_frame_vif<s> launch per scale, tiles as for MS-SSIM (ccd_ssim_tiles over the plane at scale
 // s); a tile stages CCD_SSIM_T + N_s - 1 rows and columns of both images and writes its share of scale s + 1.
 #define CCD_VIF_SCALES 4
-struct VifJobDev {
-    const float *p[3];          // finished planes (FrameData layout), read at scale 0
-    const void *src;            // source samples as for DistJobDev
+struct VifJobDev : FramePairDev {
     double2 *lvl[3][CCD_VIF_SCALES];  // scales 1..3 per plane: (decoded, source) in 8-bit units
     double *part[CCD_VIF_SCALES];     // per scale: (sum num, sum den) of each of the job's tiles, in tile order
-    int32_t h, w, cs, hwc, wide;
-    float M;
     double Md;                  // M in f64: a sample k is v = k * 255 / M
-    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
 };
 // the window of scale s: N_s = 2^(4 - s) + 1 taps
 static __host__ __device__ __forceinline__ constexpr int ccd_vif_taps(int s) { return (1 << (4 - s)) + 1; }
@@ -341,22 +341,16 @@ static __host__ __device__ __forceinline__ int ccd_vif_side(int n, int s) {
 int ccd_vif_launch(const VifJobDev *d_jobs, int n_jobs, const int max_tiles[CCD_VIF_SCALES], const double g[CCD_VIF_SCALES][17],
                    cudaStream_t st);
 
-// PSNR-HVS-M (DESIGN §4.13): one k_frame_hvs launch for every plane of every job of a call, blockIdx.y = job,
-// blockIdx.x = tile over the job's planes (plane 0's tiles, then plane 1's, then plane 2's, each row-major).  A tile is
-// a strip of CCD_HVS_ROWS rows and CCD_HVS_COLS columns of its plane; the tiles cover every sample (each is read once,
-// for the off-grid check), and only the 8 x 8 blocks that lie wholly inside the plane are measured.
+// PSNR-HVS-M (DESIGN §4.13): one k_frame_hvs launch for every plane of every job of a call, tiles laid out as for
+// MS-SSIM.  A tile is a strip of CCD_HVS_ROWS rows and CCD_HVS_COLS columns of its plane; the tiles cover every sample
+// (each is read once, for the off-grid check), and only the 8 x 8 blocks that lie wholly inside the plane are measured.
 #define CCD_HVS_ROWS 8
 #define CCD_HVS_COLS 256
-struct HvsJobDev {
-    const float *p[3];          // finished planes (FrameData layout)
-    const void *src;            // source samples as for DistJobDev
+struct HvsJobDev : FramePairDev {
     float *map[3];              // optional [h_c >> 3][w_c >> 3]: each block's S_hvs_m / 64 / 255^2
     double *part;               // (sum S_hvs_m, sum S_hvs) of each of the job's tiles, in tile order
-    int32_t h, w, cs, hwc, wide;
-    float M;
     double Md;                  // M in f64: a sample k is v = k * 255 / M
     double s2;                  // (255 / M)^2: integer variances to 8-bit units
-    unsigned long long *bad;    // smallest planar index of an off-grid decoded sample (~0 if none)
 };
 // tiles of one plane of h x w samples
 static __host__ __device__ __forceinline__ int ccd_hvs_tiles(int h, int w) {

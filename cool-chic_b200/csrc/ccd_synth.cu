@@ -1540,15 +1540,20 @@ int ccd_pack_flat(const float *d_in, size_t n, int bitdepth, int sample_bytes, v
 // [H][W][3], never widened on the host).  A thread owns pixels of the luma grid; with 4:2:0 chroma only the thread of
 // the even (x, y) counts the chroma sample, the others read it only for the error map.  Sums are integers: exact, and
 // the same whatever the order of the atomics.
-static __device__ __forceinline__ int source_sample(const void *src, bool wide, size_t k) {
-    return wide ? (int)__ldg(static_cast<const uint16_t *>(src) + k) : (int)__ldg(static_cast<const uint8_t *>(src) + k);
+// Sample s of plane c of a frame pair whose planes hold n0 and n1 samples (computed once per kernel): the decoded sample,
+// the source integer ks and the planar (FrameData) index that bad_index reports.  The caller tests CCD_OFF_GRID(d)
+// under its own condition.
+struct SamplePair { DecodedSample d; int ks; unsigned pidx; };
+static __device__ __forceinline__ SamplePair read_pair(const FramePairDev &F, int c, unsigned s, unsigned n0, unsigned n1) {
+    const DecodedSample D = read_decoded(F.p[c], s, F.M);
+    const unsigned pidx = c == 0 ? s : n0 + (unsigned)(c - 1) * n1 + s;
+    return SamplePair{D, source_sample(F.src, F.wide, F.hwc ? (size_t)s * 3 + c : (size_t)pidx), pidx};
 }
 
 __global__ void __launch_bounds__(256) k_frame_dist(const DistJobDev *__restrict__ jobs) {
     const DistJobDev &J = jobs[blockIdx.y];
     const unsigned w = (unsigned)J.w, cs = (unsigned)J.cs, n0 = (unsigned)J.h * w;
     const unsigned wc = w >> cs, n1 = ((unsigned)J.h >> cs) * wc;
-    const float M = J.M;
     const bool want_map = J.map != nullptr;
     unsigned long long s[3] = {0ull, 0ull, 0ull}, bad = ~0ull;
     unsigned mx[3] = {0u, 0u, 0u};
@@ -1559,19 +1564,14 @@ __global__ void __launch_bounds__(256) k_frame_dist(const DistJobDev *__restrict
 #pragma unroll
         for (int c = 0; c < 3; c++) {
             if (c > 0 && !own && !want_map) continue;
-            const unsigned j = c == 0 ? i : (y >> cs) * wc + (x >> cs);
-            const unsigned pidx = c == 0 ? i : n0 + (unsigned)(c - 1) * n1 + j;  // planar (FrameData) sample index
-            const size_t k = J.hwc ? (size_t)i * 3 + c : (size_t)pidx;
-            const DecodedSample D = read_decoded(J.p[c], j, M);
-            const float kd = D.kd;
-            const int ks = source_sample(J.src, J.wide, k);
-            const unsigned a = (unsigned)abs((int)kd - ks);
+            const SamplePair P = read_pair(J, c, c == 0 ? i : (y >> cs) * wc + (x >> cs), n0, n1);
+            const unsigned a = (unsigned)abs((int)P.d.kd - P.ks);
             const unsigned long long d2 = (unsigned long long)a * a;
             e += d2;
             if (c == 0 || own) {
                 s[c] += d2;
                 mx[c] = max(mx[c], a);
-                if (CCD_OFF_GRID(D)) bad = min(bad, (unsigned long long)pidx);
+                if (CCD_OFF_GRID(P.d)) bad = min(bad, (unsigned long long)P.pidx);
             }
         }
         if (want_map) J.map[i] = __fdiv_rn(__ull2float_rn(e), J.M2);
@@ -1615,6 +1615,24 @@ static_assert((CCD_SSIM_T / 2) * (CCD_SSIM_T / 2) == 32 * kTileWarps, "one next-
 static __device__ __forceinline__ void report_bad(unsigned long long bad, unsigned long long *out, int tid) {
     for (int o = 16; o > 0; o >>= 1) bad = min(bad, __shfl_down_sync(0xffffffffu, bad, o));
     if ((tid & 31) == 0 && bad != ~0ull) atomicMin(out, bad);
+}
+
+// The plane c and tile t of this CTA (MS-SSIM, VIF, PSNR-HVS-M: blockIdx.x = tile over the job's planes, plane 0's
+// tiles first), and that plane's h x w at this scale.  side(n): a side of n samples at this scale; tiles(h, w): the
+// tiles of a plane.  The host's TilePlan (ccd_api.cu) lays out the call from the same two.
+struct PlaneTile { int c, t, h, w; };  // c == 3: past the job's last tile
+template <class Side, class Tiles>
+static __device__ __forceinline__ PlaneTile locate_tile(const FramePairDev &F, Side side, Tiles tiles) {
+    int c = 0, t = (int)blockIdx.x, h = 0, w = 0;
+    for (;; c++) {
+        if (c == 3) break;
+        h = side(c ? F.h >> F.cs : F.h);
+        w = side(c ? F.w >> F.cs : F.w);
+        const int n = tiles(h, w);
+        if (t < n) break;
+        t -= n;
+    }
+    return PlaneTile{c, t, h, w};
 }
 
 // Horizontal pass: rows [0, In) of the staged [In][In] images sx, sy, filtered with the NT taps g at T positions per
@@ -1712,15 +1730,8 @@ __global__ void __launch_bounds__(32 * kTileWarps, 3) k_frame_ssim(const SsimJob
     double *sred = reinterpret_cast<double *>(sy + kSsimIn * kSsimIn);  // [warps][2]
     const SsimJobDev &J = jobs[blockIdx.y];
     const int j = a.scale, tid = (int)threadIdx.x;
-    int c = 0, t = (int)blockIdx.x, h = 0, w = 0;
-    for (;; c++) {  // the plane and tile of this CTA
-        if (c == 3) return;
-        h = (c ? J.h >> J.cs : J.h) >> j;
-        w = (c ? J.w >> J.cs : J.w) >> j;
-        const int n = ccd_ssim_tiles(h, w);
-        if (t < n) break;
-        t -= n;
-    }
+    const auto [c, t, h, w] = locate_tile(J, [j](int n) { return n >> j; }, ccd_ssim_tiles);
+    if (c == 3) return;
     const int tw = (w + T - 1) / T, y0 = t / tw * T, x0 = t % tw * T;
 
     unsigned long long bad = ~0ull;
@@ -1731,11 +1742,10 @@ __global__ void __launch_bounds__(32 * kTileWarps, 3) k_frame_ssim(const SsimJob
         if (y < h && x < w) {
             const unsigned s = (unsigned)y * (unsigned)w + (unsigned)x;
             if (j == 0) {
-                const DecodedSample D = read_decoded(J.p[c], s, J.M);
-                const unsigned pidx = c == 0 ? s : n0 + (unsigned)(c - 1) * n1 + s;  // as k_frame_dist reports it
-                vx = D.kd;
-                vy = source_sample(J.src, J.wide, J.hwc ? (size_t)s * 3 + c : (size_t)pidx);
-                if (r < T && q < T && CCD_OFF_GRID(D)) bad = min(bad, (unsigned long long)pidx);
+                const SamplePair P = read_pair(J, c, s, n0, n1);
+                vx = P.d.kd;
+                vy = (float)P.ks;
+                if (r < T && q < T && CCD_OFF_GRID(P.d)) bad = min(bad, (unsigned long long)P.pidx);
             } else {
                 const uint2 v = J.lvl[c][j][s];
                 vx = (float)v.x;
@@ -1833,15 +1843,8 @@ __global__ void __launch_bounds__(32 * kTileWarps, 2) k_frame_vif(const VifJobDe
     double *sred = sy + In * In;                     // [warps][2]
     const VifJobDev &J = jobs[blockIdx.y];
     const int tid = (int)threadIdx.x;
-    int c = 0, t = (int)blockIdx.x, h = 0, w = 0;
-    for (;; c++) {  // the plane and tile of this CTA
-        if (c == 3) return;
-        h = ccd_vif_side(c ? J.h >> J.cs : J.h, S);
-        w = ccd_vif_side(c ? J.w >> J.cs : J.w, S);
-        const int n = ccd_ssim_tiles(h, w);
-        if (t < n) break;
-        t -= n;
-    }
+    const auto [c, t, h, w] = locate_tile(J, [](int n) { return ccd_vif_side(n, S); }, ccd_ssim_tiles);
+    if (c == 3) return;
     const int tw = (w + T - 1) / T, y0 = t / tw * T, x0 = t % tw * T;
 
     unsigned long long bad = ~0ull;
@@ -1852,11 +1855,10 @@ __global__ void __launch_bounds__(32 * kTileWarps, 2) k_frame_vif(const VifJobDe
         if (y < h && x < w) {
             const unsigned s = (unsigned)y * (unsigned)w + (unsigned)x;
             if constexpr (S == 0) {
-                const DecodedSample D = read_decoded(J.p[c], s, J.M);
-                const unsigned pidx = c == 0 ? s : n0 + (unsigned)(c - 1) * n1 + s;  // as k_frame_dist reports it
-                vx = __ddiv_rn(__dmul_rn((double)D.kd, 255.0), J.Md);
-                vy = __ddiv_rn(__dmul_rn((double)source_sample(J.src, J.wide, J.hwc ? (size_t)s * 3 + c : (size_t)pidx), 255.0), J.Md);
-                if (r < T && q < T && CCD_OFF_GRID(D)) bad = min(bad, (unsigned long long)pidx);
+                const SamplePair P = read_pair(J, c, s, n0, n1);
+                vx = __ddiv_rn(__dmul_rn((double)P.d.kd, 255.0), J.Md);
+                vy = __ddiv_rn(__dmul_rn((double)P.ks, 255.0), J.Md);
+                if (r < T && q < T && CCD_OFF_GRID(P.d)) bad = min(bad, (unsigned long long)P.pidx);
             } else {
                 const double2 v = J.lvl[c][S][s];
                 vx = v.x;
@@ -2048,15 +2050,8 @@ __global__ void __launch_bounds__(32 * kTileWarps) k_frame_hvs(const HvsJobDev *
     int *si = reinterpret_cast<int *>(hvs_sm);
     const HvsJobDev &J = jobs[blockIdx.y];
     const int tid = (int)threadIdx.x;
-    int c = 0, t = (int)blockIdx.x, h = 0, w = 0;
-    for (;; c++) {  // the plane and tile of this CTA
-        if (c == 3) return;
-        h = c ? J.h >> J.cs : J.h;
-        w = c ? J.w >> J.cs : J.w;
-        const int n = ccd_hvs_tiles(h, w);
-        if (t < n) break;
-        t -= n;
-    }
+    const auto [c, t, h, w] = locate_tile(J, [](int n) { return n; }, ccd_hvs_tiles);
+    if (c == 3) return;
     const int tw = (w + W - 1) / W, y0 = t / tw * R, x0 = t % tw * W;
 
     // every sample of the strip, for the off-grid check; rows [0, R) of A (source), then of B (decoded)
@@ -2067,11 +2062,10 @@ __global__ void __launch_bounds__(32 * kTileWarps) k_frame_hvs(const HvsJobDev *
         int ka = 0, kb = 0;
         if (y < h && x < w) {
             const unsigned s = (unsigned)y * (unsigned)w + (unsigned)x;
-            const DecodedSample D = read_decoded(J.p[c], s, J.M);
-            const unsigned pidx = c == 0 ? s : n0 + (unsigned)(c - 1) * n1 + s;  // as k_frame_dist reports it
-            kb = (int)D.kd;
-            ka = source_sample(J.src, J.wide, J.hwc ? (size_t)s * 3 + c : (size_t)pidx);
-            if (CCD_OFF_GRID(D)) bad = min(bad, (unsigned long long)pidx);
+            const SamplePair P = read_pair(J, c, s, n0, n1);
+            kb = (int)P.d.kd;
+            ka = P.ks;
+            if (CCD_OFF_GRID(P.d)) bad = min(bad, (unsigned long long)P.pidx);
         }
         si[r * kHvsLd + q] = ka;
         si[(R + r) * kHvsLd + q] = kb;

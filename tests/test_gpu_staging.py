@@ -49,6 +49,9 @@ def test_one_copy_each_way_per_call(ctx, kodim14):
                                               "v": v.view(1, 1, h // 2, w // 2)}))
         srcs.append(k.to(torch.uint8))
     assert _copies(lambda: ctx.frame_distortion(frames, srcs, ["planar"] * 32)) == (1, 1)
+    assert _copies(lambda: ctx.frame_ssim(frames, srcs, ["planar"] * 32)) == (1, 1)
+    assert _copies(lambda: ctx.frame_vif(frames, srcs, ["planar"] * 32)) == (1, 1)
+    assert _copies(lambda: ctx.frame_hvs(frames, srcs, ["planar"] * 32)) == (1, 1)
 
     # one P frame: the statistics come back in one copy, and nothing goes up
     h, w = 128, 192

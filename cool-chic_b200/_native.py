@@ -167,6 +167,12 @@ def _source_fits(src, h, w, cs, bitdepth):
     return dtype_ok, h * w + 2 * (h >> cs) * (w >> cs)
 
 
+def _check_symbols(name, t, n, dtype=torch.int8, label="int8"):
+    """A ValueError naming t and its type (label) unless t is a contiguous dtype CUDA tensor of n symbols"""
+    if not (t.is_cuda and t.dtype == dtype and t.is_contiguous() and t.numel() == n):
+        raise ValueError(f"{name} must be a contiguous {label} CUDA tensor of {n} symbols")
+
+
 class CcdInterFrame(ctypes.Structure):
     _fields_ = [
         ("d_residue", ctypes.c_void_p),
@@ -437,8 +443,7 @@ class Context:
             jobs[i].grid_end = int(grid_ends[i])
             lat = latents[i] if latents is not None else None
             if lat is not None:
-                if not (lat.is_cuda and lat.dtype == torch.int8 and lat.is_contiguous() and lat.numel() == d.n_symbols()):
-                    raise ValueError(f"latents[{i}] must be a contiguous int8 CUDA tensor of {d.n_symbols()} symbols")
+                _check_symbols(f"latents[{i}]", lat, d.n_symbols())
                 jobs[i].d_latents = lat.data_ptr()
             st = states[i] if states is not None else None
             if st is not None:
@@ -494,8 +499,7 @@ class Context:
             d = descs[i]
             nn = np.ascontiguousarray(nn_ints[i], dtype=np.int64)
             lat = latents[i]
-            if not (lat.is_cuda and lat.dtype == torch.int8 and lat.is_contiguous() and lat.numel() == d.n_symbols()):
-                raise ValueError(f"latents[{i}] must be a contiguous int8 CUDA tensor of {d.n_symbols()} symbols")
+            _check_symbols(f"latents[{i}]", lat, d.n_symbols())
             keep += [nn, lat]
             jobs[i].desc = ctypes.pointer(d)
             jobs[i].nn_ints = nn.ctypes.data
@@ -689,8 +693,7 @@ class Context:
             d = descs[i]
             nn = np.ascontiguousarray(nn_ints[i], dtype=np.int64)
             lat = latents[i]
-            if not (lat.is_cuda and lat.dtype == torch.int8 and lat.is_contiguous() and lat.numel() == d.n_symbols()):
-                raise ValueError(f"latents[{i}] must be a contiguous int8 CUDA tensor of {d.n_symbols()} symbols")
+            _check_symbols(f"latents[{i}]", lat, d.n_symbols())
             r = {"bits": torch.empty((d.n_symbols(),), dtype=torch.float32, device=dev)}
             if want_freq:
                 r["freq"] = torch.empty((d.n_symbols(),), dtype=torch.int32, device=dev)
@@ -723,9 +726,7 @@ class Context:
         ``decode_nn`` order (ARM and IFCE integers only).  Returns (bits float64 [1 + k][n_grids], grid 0 = finest,
         row 0 the model itself; fast bool [1 + k]: the model takes the fast entropy kernel)."""
         nn = np.ascontiguousarray(nn_ints, dtype=np.int64)
-        if not (latents.is_cuda and latents.dtype == torch.int8 and latents.is_contiguous()
-                and latents.numel() == desc.n_symbols()):
-            raise ValueError(f"latents must be a contiguous int8 CUDA tensor of {desc.n_symbols()} symbols")
+        _check_symbols("latents", latents, desc.n_symbols())
         k = len(cands)
         arr = (CcdCandidate * max(k, 1))(*[CcdCandidate(int(i), int(dl)) for i, dl in cands])
         bits = np.zeros((k + 1, desc.n_grids), dtype=np.float64)
@@ -750,8 +751,7 @@ class Context:
         for i in range(n):
             d, lat, ms = descs[i], latents[i], mu_sc[i]
             for name, t, dt in (("latents", lat, torch.int8), ("mu_sc", ms, torch.int32)):
-                if not (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == d.n_symbols()):
-                    raise ValueError(f"{name}[{i}] must be a contiguous {dt} CUDA tensor of {d.n_symbols()} symbols")
+                _check_symbols(f"{name}[{i}]", t, d.n_symbols(), dt, str(dt))
             jobs[i].desc = ctypes.pointer(d)
             jobs[i].d_latents = lat.data_ptr()
             jobs[i].d_mu_sc = ms.data_ptr()

@@ -1709,14 +1709,65 @@ int ccd_synthesize_many(CcdContext *ctx, CcdSynthJob *jobs, int n_jobs, void *cu
     return job_call(ctx, jobs, n_jobs, cuda_stream, [&](cudaStream_t st) -> int { return synthesize_body(ctx, jobs, n_jobs, st); });
 }
 
+// The tiles of a rate-pass call (ccd_latent_rate, ccd_rate_sweep, ccd_rate_candidates) in the order the kernels
+// write their partials: per job, its grids in decode order, each grid's CCD_RATE_TH x CCD_RATE_TW tiles row by row.
+struct RateTilePlan {
+    std::vector<RateTile> tiles;
+    std::vector<size_t> at{0};       // the call's k-th grid: tiles [at[k], at[k + 1])
+    std::vector<size_t> grid_at{0};  // job i's decode-order grids: k in [grid_at[i], grid_at[i + 1])
+    void add(int job, const CcdCoolChicDesc *d) {
+        for (int gi = 0; gi < d->n_grids; gi++) {
+            const int g = d->n_grids - 1 - gi;
+            for (int y0 = 0; y0 < d->grid_h[g]; y0 += CCD_RATE_TH)
+                for (int x0 = 0; x0 < d->grid_w[g]; x0 += CCD_RATE_TW) tiles.push_back(RateTile{job, gi, y0, x0});
+            at.push_back(tiles.size());
+        }
+        grid_at.push_back(at.size() - 1);
+    }
+    int check() const {
+        return tiles.size() > (size_t)INT32_MAX ? fail(CCD_ERR_UNSUPPORTED, "too many rate tiles") : CCD_OK;
+    }
+    // grid g (finest first) of job i: partial k of stride s of its tiles, added in tile order
+    double sum(const double *part, int i, int g, size_t k = 0, size_t s = 1) const {
+        const size_t j = grid_at[(size_t)i + 1] - 1 - (size_t)g;
+        return ordered_sum(part + at[j] * s + k, at[j + 1] - at[j], s);
+    }
+};
+
+// CCD_OK, or the failure of a launch that returned CUDA error e
+static int launched(int e, const char *what) {
+    return e ? fail(CCD_ERR_CUDA, "%s launch failed: %s", what, cudaGetErrorString((cudaError_t)e)) : CCD_OK;
+}
+
+// The call path of a rate-pass call once A holds its other inputs: T's tiles, n_bad bad words (~0) and n_counters
+// counters (0) go up with them; `stride` partials per tile come back with the results.  fill(bad, counters) writes the
+// inputs into A.h, launch(tiles, n_tiles, part) runs the kernels, read(bad, counters, part) takes the results: all on
+// the device, but read's in A.h.  Returns read's status, or the first failure.
+extern "C++" template <class Fill, class Launch, class Read>
+int rate_call(CcdContext *ctx, Arena &A, const RateTilePlan &T, size_t n_bad, size_t n_counters, size_t stride,
+              const char *what, cudaStream_t st, Fill &&fill, Launch &&launch, Read &&read) {
+    using u64 = unsigned long long;
+    const size_t off_tiles = A.take(sizeof(RateTile) * T.tiles.size()), off_bad = A.take(sizeof(u64) * n_bad);
+    const size_t off_cnt = A.take(sizeof(u64) * n_counters), off_part = A.take(sizeof(double) * stride * T.tiles.size());
+    if (int rc = stage(ctx, A)) return rc;
+    memcpy(A.h + off_tiles, T.tiles.data(), sizeof(RateTile) * T.tiles.size());
+    memset(A.h + off_bad, 0xff, sizeof(u64) * n_bad);
+    memset(A.h + off_cnt, 0, sizeof(u64) * n_counters);
+    fill(reinterpret_cast<u64 *>(A.dv + off_bad), reinterpret_cast<u64 *>(A.dv + off_cnt));
+    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
+    const RateTile *tiles = reinterpret_cast<const RateTile *>(A.dv + off_tiles);
+    if (int rc = launch(tiles, (int)T.tiles.size(), reinterpret_cast<double *>(A.dv + off_part))) return rc;
+    if (int rc = download(A, off_bad, st, what)) return rc;
+    return read(reinterpret_cast<const u64 *>(A.h + off_bad), reinterpret_cast<const u64 *>(A.h + off_cnt),
+                reinterpret_cast<const double *>(A.h + off_part));
+}
+
 static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, const CcdModelEdit *edits, int n_jobs, cudaStream_t st) {
     if (edits)
         for (int i = 0; i < n_jobs; i++)
             if (int rc = check_edit(edits[i], jobs[i].desc, i)) return jobs[i].status = rc;
     std::vector<PreparedJob> P((size_t)n_jobs);
-    std::vector<RateTile> tiles;
-    // tiles of job i, decode-order grid gi: [tile_at[i][gi], tile_at[i][gi + 1])
-    std::vector<std::vector<size_t>> tile_at((size_t)n_jobs);
+    RateTilePlan T;
     std::vector<RateSpatialDev> sp;
     int64_t max_pixels = 0;
     Arena A;
@@ -1733,13 +1784,7 @@ static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, const CcdModelEdi
         J.off_blob = A.take(J.blob.size());
         smem = std::max(smem, ccd_rate_smem_bytes(J.es.arm_blob_bytes, J.es.ifce_blob_max));
         const CcdCoolChicDesc *d = J.d;
-        tile_at[(size_t)i].push_back(tiles.size());
-        for (int gi = 0; gi < d->n_grids; gi++) {
-            const EntGrid &G = J.es.grid[gi];
-            for (int y0 = 0; y0 < G.h; y0 += CCD_RATE_TH)
-                for (int x0 = 0; x0 < G.w; x0 += CCD_RATE_TW) tiles.push_back(RateTile{i, gi, y0, x0});
-            tile_at[(size_t)i].push_back(tiles.size());
-        }
+        T.add(i, d);
         if (R.d_spatial) {
             RateSpatialDev S;
             memset(&S, 0, sizeof(S));
@@ -1760,54 +1805,47 @@ static int latent_rate_body(CcdContext *ctx, CcdRateJob *jobs, const CcdModelEdi
             max_pixels = std::max(max_pixels, (int64_t)d->img_h * d->img_w);
         }
     }
-    if (tiles.size() > (size_t)INT32_MAX) return fail(CCD_ERR_UNSUPPORTED, "too many rate tiles");
+    if (int rc = T.check()) return rc;
     if (smem > CCD_SMEM_MAX) return fail(CCD_ERR_UNSUPPORTED, "rate pass needs %zu bytes of shared memory", smem);
     const size_t off_es = A.take(sizeof(EntStream) * (size_t)n_jobs);
     const size_t off_jobs = A.take(sizeof(RateJobDev) * (size_t)n_jobs);
-    const size_t off_tiles = A.take(sizeof(RateTile) * tiles.size());
     const size_t off_sp = A.take(sizeof(RateSpatialDev) * sp.size());
-    // results: the bad words (~0 before the launch), then the partials, which are not uploaded
-    const size_t off_bad = A.take(sizeof(unsigned long long) * (size_t)n_jobs);
-    const size_t off_part = A.take(sizeof(double) * tiles.size());
-    if (int rc = stage(ctx, A)) return rc;
-    memset(A.h + off_bad, 0xff, sizeof(unsigned long long) * (size_t)n_jobs);
-    for (int i = 0; i < n_jobs; i++) {
-        PreparedJob &J = P[(size_t)i];
-        memcpy(A.h + J.off_blob, J.blob.data(), J.blob.size());
-        J.es.latents = const_cast<int8_t *>(jobs[i].d_latents);
-        J.es.blob = A.dv + J.off_blob;
-        memcpy(A.h + off_es + sizeof(EntStream) * (size_t)i, &J.es, sizeof(EntStream));
-        RateJobDev D;
-        D.es = reinterpret_cast<const EntStream *>(A.dv + off_es) + i;
-        D.bits = jobs[i].d_bits;
-        D.freq = jobs[i].d_freq;
-        D.mu_sc = jobs[i].d_mu_sc;
-        D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
-        D.kind = ccd_rate_kind(J.d->n_ctx, J.es.cf, J.fast);
-        memcpy(A.h + off_jobs + sizeof(RateJobDev) * (size_t)i, &D, sizeof(D));
-    }
-    memcpy(A.h + off_tiles, tiles.data(), sizeof(RateTile) * tiles.size());
-    if (!sp.empty()) memcpy(A.h + off_sp, sp.data(), sizeof(RateSpatialDev) * sp.size());
-    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
-    int e = ccd_rate_launch(reinterpret_cast<const RateTile *>(A.dv + off_tiles), (int)tiles.size(),
-                            reinterpret_cast<const RateJobDev *>(A.dv + off_jobs), smem, ctx->d_cdf, ctx->d_scale,
-                            reinterpret_cast<double *>(A.dv + off_part), st);
-    if (e != 0) return fail(CCD_ERR_CUDA, "rate kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    if (!sp.empty()) {
-        e = ccd_rate_spatial_launch(reinterpret_cast<const RateSpatialDev *>(A.dv + off_sp), (int)sp.size(), max_pixels, st);
-        if (e != 0) return fail(CCD_ERR_CUDA, "spatial rate launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    }
-    if (int rc = download(A, off_bad, st, "rate kernel")) return rc;
-    const double *part = reinterpret_cast<const double *>(A.h + off_part);
-    for (int i = 0; i < n_jobs; i++) {
-        const std::vector<size_t> &at = tile_at[(size_t)i];  // a grid's sum: its tiles in order
-        const int n_grids = P[(size_t)i].d->n_grids;
-        for (int g = 0; g < CCD_MAX_GRIDS; g++) jobs[i].grid_bits[g] = 0.0;
-        for (int gi = 0; gi < n_grids; gi++) jobs[i].grid_bits[n_grids - 1 - gi] = ordered_sum(part + at[gi], at[gi + 1] - at[gi]);
-    }
-    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {
-        return fail(CCD_ERR_ARG, "job %d: latent %lld is outside [-64, 63]", i, (long long)jobs[i].bad_index);
-    });
+    return rate_call(
+        ctx, A, T, (size_t)n_jobs, 0, 1, "rate kernel", st,
+        [&](unsigned long long *bad, unsigned long long *) {
+            for (int i = 0; i < n_jobs; i++) {
+                PreparedJob &J = P[(size_t)i];
+                memcpy(A.h + J.off_blob, J.blob.data(), J.blob.size());
+                J.es.latents = const_cast<int8_t *>(jobs[i].d_latents);
+                J.es.blob = A.dv + J.off_blob;
+                memcpy(A.h + off_es + sizeof(EntStream) * (size_t)i, &J.es, sizeof(EntStream));
+                RateJobDev D;
+                D.es = reinterpret_cast<const EntStream *>(A.dv + off_es) + i;
+                D.bits = jobs[i].d_bits;
+                D.freq = jobs[i].d_freq;
+                D.mu_sc = jobs[i].d_mu_sc;
+                D.bad = bad + i;
+                D.kind = ccd_rate_kind(J.d->n_ctx, J.es.cf, J.fast);
+                memcpy(A.h + off_jobs + sizeof(RateJobDev) * (size_t)i, &D, sizeof(D));
+            }
+            if (!sp.empty()) memcpy(A.h + off_sp, sp.data(), sizeof(RateSpatialDev) * sp.size());
+        },
+        [&](const RateTile *tiles, int n_tiles, double *part) {
+            const int rc = launched(ccd_rate_launch(tiles, n_tiles, reinterpret_cast<const RateJobDev *>(A.dv + off_jobs),
+                                                    smem, ctx->d_cdf, ctx->d_scale, part, st),
+                                    "rate kernel");
+            if (rc || sp.empty()) return rc;
+            const RateSpatialDev *d_sp = reinterpret_cast<const RateSpatialDev *>(A.dv + off_sp);
+            return launched(ccd_rate_spatial_launch(d_sp, (int)sp.size(), max_pixels, st), "spatial rate");
+        },
+        [&](const unsigned long long *bad, const unsigned long long *, const double *part) {
+            for (int i = 0; i < n_jobs; i++)
+                for (int g = 0; g < CCD_MAX_GRIDS; g++)
+                    jobs[i].grid_bits[g] = g < P[(size_t)i].d->n_grids ? T.sum(part, i, g) : 0.0;
+            return report(jobs, n_jobs, bad, [&](int i) {
+                return fail(CCD_ERR_ARG, "job %d: latent %lld is outside [-64, 63]", i, (long long)jobs[i].bad_index);
+            });
+        });
 }
 
 int ccd_latent_rate(CcdContext *ctx, CcdRateJob *jobs, int n_jobs, void *cuda_stream) {
@@ -1821,11 +1859,8 @@ int ccd_latent_rate_edited(CcdContext *ctx, CcdRateJob *jobs, const CcdModelEdit
 }
 
 static int rate_sweep_body(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, cudaStream_t st) {
-    std::vector<RateTile> tiles;
-    std::vector<size_t> tile_at;  // tiles of job i, decode-order grid gi: [tile_at[k], tile_at[k + 1]), k = hist_at[i] + gi
-    std::vector<size_t> hist_at((size_t)n_jobs);  // first decode-order grid of job i in the histogram array
+    RateTilePlan T;  // job i's grid histograms: [128] each, from 128 * T.grid_at[i], decode order
     std::vector<SweepJobDev> D((size_t)n_jobs);
-    size_t n_hist = 0;
     for (int i = 0; i < n_jobs; i++) {
         CcdSweepJob &S = jobs[i];
         S.bad_index = -1;
@@ -1845,62 +1880,48 @@ static int rate_sweep_body(CcdContext *ctx, CcdSweepJob *jobs, int n_jobs, cudaS
         J.mu_sc = S.d_mu_sc;
         J.n_off = S.n_offsets;
         for (int k = 0; k < S.n_offsets; k++) J.off[k] = S.sc_offset[k];
-        hist_at[(size_t)i] = n_hist;
         for (int gi = 0; gi < d->n_grids; gi++) {
             const int g = d->n_grids - 1 - gi;
             J.h[gi] = d->grid_h[g];
             J.w[gi] = d->grid_w[g];
             J.lat_off[gi] = off_by_grid[g];
-            tile_at.push_back(tiles.size());
-            for (int y0 = 0; y0 < J.h[gi]; y0 += CCD_RATE_TH)
-                for (int x0 = 0; x0 < J.w[gi]; x0 += CCD_RATE_TW) tiles.push_back(RateTile{i, gi, y0, x0});
         }
-        n_hist += (size_t)d->n_grids;
+        T.add(i, d);
     }
-    tile_at.push_back(tiles.size());
-    if (tiles.size() > (size_t)INT32_MAX) return fail(CCD_ERR_UNSUPPORTED, "too many rate tiles");
+    if (int rc = T.check()) return rc;
     Arena A;
     const size_t off_jobs = A.take(sizeof(SweepJobDev) * (size_t)n_jobs);
-    const size_t off_tiles = A.take(sizeof(RateTile) * tiles.size());
-    // results: the bad words (~0) and the histograms (0) on the way up, then the partials, which are not uploaded
-    const size_t off_bad = A.take(sizeof(unsigned long long) * (size_t)n_jobs);
-    const size_t off_hist = A.take(sizeof(unsigned long long) * 128 * n_hist);
-    const size_t off_part = A.take(sizeof(double) * CCD_SWEEP_MAX_OFFSETS * tiles.size());
-    if (int rc = stage(ctx, A)) return rc;
-    for (int i = 0; i < n_jobs; i++) {
-        D[(size_t)i].bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad) + i;
-        D[(size_t)i].hist = reinterpret_cast<unsigned long long *>(A.dv + off_hist) + 128 * hist_at[(size_t)i];
-    }
-    memcpy(A.h + off_jobs, D.data(), sizeof(SweepJobDev) * (size_t)n_jobs);
-    memcpy(A.h + off_tiles, tiles.data(), sizeof(RateTile) * tiles.size());
-    memset(A.h + off_bad, 0xff, sizeof(unsigned long long) * (size_t)n_jobs);
-    memset(A.h + off_hist, 0, sizeof(unsigned long long) * 128 * n_hist);
-    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
-    int e = ccd_rate_sweep_launch(reinterpret_cast<const RateTile *>(A.dv + off_tiles), (int)tiles.size(),
-                                  reinterpret_cast<const SweepJobDev *>(A.dv + off_jobs), ctx->d_cdf, ctx->d_scale,
-                                  reinterpret_cast<double *>(A.dv + off_part), st);
-    if (e != 0) return fail(CCD_ERR_CUDA, "sweep kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    if (int rc = download(A, off_bad, st, "sweep kernel")) return rc;
-    const double *part = reinterpret_cast<const double *>(A.h + off_part);
-    const unsigned long long *hist = reinterpret_cast<const unsigned long long *>(A.h + off_hist);
-    for (int i = 0; i < n_jobs; i++) {
-        CcdSweepJob &S = jobs[i];
-        const int n_grids = S.desc->n_grids;
-        memset(S.bits, 0, sizeof(S.bits));
-        memset(S.hist, 0, sizeof(S.hist));
-        for (int gi = 0; gi < n_grids; gi++) {
-            const int g = n_grids - 1 - gi;
-            const size_t k0 = hist_at[(size_t)i] + (size_t)gi;  // a grid's sum: its tiles in order
-            for (int k = 0; k < S.n_offsets; k++)
-                S.bits[g][k] = ordered_sum(part + CCD_SWEEP_MAX_OFFSETS * tile_at[k0] + k, tile_at[k0 + 1] - tile_at[k0],
-                                           CCD_SWEEP_MAX_OFFSETS);
-            for (int s = 0; s < 128; s++) S.hist[g][s] = hist[128 * k0 + s];
-        }
-    }
-    return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {
-        return fail(CCD_ERR_ARG, "job %d: symbol %lld has a latent outside [-64, 63] or a (mu_idx, sc_idx) outside its table",
-                    i, (long long)jobs[i].bad_index);
-    });
+    return rate_call(
+        ctx, A, T, (size_t)n_jobs, 128 * T.grid_at.back(), CCD_SWEEP_MAX_OFFSETS, "sweep kernel", st,
+        [&](unsigned long long *bad, unsigned long long *hist) {
+            for (int i = 0; i < n_jobs; i++) {
+                D[(size_t)i].bad = bad + i;
+                D[(size_t)i].hist = hist + 128 * T.grid_at[(size_t)i];
+            }
+            memcpy(A.h + off_jobs, D.data(), sizeof(SweepJobDev) * (size_t)n_jobs);
+        },
+        [&](const RateTile *tiles, int n_tiles, double *part) {
+            return launched(ccd_rate_sweep_launch(tiles, n_tiles, reinterpret_cast<const SweepJobDev *>(A.dv + off_jobs),
+                                                  ctx->d_cdf, ctx->d_scale, part, st),
+                            "sweep kernel");
+        },
+        [&](const unsigned long long *bad, const unsigned long long *hist, const double *part) {
+            for (int i = 0; i < n_jobs; i++) {
+                CcdSweepJob &S = jobs[i];
+                const int n_grids = S.desc->n_grids;
+                memset(S.bits, 0, sizeof(S.bits));
+                memset(S.hist, 0, sizeof(S.hist));
+                for (int g = 0; g < n_grids; g++) {
+                    for (int k = 0; k < S.n_offsets; k++) S.bits[g][k] = T.sum(part, i, g, k, CCD_SWEEP_MAX_OFFSETS);
+                    const size_t k0 = T.grid_at[(size_t)i] + (size_t)(n_grids - 1 - g);
+                    for (int s = 0; s < 128; s++) S.hist[g][s] = hist[128 * k0 + s];
+                }
+            }
+            return report(jobs, n_jobs, bad, [&](int i) {
+                return fail(CCD_ERR_ARG, "job %d: symbol %lld has a latent outside [-64, 63] or a (mu_idx, sc_idx) outside its table",
+                            i, (long long)jobs[i].bad_index);
+            });
+        });
 }
 
 // One candidate of ccd_rate_candidates as the kernel prices it: which fixed-point weight or bias moves, by how much
@@ -1999,17 +2020,9 @@ static int rate_candidates_body(CcdContext *ctx, const CcdCoolChicDesc *desc, co
             if (fast_out) fast_out[j + 1] = fast ? 1 : 0;
         }
     }
-    const int n_grids = desc->n_grids;
-    std::vector<RateTile> tiles;
-    std::vector<size_t> tile_at;  // tiles of decode-order grid gi: [tile_at[gi], tile_at[gi + 1])
-    for (int gi = 0; gi < n_grids; gi++) {
-        const EntGrid &G = J.es.grid[gi];
-        tile_at.push_back(tiles.size());
-        for (int y0 = 0; y0 < G.h; y0 += CCD_RATE_TH)
-            for (int x0 = 0; x0 < G.w; x0 += CCD_RATE_TW) tiles.push_back(RateTile{0, gi, y0, x0});
-    }
-    tile_at.push_back(tiles.size());
-    if (tiles.size() > (size_t)INT32_MAX) return fail(CCD_ERR_UNSUPPORTED, "too many rate tiles");
+    RateTilePlan T;
+    T.add(0, desc);
+    if (int rc = T.check()) return rc;
     const size_t smem = ccd_rate_candidates_smem_bytes(J.es.arm_blob_bytes, J.es.ifce_blob_max, nk);
     if (smem > CCD_SMEM_MAX)
         return fail(CCD_ERR_UNSUPPORTED, "candidate pricing needs %zu bytes of shared memory, %d are available", smem,
@@ -2019,40 +2032,33 @@ static int rate_candidates_body(CcdContext *ctx, const CcdCoolChicDesc *desc, co
     const size_t off_es = A.take(sizeof(EntStream));
     const size_t off_job = A.take(sizeof(CandJobDev));
     const size_t off_cand = A.take(sizeof(CandDev) * (size_t)nk);
-    const size_t off_tiles = A.take(sizeof(RateTile) * tiles.size());
-    // results: the bad word (~0 before the launch), then the partials, which are not uploaded
-    const size_t off_bad = A.take(sizeof(unsigned long long));
-    const size_t off_part = A.take(sizeof(double) * tiles.size() * (size_t)nk);
-    if (int rc = stage(ctx, A)) return rc;
-    memcpy(A.h + J.off_blob, J.blob.data(), J.blob.size());
-    J.es.latents = const_cast<int8_t *>(d_latents);
-    J.es.blob = A.dv + J.off_blob;
-    memcpy(A.h + off_es, &J.es, sizeof(EntStream));
-    CandJobDev D;
-    memset(&D, 0, sizeof(D));
-    D.es = reinterpret_cast<const EntStream *>(A.dv + off_es);
-    D.bad = reinterpret_cast<unsigned long long *>(A.dv + off_bad);
-    D.n_cand = nk;
-    memcpy(A.h + off_job, &D, sizeof(D));
-    memcpy(A.h + off_cand, C.data(), sizeof(CandDev) * (size_t)nk);
-    memcpy(A.h + off_tiles, tiles.data(), sizeof(RateTile) * tiles.size());
-    memset(A.h + off_bad, 0xff, sizeof(unsigned long long));
-    CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_part, cudaMemcpyHostToDevice, st));
-    const bool wide = L.dim > 32 || desc->arm_hidden > 3;
-    int e = ccd_rate_candidates_launch(reinterpret_cast<const RateTile *>(A.dv + off_tiles), (int)tiles.size(),
-                                       reinterpret_cast<const CandJobDev *>(A.dv + off_job),
-                                       reinterpret_cast<const CandDev *>(A.dv + off_cand), wide, smem, ctx->d_cdf,
-                                       ctx->d_scale, reinterpret_cast<double *>(A.dv + off_part), st);
-    if (e != 0) return fail(CCD_ERR_CUDA, "candidate kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
-    if (int rc = download(A, off_bad, st, "candidate kernel")) return rc;
-    const double *part = reinterpret_cast<const double *>(A.h + off_part);
-    for (int c = 0; c < nk; c++)
-        for (int gi = 0; gi < n_grids; gi++)  // a grid's sum: its tiles in order
-            bits_out[(size_t)c * n_grids + (n_grids - 1 - gi)] =
-                ordered_sum(part + tile_at[gi] * (size_t)nk + c, tile_at[gi + 1] - tile_at[gi], (size_t)nk);
-    const unsigned long long bad = *reinterpret_cast<const unsigned long long *>(A.h + off_bad);
-    if (bad != ~0ull) return fail(CCD_ERR_ARG, "latent %lld is outside [-64, 63]", (long long)bad);
-    return CCD_OK;
+    return rate_call(
+        ctx, A, T, 1, 0, (size_t)nk, "candidate kernel", st,
+        [&](unsigned long long *bad, unsigned long long *) {
+            memcpy(A.h + J.off_blob, J.blob.data(), J.blob.size());
+            J.es.latents = const_cast<int8_t *>(d_latents);
+            J.es.blob = A.dv + J.off_blob;
+            memcpy(A.h + off_es, &J.es, sizeof(EntStream));
+            CandJobDev D;
+            memset(&D, 0, sizeof(D));
+            D.es = reinterpret_cast<const EntStream *>(A.dv + off_es);
+            D.bad = bad;
+            D.n_cand = nk;
+            memcpy(A.h + off_job, &D, sizeof(D));
+            memcpy(A.h + off_cand, C.data(), sizeof(CandDev) * (size_t)nk);
+        },
+        [&](const RateTile *tiles, int n_tiles, double *part) {
+            const bool wide = L.dim > 32 || desc->arm_hidden > 3;
+            return launched(ccd_rate_candidates_launch(tiles, n_tiles, reinterpret_cast<const CandJobDev *>(A.dv + off_job),
+                                                       reinterpret_cast<const CandDev *>(A.dv + off_cand), wide, smem,
+                                                       ctx->d_cdf, ctx->d_scale, part, st),
+                            "candidate kernel");
+        },
+        [&](const unsigned long long *bad, const unsigned long long *, const double *part) {
+            for (int c = 0; c < nk; c++)
+                for (int g = 0; g < desc->n_grids; g++) bits_out[(size_t)c * desc->n_grids + g] = T.sum(part, 0, g, c, nk);
+            return *bad == ~0ull ? (int)CCD_OK : fail(CCD_ERR_ARG, "latent %lld is outside [-64, 63]", (long long)*bad);
+        });
 }
 
 int ccd_rate_candidates(CcdContext *ctx, const CcdCoolChicDesc *desc, const int64_t *nn_ints, const int8_t *d_latents,
@@ -2180,8 +2186,7 @@ int frame_pair_call(CcdContext *ctx, Job *jobs, int n_jobs, const char *what, si
         memcpy(A.h + off_jobs + sizeof(Dev) * (size_t)i, &D, sizeof(D));
     }
     CUDA_TRY(cudaMemcpyAsync(A.dv, A.h, off_res + res_up, cudaMemcpyHostToDevice, st));
-    if (int e = launch(reinterpret_cast<const Dev *>(A.dv + off_jobs)))
-        return fail(CCD_ERR_CUDA, "%s launch failed: %s", what, cudaGetErrorString((cudaError_t)e));
+    if (int rc = launched(launch(reinterpret_cast<const Dev *>(A.dv + off_jobs)), what)) return rc;
     if (int rc = download(A, off_bad, st, what)) return rc;
     read(A.h + off_res);
     return report(jobs, n_jobs, reinterpret_cast<const unsigned long long *>(A.h + off_bad), [&](int i) {

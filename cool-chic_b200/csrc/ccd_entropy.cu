@@ -1515,10 +1515,16 @@ __global__ void __launch_bounds__(CCD_ENT_THREADS, 1)
     }
 }
 
-template <int NCTX, int CF, bool FAST>
+// The ARM shapes (n_ctx, cf) with a fast (DmmaArm) kernel, then the generic kernel's (0, 0).  A shape's index is its
+// kind (ccd_rate_kind); k_entropy and k_latent_rate take a kind's shape as template constants, so their dispatch is a
+// switch with a case per kind.
+constexpr int kArmShapes[][2] = {{6, 2}, {10, 2}, {10, 4}, {14, 6}, {20, 6}, {0, 0}};
+constexpr int kGenericKind = 5;
+
+template <int K>
 int launch_t(const EntStream *d_streams, int n, size_t smem, int threads, const uint32_t *cdf, const float *scale,
              cudaStream_t st) {
-    auto kern = k_entropy<NCTX, CF, FAST>;
+    auto kern = k_entropy<kArmShapes[K][0], kArmShapes[K][1], K != kGenericKind>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
@@ -1554,74 +1560,120 @@ __device__ __forceinline__ uint32_t coder_freq(int sym, int mu_idx, int sc_idx, 
     return l1 - l0;
 }
 
-// One symbol: clamp (latent.py:165, rangecoder.py:89-91), then the coder's interval.  Returns the f64 bits.
+// (mu_idx, sc_idx): the table indices of the ARM's outputs (o0, o1), clamped (latent.py:165, rangecoder.py:89-91)
+__device__ __forceinline__ int2 mu_sc_index(long long o0, long long o1) {
+    const long long im = o0 + 16384, is = o1 + 1280;
+    return make_int2((int)(im < 0 ? 0 : (im > 32767 ? 32767 : im)), (int)(is < 0 ? 0 : (is > 2560 ? 2560 : is)));
+}
+
+// A symbol outside [-64, 63] has no interval: its decode-order index goes to *bad (the smallest one stays)
+__device__ __forceinline__ bool bad_symbol(int sym, long long idx, unsigned long long *bad) {
+    if (sym >= kSymMin && sym <= kSymMax) return false;
+    atomicMin(bad, (unsigned long long)idx);
+    return true;
+}
+
+// One symbol: clamp, then the coder's interval.  Returns the f64 bits.
 __device__ __forceinline__ double rate_symbol(long long o0, long long o1, int sym, long long idx, const RateJobDev &J,
                                               const uint32_t *__restrict__ cdf, const float *__restrict__ scale_tab) {
-    long long im = o0 + 16384, is = o1 + 1280;
-    im = im < 0 ? 0 : (im > 32767 ? 32767 : im);
-    is = is < 0 ? 0 : (is > 2560 ? 2560 : is);
-    const int mu_idx = (int)im, sc_idx = (int)is;
-    if (sym < kSymMin || sym > kSymMax) {
-        atomicMin(J.bad, (unsigned long long)idx);
-        return 0.0;
-    }
-    const uint32_t freq = coder_freq(sym, mu_idx, sc_idx, cdf, scale_tab);
+    const int2 m = mu_sc_index(o0, o1);
+    if (bad_symbol(sym, idx, J.bad)) return 0.0;
+    const uint32_t freq = coder_freq(sym, m.x, m.y, cdf, scale_tab);
     const double bits = 24.0 - log2((double)freq);
     J.bits[idx] = (float)bits;
     if (J.freq) J.freq[idx] = freq;
-    if (J.mu_sc) J.mu_sc[idx] = (uint32_t)mu_idx | ((uint32_t)sc_idx << 16);
+    if (J.mu_sc) J.mu_sc[idx] = (uint32_t)m.x | ((uint32_t)m.y << 16);
     return bits;
 }
 
-// One tile: rows y0-4 .. y0+nr-1 and columns x0-4 .. x0+59 of the grid are staged in the 32 x 64 row ring (the
-// causal neighbourhood is dy -4..0, dx -4..4), then every symbol of the tile is evaluated.  FAST: a quad of lanes
-// per symbol (64 symbols per pass of the CTA), GENERIC: a thread per symbol.
-template <int NCTX, int CF, bool FAST>
+// A tile in shared memory: the grid's descriptor, the ARM blob, the grid's IFCE blob, then the 32 x 64 row ring
+// (rows: its shared-space address) with rows y0-4 .. y0+nr-1 and columns x0-4 .. x0+59 of the grid (the causal
+// neighbourhood is dy -4..0, dx -4..4).
+struct RateStage {
+    const EntGrid *g;
+    const unsigned char *arm, *ifce;
+    unsigned char *ring;
+    uint32_t rows;
+    int nr, nc;
+};
+
+// Stages tile t of stream G at smem, all threads of the CTA; the caller synchronises before reading it
+__device__ __forceinline__ RateStage stage_rate_tile(const RateTile &t, const EntStream &G, unsigned char *smem) {
+    const EntGrid &Gg = G.grid[t.grid];
+    const int tid = threadIdx.x, w = Gg.w;
+    const long long base = Gg.lat_off;
+    EntGrid *g = reinterpret_cast<EntGrid *>(smem);
+    unsigned char *arm = smem + align16(sizeof(EntGrid));
+    unsigned char *ifce = arm + align16((size_t)G.arm_blob_bytes);
+    unsigned char *ring = ifce + align16((size_t)G.ifce_blob_max);
+    const uint32_t rows = (uint32_t)__cvta_generic_to_shared(ring);
+    const uint32_t *src = reinterpret_cast<const uint32_t *>(&Gg);
+    uint32_t *dst = reinterpret_cast<uint32_t *>(g);
+    for (int i = tid; i < (int)(sizeof(EntGrid) / 4); i += CCD_RATE_THREADS) dst[i] = src[i];
+    for (int i = tid * 4; i < G.arm_blob_bytes; i += CCD_RATE_THREADS * 4)
+        *reinterpret_cast<uint32_t *>(arm + i) = *reinterpret_cast<const uint32_t *>(G.blob + i);
+    for (int i = tid * 4; i < Gg.ifce_blob_bytes; i += CCD_RATE_THREADS * 4)
+        *reinterpret_cast<uint32_t *>(ifce + i) = *reinterpret_cast<const uint32_t *>(G.blob + Gg.ifce_blob_off + i);
+    const int nr = min(CCD_RATE_TH, Gg.h - t.y0), nc = min(CCD_RATE_TW, w - t.x0);
+    for (int i = tid; i < (nr + 4) * CCD_ROW_COLS; i += CCD_RATE_THREADS) {
+        const int yy = t.y0 - 4 + (i >> 6), xx = t.x0 - 4 + (i & (CCD_ROW_COLS - 1));
+        int v = 0;
+        if (yy >= 0 && xx >= 0 && xx < w) v = G.latents[base + (long long)yy * w + xx];
+        sts_u8(rows + ((((uint32_t)yy & (CCD_RATE_ROWS - 1)) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))), v);
+    }
+    return RateStage{g, arm, ifce, ring, rows, nr, nc};
+}
+
+// The sum of a over the warp by butterfly: every lane gets the same sum on every run
+__device__ __forceinline__ double warp_sum(double a) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
+    return a;
+}
+
+// Fixed-order sum of one double per thread of the CTA: warp_sum, then the warps in order -- the same sum on every
+// run.  Every thread calls it; thread 0 gets the sum.
+__device__ __forceinline__ double block_sum(double a) {
+    __shared__ double wsum[CCD_RATE_THREADS / 32];
+    a = warp_sum(a);
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = a;
+    __syncthreads();
+    double s = 0.0;
+    if (threadIdx.x == 0)
+        for (int i = 0; i < CCD_RATE_THREADS / 32; i++) s += wsum[i];
+    return s;
+}
+
+// One tile: staged, then every symbol of the tile is evaluated.  A fast kind: a quad of lanes per symbol (64 symbols
+// per pass of the CTA), the generic one: a thread per symbol.
+template <int K>
 __device__ __forceinline__ void rate_tile(const RateTile &t, const RateJobDev &J, unsigned char *smem,
                                           const uint32_t *__restrict__ cdf, const float *__restrict__ scale_tab,
                                           double *__restrict__ part) {
     const EntStream &G = *J.es;
     const EntGrid &Gg = G.grid[t.grid];
-    const int tid = threadIdx.x, nthr = blockDim.x;
-    EntGrid *g = reinterpret_cast<EntGrid *>(smem);
-    unsigned char *arm = smem + align16(sizeof(EntGrid));
-    unsigned char *ifce = arm + align16((size_t)G.arm_blob_bytes);
-    const uint32_t rows = (uint32_t)__cvta_generic_to_shared(ifce + align16((size_t)G.ifce_blob_max));
     const int8_t *lat = G.latents;
-    const int h = Gg.h, w = Gg.w, n_hidden = G.n_hidden;
+    const int tid = threadIdx.x, w = Gg.w, n_hidden = G.n_hidden;
     const long long base = Gg.lat_off;
-    {
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(&Gg);
-        uint32_t *dst = reinterpret_cast<uint32_t *>(g);
-        for (int i = tid; i < (int)(sizeof(EntGrid) / 4); i += nthr) dst[i] = src[i];
-        for (int i = tid * 4; i < G.arm_blob_bytes; i += nthr * 4)
-            *reinterpret_cast<uint32_t *>(arm + i) = *reinterpret_cast<const uint32_t *>(G.blob + i);
-        for (int i = tid * 4; i < Gg.ifce_blob_bytes; i += nthr * 4)
-            *reinterpret_cast<uint32_t *>(ifce + i) = *reinterpret_cast<const uint32_t *>(G.blob + Gg.ifce_blob_off + i);
-    }
-    const int nr = min(CCD_RATE_TH, h - t.y0), nc = min(CCD_RATE_TW, w - t.x0);
-    for (int i = tid; i < (nr + 4) * CCD_ROW_COLS; i += nthr) {
-        const int yy = t.y0 - 4 + (i >> 6), xx = t.x0 - 4 + (i & (CCD_ROW_COLS - 1));
-        int v = 0;
-        if (yy >= 0 && xx >= 0 && xx < w) v = lat[base + (long long)yy * w + xx];
-        sts_u8(rows + ((((uint32_t)yy & (CCD_RATE_ROWS - 1)) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))), v);
-    }
+    const RateStage T = stage_rate_tile(t, G, smem);
     __syncthreads();
-    const uint32_t row_mask = CCD_RATE_ROWS - 1;
-    const int n = nr * nc;
+    const EntGrid *g = T.g;
+    const uint32_t rows = T.rows, row_mask = CCD_RATE_ROWS - 1;
+    const int nc = T.nc, n = T.nr * nc;
     double acc = 0.0;
-    if constexpr (FAST) {
+    if constexpr (K != kGenericKind) {
+        using Arm = DmmaArm<kArmShapes[K][0], kArmShapes[K][1]>;
         const int member = tid & 3;
-        for (int s0 = 0; s0 < n; s0 += nthr >> 2) {
+        for (int s0 = 0; s0 < n; s0 += CCD_RATE_THREADS >> 2) {
             // uniform trip count: every lane of a warp takes part in the DMMAs and quad shuffles
             const int s = s0 + (tid >> 2);
             const bool valid = s < n;
             const int ty = valid ? s / nc : 0, tx = valid ? s - ty * nc : 0;
             const int y = t.y0 + ty, x = t.x0 + tx;
             int ifv[CCD_IFCE_FAST_MAX];
-            DmmaArm<NCTX, CF>::ifce_prefetch(g, lat, y, x, member, ifv);
+            Arm::ifce_prefetch(g, lat, y, x, member, ifv);
             long long o0, o1;
-            DmmaArm<NCTX, CF>::run(g, arm, ifce, ifv, rows, row_mask, n_hidden, y, x, member, o0, o1);
+            Arm::run(g, T.arm, T.ifce, ifv, rows, row_mask, n_hidden, y, x, member, o0, o1);
             if (valid && member == 0) {
                 const int sym = lds_s8(rows + (((uint32_t)y & row_mask) << 6 | ((uint32_t)x & (CCD_ROW_COLS - 1))));
                 acc += rate_symbol(o0, o1, sym, base + (long long)y * w + x, J, cdf, scale_tab);
@@ -1629,7 +1681,7 @@ __device__ __forceinline__ void rate_tile(const RateTile &t, const RateJobDev &J
         }
     } else {
         const int n_ctx = G.n_ctx, cf = G.cf;
-        for (int s = tid; s < n; s += nthr) {
+        for (int s = tid; s < n; s += CCD_RATE_THREADS) {
             const int ty = s / nc, tx = s - ty * nc;
             const int y = t.y0 + ty, x = t.x0 + tx;
             long long xin[CCD_MAX_DIM];
@@ -1640,24 +1692,15 @@ __device__ __forceinline__ void rate_tile(const RateTile &t, const RateJobDev &J
                     v = lds_s8(rows + ((((uint32_t)yy & row_mask) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))));
                 xin[c] = v;
             }
-            if (cf > 0) GenericArm::ifce(g, ifce, lat, cf, y >> 1, x >> 1, xin + n_ctx);
+            if (cf > 0) GenericArm::ifce(g, T.ifce, lat, cf, y >> 1, x >> 1, xin + n_ctx);
             long long o0, o1;
-            GenericArm::arm(arm, n_ctx + cf, n_hidden, xin, o0, o1);
+            GenericArm::arm(T.arm, n_ctx + cf, n_hidden, xin, o0, o1);
             const int sym = lds_s8(rows + (((uint32_t)y & row_mask) << 6 | ((uint32_t)x & (CCD_ROW_COLS - 1))));
             acc += rate_symbol(o0, o1, sym, base + (long long)y * w + x, J, cdf, scale_tab);
         }
     }
-    // fixed-order reduction: lanes (butterfly), then the warps in order -- the same sum on every run
-    __shared__ double wsum[CCD_RATE_THREADS / 32];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
-    if ((tid & 31) == 0) wsum[tid >> 5] = acc;
-    __syncthreads();
-    if (tid == 0) {
-        double s = 0.0;
-        for (int i = 0; i < (nthr >> 5); i++) s += wsum[i];
-        part[blockIdx.x] = s;
-    }
+    const double sum = block_sum(acc);
+    if (tid == 0) part[blockIdx.x] = sum;
 }
 
 // ONE launch for every grid of every job; the ARM variant is chosen per CTA (uniform branch).
@@ -1668,12 +1711,12 @@ __global__ void __launch_bounds__(CCD_RATE_THREADS)
     const RateTile t = tiles[blockIdx.x];
     const RateJobDev &J = jobs[t.job];
     switch (J.kind) {
-        case 0: rate_tile<6, 2, true>(t, J, smem_raw, cdf, scale_tab, part); break;
-        case 1: rate_tile<10, 2, true>(t, J, smem_raw, cdf, scale_tab, part); break;
-        case 2: rate_tile<10, 4, true>(t, J, smem_raw, cdf, scale_tab, part); break;
-        case 3: rate_tile<14, 6, true>(t, J, smem_raw, cdf, scale_tab, part); break;
-        case 4: rate_tile<20, 6, true>(t, J, smem_raw, cdf, scale_tab, part); break;
-        default: rate_tile<0, 0, false>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 0: rate_tile<0>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 1: rate_tile<1>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 2: rate_tile<2>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 3: rate_tile<3>(t, J, smem_raw, cdf, scale_tab, part); break;
+        case 4: rate_tile<4>(t, J, smem_raw, cdf, scale_tab, part); break;
+        default: rate_tile<kGenericKind>(t, J, smem_raw, cdf, scale_tab, part); break;
     }
 }
 
@@ -1724,8 +1767,7 @@ __global__ void __launch_bounds__(CCD_RATE_THREADS)
             s2 = s2 < 0 ? 0 : (s2 > 2560 ? 2560 : s2);
             acc += 24.0 - log2((double)coder_freq(sym[j], (int)(ms[j] & 0xFFFFu), s2, cdf, scale_tab));
         }
-#pragma unroll
-        for (int m = 16; m > 0; m >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, m);
+        acc = warp_sum(acc);
         if ((tid & 31) == 0) wsum[k][tid >> 5] = acc;
     }
     __syncthreads();
@@ -1846,56 +1888,34 @@ __global__ void __launch_bounds__(CCD_RATE_THREADS)
                       const CandDev *__restrict__ cand_g, const uint32_t *__restrict__ cdf,
                       const float *__restrict__ scale_tab, double *__restrict__ part) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    __shared__ double wsum[CCD_RATE_THREADS / 32];
     const RateTile t = tiles[blockIdx.x];
     const CandJobDev &J = *job;
     const EntStream &G = *J.es;
-    const EntGrid &Gg = G.grid[t.grid];
     const int tid = threadIdx.x;
     const int nk = J.n_cand;
-    EntGrid *g = reinterpret_cast<EntGrid *>(smem_raw);
-    unsigned char *arm = smem_raw + align16(sizeof(EntGrid));
-    unsigned char *ifce = arm + align16((size_t)G.arm_blob_bytes);
-    unsigned char *rows_p = ifce + align16((size_t)G.ifce_blob_max);
-    CandDev *cand = reinterpret_cast<CandDev *>(rows_p + CCD_RATE_ROWS * CCD_ROW_COLS);
+    const RateStage T = stage_rate_tile(t, G, smem_raw);
+    CandDev *cand = reinterpret_cast<CandDev *>(T.ring + CCD_RATE_ROWS * CCD_ROW_COLS);
     uint32_t *fq = reinterpret_cast<uint32_t *>(cand + nk);  // [nk][CCD_RATE_THREADS]
     double *red = reinterpret_cast<double *>(fq + (size_t)nk * CCD_RATE_THREADS);
-    const uint32_t rows = (uint32_t)__cvta_generic_to_shared(rows_p);
-    const int8_t *lat = G.latents;
-    const int h = Gg.h, w = Gg.w;
-    const long long base = Gg.lat_off;
-    {
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(&Gg);
-        uint32_t *dst = reinterpret_cast<uint32_t *>(g);
-        for (int i = tid; i < (int)(sizeof(EntGrid) / 4); i += CCD_RATE_THREADS) dst[i] = src[i];
-        for (int i = tid * 4; i < G.arm_blob_bytes; i += CCD_RATE_THREADS * 4)
-            *reinterpret_cast<uint32_t *>(arm + i) = *reinterpret_cast<const uint32_t *>(G.blob + i);
-        for (int i = tid * 4; i < Gg.ifce_blob_bytes; i += CCD_RATE_THREADS * 4)
-            *reinterpret_cast<uint32_t *>(ifce + i) = *reinterpret_cast<const uint32_t *>(G.blob + Gg.ifce_blob_off + i);
-        for (int i = tid; i < nk; i += CCD_RATE_THREADS) cand[i] = cand_g[i];
-    }
-    const int nr = min(CCD_RATE_TH, h - t.y0), nc = min(CCD_RATE_TW, w - t.x0);
-    for (int i = tid; i < (nr + 4) * CCD_ROW_COLS; i += CCD_RATE_THREADS) {
-        const int yy = t.y0 - 4 + (i >> 6), xx = t.x0 - 4 + (i & (CCD_ROW_COLS - 1));
-        int v = 0;
-        if (yy >= 0 && xx >= 0 && xx < w) v = lat[base + (long long)yy * w + xx];
-        sts_u8(rows + ((((uint32_t)yy & (CCD_RATE_ROWS - 1)) << 6) | ((uint32_t)xx & (CCD_ROW_COLS - 1))), v);
-    }
+    for (int i = tid; i < nk; i += CCD_RATE_THREADS) cand[i] = cand_g[i];
     __syncthreads();
-    const uint32_t row_mask = CCD_RATE_ROWS - 1;
-    const int n = nr * nc;
+    const EntGrid *g = T.g;
+    const uint32_t rows = T.rows, row_mask = CCD_RATE_ROWS - 1;
+    const int8_t *lat = G.latents;
+    const int w = G.grid[t.grid].w, nc = T.nc, n = T.nr * nc;
+    const long long base = G.grid[t.grid].lat_off;
     const int n_ctx = G.n_ctx, cf = G.cf, nh = G.n_hidden, dim = n_ctx + cf;
     const int n_in = g->ifce_in;
     CandEval<MAXD, MAXH> E;
     E.dim = dim;
     E.nh = nh;
-    E.Wh = reinterpret_cast<const long long *>(arm);
+    E.Wh = reinterpret_cast<const long long *>(T.arm);
     E.Wl = E.Wh + (size_t)nh * dim * dim;
     E.Ws = E.Wl + (size_t)dim * 2;
     E.Bh = E.Ws + (size_t)dim * 2;
     const long long *Bl = E.Bh + (size_t)nh * dim;
     const long long *Bs = Bl + 2;
-    const long long *IW = reinterpret_cast<const long long *>(ifce);
+    const long long *IW = reinterpret_cast<const long long *>(T.ifce);
     const long long *IB = IW + (size_t)n_in * cf;
     long long IA[31];  // IFCE pre-rounding sums
     int IV[31];        // IFCE inputs
@@ -1928,13 +1948,10 @@ __global__ void __launch_bounds__(CCD_RATE_THREADS)
             }
             E.base(Bl, Bs);
             const int sym = lds_s8(rows + (((uint32_t)y & row_mask) << 6 | ((uint32_t)x & (CCD_ROW_COLS - 1))));
-            const bool bad = sym < kSymMin || sym > kSymMax;
-            if (bad) atomicMin(J.bad, (unsigned long long)(base + (long long)y * w + x));
-            auto clamp_mu = [](long long o0) { long long v = o0 + 16384; return (int)(v < 0 ? 0 : (v > 32767 ? 32767 : v)); };
-            auto clamp_sc = [](long long o1) { long long v = o1 + 1280; return (int)(v < 0 ? 0 : (v > 2560 ? 2560 : v)); };
-            const int mu = clamp_mu((E.a0 + E.s0) >> 24), sc = clamp_sc((E.a1 + E.s1) >> 24);
+            const bool bad = bad_symbol(sym, base + (long long)y * w + x, J.bad);
+            const int2 m = mu_sc_index((E.a0 + E.s0) >> 24, (E.a1 + E.s1) >> 24);
             // a bad symbol adds 0 bits, as in the rate kernel
-            const uint32_t f0 = bad ? (1u << 24) : coder_freq(sym, mu, sc, cdf, scale_tab);
+            const uint32_t f0 = bad ? (1u << 24) : coder_freq(sym, m.x, m.y, cdf, scale_tab);
             fq[tid] = f0;
             for (int k = 1; k < nk; k++) {
                 const CandDev c = cand[k];
@@ -1963,9 +1980,8 @@ __global__ void __launch_bounds__(CCD_RATE_THREADS)
                 }
                 uint32_t f = f0;
                 if (!bad && (r0 | r1 | q0 | q1) != 0) {
-                    const int mu2 = clamp_mu((E.a0 + r0 + E.s0 + q0) >> 24);
-                    const int sc2 = clamp_sc((E.a1 + r1 + E.s1 + q1) >> 24);
-                    if (mu2 != mu || sc2 != sc) f = coder_freq(sym, mu2, sc2, cdf, scale_tab);
+                    const int2 m2 = mu_sc_index((E.a0 + r0 + E.s0 + q0) >> 24, (E.a1 + r1 + E.s1 + q1) >> 24);
+                    if (m2.x != m.x || m2.y != m.y) f = coder_freq(sym, m2.x, m2.y, cdf, scale_tab);
                 }
                 fq[k * CCD_RATE_THREADS + tid] = f;
             }
@@ -1990,16 +2006,8 @@ __global__ void __launch_bounds__(CCD_RATE_THREADS)
         if (!quad) red[tid] = acc[k];
         else if ((k & 3) == (tid >> 6)) red[tid & 63] = acc[k];
         __syncthreads();
-        double a = quad ? ((tid & 3) == 0 ? red[tid >> 2] : 0.0) : red[tid];
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
-        if ((tid & 31) == 0) wsum[tid >> 5] = a;
-        __syncthreads();
-        if (tid == 0) {
-            double sum = 0.0;
-            for (int i = 0; i < CCD_RATE_THREADS / 32; i++) sum += wsum[i];
-            part[(size_t)blockIdx.x * nk + k] = sum;
-        }
+        const double sum = block_sum(quad ? ((tid & 3) == 0 ? red[tid >> 2] : 0.0) : red[tid]);
+        if (tid == 0) part[(size_t)blockIdx.x * nk + k] = sum;
     }
 }
 
@@ -2014,21 +2022,18 @@ size_t ccd_entropy_smem_bytes(int ring, int rows, int arm_blob_bytes, int ifce_b
     return p;
 }
 
-bool ccd_entropy_has_fast(int n_ctx, int cf) {
-    return (n_ctx == 6 && cf == 2) || (n_ctx == 10 && cf == 2) || (n_ctx == 10 && cf == 4) ||
-           (n_ctx == 14 && cf == 6) || (n_ctx == 20 && cf == 6);
-}
+bool ccd_entropy_has_fast(int n_ctx, int cf) { return ccd_rate_kind(n_ctx, cf, true) != kGenericKind; }
 
 int ccd_entropy_launch(const EntStream *d_streams, int n_streams, const EntLaunchCfg &cfg,
                        const uint32_t *d_cdf, const float *d_scale, cudaStream_t st) {
-    if (cfg.fast) {
-        if (cfg.n_ctx == 6 && cfg.cf == 2) return launch_t<6, 2, true>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
-        if (cfg.n_ctx == 10 && cfg.cf == 2) return launch_t<10, 2, true>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
-        if (cfg.n_ctx == 10 && cfg.cf == 4) return launch_t<10, 4, true>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
-        if (cfg.n_ctx == 14 && cfg.cf == 6) return launch_t<14, 6, true>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
-        if (cfg.n_ctx == 20 && cfg.cf == 6) return launch_t<20, 6, true>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
+    switch (ccd_rate_kind(cfg.n_ctx, cfg.cf, cfg.fast)) {
+        case 0: return launch_t<0>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
+        case 1: return launch_t<1>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
+        case 2: return launch_t<2>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
+        case 3: return launch_t<3>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
+        case 4: return launch_t<4>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
+        default: return launch_t<kGenericKind>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
     }
-    return launch_t<0, 0, false>(d_streams, n_streams, cfg.smem_bytes, cfg.threads, d_cdf, d_scale, st);
 }
 
 int ccd_cdf_table_build(uint32_t *d_cdf, const float *d_scale, cudaStream_t st) {
@@ -2045,14 +2050,9 @@ int ccd_laplace_domain(const float *d_scale, int sc_lo, int sc_hi, uint32_t *d_l
 }
 
 int ccd_rate_kind(int n_ctx, int cf, bool fast) {
-    if (fast) {
-        if (n_ctx == 6 && cf == 2) return 0;
-        if (n_ctx == 10 && cf == 2) return 1;
-        if (n_ctx == 10 && cf == 4) return 2;
-        if (n_ctx == 14 && cf == 6) return 3;
-        if (n_ctx == 20 && cf == 6) return 4;
-    }
-    return 5;
+    for (int k = 0; fast && k < kGenericKind; k++)
+        if (kArmShapes[k][0] == n_ctx && kArmShapes[k][1] == cf) return k;
+    return kGenericKind;
 }
 
 size_t ccd_rate_smem_bytes(int arm_blob_bytes, int ifce_blob_max) {

@@ -139,6 +139,7 @@ struct RateSpatialDev {
     float sy[CCD_MAX_GRIDS], sx[CCD_MAX_GRIDS];  // nearest-resize scales h / H, w / W (fp32)
 };
 
+// The kind k_entropy and k_latent_rate dispatch on: the shape's index among the fast shapes when fast, else generic
 int ccd_rate_kind(int n_ctx, int cf, bool fast);
 size_t ccd_rate_smem_bytes(int arm_blob_bytes, int ifce_blob_max);
 int ccd_rate_launch(const RateTile *d_tiles, int n_tiles, const RateJobDev *d_jobs, size_t smem, const uint32_t *d_cdf,

@@ -24,10 +24,12 @@ def _copies(fn):
 
 @pytest.mark.gpu
 def test_one_copy_each_way_per_call(ctx, kodim14):
+    import numpy as np
     import torch
 
     from coolchic_b200 import _native
     from coolchic_b200.io.framedata import FrameData
+    from test_optimize import _draw
 
     dev = ctx.torch_device
     n = 132
@@ -37,6 +39,10 @@ def test_one_copy_each_way_per_call(ctx, kodim14):
     _, lats = ctx.decode_many([d] * n, [nb] * n, [lb] * n, want_latents=True)
     nn = _native.decode_nn(d, nb)
     assert _copies(lambda: ctx.latent_rate([d] * n, [nn] * n, lats, want_spatial=True)) == (1, 1)
+    mu_sc = [r["mu_sc"] for r in ctx.latent_rate([d] * n, [nn] * n, lats, want_mu_sc=True)]
+    assert _copies(lambda: ctx.rate_sweep([d] * n, lats, mu_sc, list(range(-16, 16)))) == (1, 1)
+    cands = _draw(d, np.random.default_rng(0), _native.CCD_CAND_MAX)
+    assert _copies(lambda: ctx.rate_candidates(d, nn, lats[0], cands)) == (1, 1)
 
     # 32 frames of 1080p 4:2:0, the size of the frames of bench.py's gop32_1080p_yuv420 workload
     h, w = 1080, 1920
